@@ -6,6 +6,7 @@
     python bench.py --config sintel ...                           # configs[2]: 448x1024 (436x1024 padded), iters_pred=24
     python bench.py --config train ...                            # configs[3]: training step 384x512, iters=12
     python bench.py --impl reference --steps K --warmup W         # the reference algorithm on the host CPU cores
+    python bench.py ... --dump-outputs DIR                        # also write the last timed step's outputs as DIR/<name>.npy
 
 N > 1 is launched by torchrun (one rank per GPU): the batch axis shards (weak scaling: 4 pairs per GPU); inference has
 no data-path collective, the training step all-reduces one flat gradient buffer (NCCL) and the context encoder's
@@ -38,15 +39,10 @@ CONFIGS = {
                            'AdamW + one-cycle LR + global-norm clip, NCCL gradient all-reduce (BASELINE.json configs[3])'),
 }
 METRIC = 'frame-pairs/sec at 448\u00d7512 iters=12; final-flow max-abs vs ref'        # BASELINE.json's string, verbatim (\u00d7 = multiplication sign)
-N_ROTATE = 12            # distinct input batches cycled through: 12 x 2 x 11 MB = 264 MB > 126 MB L2
+N_ROTATE = 12            # distinct input batches cycled through: 12 x 2 x 11 MB = 264 MB > 50 MB L2
 
 # Algorithmic work of BasicUpdateBlock per feature-grid pixel (update.py:128-153, SURVEY.md section 8(d))
 UPDATE_MAC_PER_PX = 3_118_336
-# Tensor-core layers of one BasicUpdateBlock application without the mask head (update.py:143-153): (output columns N of the
-# tile, 64-channel K chunks incl. taps) -- convc1, convf1, convc2, convf2, conv, z|r x2, q x2, flow_head.conv1, flow_head.conv2
-# (N = 32: the CTA pair's minimum).  Used for the shared-memory traffic of update_mega_kernel (DESIGN.md 3.2).
-UPDATE_LAYERS_N_CHUNKS = ((256, 6), (128, 2), (192, 36), (64, 18), (128, 36), (256, 30), (256, 30), (128, 30), (128, 30),
-                          (256, 18), (32, 36))
 MASK_MAC_PER_PX = 294_912 + 147_456               # mask[0] 3x3 128->256 + mask[2] 1x1 256->576 (update.py:137-141): only
                                                   # executed on iterations whose prediction is upsampled
 
@@ -69,17 +65,17 @@ def load_peaks():
         d = json.load(open(path))
         return dict(hbm_gbs=float(d['hbm_gbs']), bf16_tflops=float(d.get('bf16_tflops_sustained', d['bf16_tflops'])),
                     bf16_tflops_burst=float(d['bf16_tflops']), source='measured (MEASURED_PEAKS.json)')
-    except Exception:
-        return dict(hbm_gbs=6650.0, bf16_tflops=1400.0, bf16_tflops_burst=1590.0, source='fallback (B200_PROFILING.md)')
+    except Exception:   # NVIDIA's H100 SXM data sheet (700 W card, dense): a bound, not a rate any kernel reaches
+        return dict(hbm_gbs=3350.0, bf16_tflops=989.0, bf16_tflops_burst=989.0, source='H100 SXM data sheet')
 
 
-def load_traffic():
-    """DRAM bytes per launch of the profiled kernels, extracted from the committed `ncu --set full` captures by
-    scripts/ncu_traffic.py (profiles/r02_traffic.json); None when the file is absent."""
-    try:
-        return json.load(open(os.path.join(ROOT, 'profiles', 'r02_traffic.json')))
-    except Exception:
-        return None
+def dump_outputs(dirname, arrays):
+    """--dump-outputs: write {name: array} as dirname/<name>.npy (float32 / float64) for output-by-output comparison of builds."""
+    import numpy as np
+    os.makedirs(dirname, exist_ok=True)
+    for name, a in arrays.items():
+        a = np.asarray(a)
+        np.save(os.path.join(dirname, name + '.npy'), a.astype(np.float64 if a.dtype == np.float64 else np.float32))
 
 
 class ClockSampler:
@@ -174,7 +170,9 @@ def run_reference(args, cfg):
         pps, sec, cores = oracle_train_time(cfg, 1, args.steps, args.warmup)
         what = 'training step (forward + autograd backward + clip + AdamW)'
     else:
-        pps, sec, cores, _ = oracle_forward_time(cfg, 1, args.steps, args.warmup)
+        pps, sec, cores, flow = oracle_forward_time(cfg, 1, args.steps, args.warmup)
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, {'final_flow': flow.numpy()})
         what = 'forward'
     sample = (f'1 pair per step ({cfg["H"]}x{cfg["W"]}, {cfg["iters"]} iterations, {what}), {args.steps} steps after '
               f'{args.warmup} warm-up')
@@ -247,9 +245,12 @@ def run_ours(args, cfg):
     if train:
         return run_train(args, cfg, model, host, dev_in, timed, barrier, rank, world, local, device)
 
+    last = {}
+
     def step_resident(i):
         a, b = dev_in[i % n_rot]
-        return model([a, b], training=False, last_only=True)[-1]
+        last['flow'] = model([a, b], training=False, last_only=True)[-1]
+        return last['flow']
 
     def step_e2e(i):
         a, b = host[i % n_rot]
@@ -274,6 +275,9 @@ def run_ours(args, cfg):
     clocks = sampler.stop() if sampler else None
     launches = launches_per_step * args.steps
     value = world * B * args.steps / dev_s
+    if args.dump_outputs and rank == 0:
+        # final flow (B, H, W, 2) of the last timed step: input batch (steps - 1) % N_ROTATE, seeded by its index
+        dump_outputs(args.dump_outputs, {'final_flow': last['flow'].float().cpu().numpy()})
 
     log(f'resident: {value:.1f} pairs/s; timing end-to-end steps')
     for i in range(min(args.warmup, 2)):
@@ -292,8 +296,8 @@ def run_ours(args, cfg):
             barrier()
             return parallel.max_over_ranks(wall, device)
         run_pipelined(2)
-        # wall-clock leg of K steps: host jitter of a shared box moves it by tens of percent from one run to the next
-        # (profiles/README.md), so it is run twice and the faster run is reported; both are kept in `e2e.runs_pairs_per_s`
+        # wall-clock leg of K steps: host jitter of a shared machine moves it by tens of percent from one run to the next,
+        # so it is run twice and the faster run is reported; both are kept in `e2e.runs_pairs_per_s`
         e2e_walls = [run_pipelined(args.steps), run_pipelined(args.steps)]
         e2e_wall = min(e2e_walls)
     else:
@@ -306,7 +310,6 @@ def run_ours(args, cfg):
     line = None
     if rank == 0:
         peaks = load_peaks()
-        traffic = load_traffic() or {}
         log(f'e2e: {e2e_value:.1f} pairs/s; kernel-level timings')
         # --- kernel-level timing for the roofline objects (rank 0, CUDA events on the launching stream) ---
         a, b = dev_in[0]
@@ -392,19 +395,18 @@ def run_ours(args, cfg):
             # --- CPU baseline: the restated reference on the host cores, bounded sample ---
             cpu_pps, cpu_sec, cores, _ = oracle_forward_time(cfg, 1, 3, 1)
 
-        mega_traffic = traffic.get('update_mega_kernel')
         line = {
             'metric': METRIC, 'value': value, 'unit': 'pairs/s', 'n_gpus': world, 'steps': args.steps,
             'warmup': args.warmup, 'ms_per_step': dev_s / args.steps * 1e3, 'higher_is_better': True,
             'scaling': 'weak', 'vs_baseline': None, 'dtype': 'f32', 'data': 'synthetic',
             'config': {'workload': cfg['workload'], 'name': args.config, 'global_batch': world * B, 'parallelism': f'dp{world}',
-                       'arithmetic': {'f16x2': 'tcgen05 fp16 hi/lo split, 3 passes, fp32 accumulate (fp32-grade)',
+                       'arithmetic': {'f16x2': 'wgmma fp16 hi/lo split, 3 passes, fp32 accumulate (fp32-grade)',
                                       'fp32': 'CUDA-core FFMA'}[precision],
-                       'encoders': {'f16x2': 'native: the same tcgen05 implicit-GEMM kernel (stride-2 TMA boxes, fused norm affine)',
+                       'encoders': {'f16x2': 'native: the same wgmma implicit-GEMM kernel (stride-2 TMA boxes, fused norm affine)',
                                     'fp32': 'cuDNN IEEE fp32 via PyTorch'}[precision],
                        'cuda_graph': not args.no_graph, 'last_only': True,
                        'l2': f'inputs rotate over {n_rot} distinct batches ({n_rot * 2 * B * H * W * 12 / 1e6:.0f} MB) and every step '
-                             f'rewrites the {B * corr_bytes_pair / 1e6:.0f} MB correlation pyramid: working set > 126 MB L2'},
+                             f'rewrites the {B * corr_bytes_pair / 1e6:.0f} MB correlation pyramid: working set > 50 MB L2'},
             'final_flow_max_abs_vs_oracle': max_abs,
             'parity': parity,
             'e2e': {'value': e2e_value, 'unit': 'pairs/s', 'h2d_bytes_per_step': h2d, 'd2h_bytes_per_step': d2h,
@@ -419,30 +421,17 @@ def run_ours(args, cfg):
                                    'iteration)',
                          'achieved': ach_tflops, 'peak': peaks['bf16_tflops'], 'unit': 'TFLOP/s',
                          'frac': ach_tflops / peaks['bf16_tflops'],
-                         'traffic': mega_traffic,
                          'algorithmic_flops_per_launch': flops_per_launch, 'ms_per_launch': t_update * 1e3,
                          'peak_source': peaks['source'] + ' (sustained cuBLAS bf16: the kernel runs inside a long step)',
                          'note': 'achieved = algorithmic fp32 FLOPs one launch executes (2*2,675,968 MAC/px; + 2*442,368 MAC/px of '
                                  'mask head on the one upsampled iteration, averaged over the launches) / CUDA-event time per '
                                  'launch measured inside raft_b200_forward_loop; the kernel executes 3 fp16 MMA passes per '
                                  'FLOP, so the tensor pipe is 3x busier than `frac`',
-                         'executed_frac': 3 * ach_tflops / peaks['bf16_tflops'],
-                         # what the mainloop is measured to sit on (profiles/README.md): per 64-channel chunk a CTA of a pair
-                         # receives 32 KB of activations + N/2 weight rows by TMA and its twelve MMAs read 12 x (4 KB + N x 32 B)
-                         'shared_memory': (lambda by, pk: {
-                             'bytes_per_launch': by, 'achieved_TBps': by / max(t_update, 1e-9) / 1e12, 'peak_TBps': pk / 1e12,
-                             'frac': by / max(t_update, 1e-9) / pk,
-                             'note': 'TMA writes + tcgen05 operand reads of shared memory per launch (mask head excluded) against '
-                                     f'148 SMs x 128 B/clk at the sampled SM clock; a layer has {B * PX // 128} tiles for 148 SMs and '
-                                     'the 9 chain layers run one after the other (at 112 tiles: 0.76 of this peak at most)'})(
-                             B * PX / 128 * sum(c * (32768 + (n // 2) * 256 + 12 * (4096 + n * 32)) for n, c in UPDATE_LAYERS_N_CHUNKS),
-                             148 * 128 * 1e6 * float((clocks or {}).get('sm_mhz') or 1965))},
+                         'executed_frac': 3 * ach_tflops / peaks['bf16_tflops']},
             'roofline_corr_lookup': {'bound': 'hbm', 'kernel': f'correlation pyramid build + {ITERS} lookups',
                                      'achieved': ach_gbs, 'peak': peaks['hbm_gbs'], 'unit': 'GB/s',
                                      'frac': ach_gbs / peaks['hbm_gbs'],
-                                     'traffic': {'lookup': traffic.get('corr_lookup_win_kernel'),
-                                                 'correlation': traffic.get('corr_tc_kernel'),
-                                                 'lookup_algorithmic_bytes': lookup_bytes,
+                                     'traffic': {'lookup_algorithmic_bytes': lookup_bytes,
                                                  'lookup_launch_im2col_rider_bytes': rider_bytes,
                                                  'correlation_algorithmic_bytes': B * corr_bytes_pair},
                                      'ms': {'pyramid_build': t_corr * 1e3, 'lookup': t_lookup * 1e3},
@@ -485,6 +474,7 @@ def run_train(args, cfg, model, host, dev_in, timed, barrier, rank, world, local
         a, b = dev_in[i % n_rot]
         out = model.train_step((a, b, dev_fl[i % n_rot], dev_va))
         losses.append(out['loss'])
+        return out
 
     def step_e2e(i):
         a, b = host[i % n_rot]
@@ -506,6 +496,8 @@ def run_train(args, cfg, model, host, dev_in, timed, barrier, rank, world, local
     dev_s, _ = timed(step_resident, args.steps)
     clocks = sampler.stop() if sampler else None
     value = world * B * args.steps / dev_s
+    if args.dump_outputs and rank == 0:         # the loss of the last timed step (its parameter update stays on the device)
+        dump_outputs(args.dump_outputs, {'loss': np.asarray([float(losses[-1])], dtype=np.float64)})
     log(f'resident: {value:.2f} pairs/s; end-to-end steps')
     _, e2e_wall = timed(step_e2e, args.steps)
     e2e_value = world * B * args.steps / e2e_wall
@@ -538,8 +530,8 @@ def run_train(args, cfg, model, host, dev_in, timed, barrier, rank, world, local
                        'collectives': 'one flat fp32 gradient all-reduce per step (NCCL) + all-reduced BatchNorm statistics of the '
                                       'context encoder (forward and backward)',
                        'gradient_bytes': int(tr.flat.g.numel() * 4), 'allreduce_ms': ar_ms,
-                       'arithmetic': 'correlation forward: tcgen05 fp16 hi/lo; lookup forward/backward, clip + AdamW: hand-written '
-                                     'CUDA; convolutions / norms / gates forward and backward: IEEE-fp32 cuDNN via torch.autograd'},
+                       'arithmetic': 'correlation forward: wgmma fp16 hi/lo; lookup forward/backward, clip + AdamW: hand-written '
+                                     'CUDA; convolutions / norms / gates forward and backward: IEEE-fp32 PyTorch CUDA kernels via torch.autograd (cuDNN off)'},
             'loss_first_last': [losses[0], losses[-1]],
             'e2e': {'value': e2e_value, 'unit': 'pairs/s', 'h2d_bytes_per_step': 2 * B * H * W * 3 * 4 + B * H * W * 2 * 4,
                     'd2h_bytes_per_step': 4, 'api': 'RAFT.train_step (images and ground-truth flow uploaded every step, loss read back)'},
@@ -566,6 +558,8 @@ def main():
                     help='end-to-end leg as one synchronous predict_step per step instead of parallel.predict_stream')
     ap.add_argument('--quick', action='store_true', help='timing only: skip the parity and CPU-baseline legs (A/B runs)')
     ap.add_argument('--precision', default=os.environ.get('RAFT_B200_PRECISION', 'f16x2'), choices=['f16x2', 'fp32'])
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='after the timed steps, write the outputs of the last one as DIR/<name>.npy')
     args = ap.parse_args()
     cfg = CONFIGS[args.config]
     # stdout must carry exactly one JSON line: libraries (NCCL prints its version banner there) get stderr instead

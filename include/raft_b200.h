@@ -1,4 +1,4 @@
-/* raft_b200.h -- C ABI of the B200-native RAFT forward/update hot path.
+/* raft_b200.h -- C ABI of the H100-native (sm_90a) RAFT forward/update hot path.
  *
  * Drop-in boundary for daigo0927/tf-raft (reference @ 3c85f54).  The reference has no FFI of
  * its own: its boundary is the Python object API of tf_raft/layers/corr.py, tf_raft/layers/update.py
@@ -17,7 +17,7 @@
  *   - return value: 0 = ok, < 0 = raft_status (argument / shape / workspace error, detected on
  *     the host before anything is launched), > 0 = cudaError_t of a failed launch;
  *   - re-entrant across host threads as long as streams and buffers differ;
- *   - there is NO CPU path: without an sm_100 device every compute entry point returns
+ *   - there is NO CPU path: without an sm_90 device every compute entry point returns
  *     RAFT_ERR_NO_DEVICE or the CUDA error.
  */
 #ifndef RAFT_B200_H_
@@ -46,9 +46,9 @@ typedef enum raft_status {
 /* Arithmetic of the contraction kernels (correlation GEMM and update-block convolutions).
  * Both are fp32-grade: the final-flow parity gate (<= 1e-3 max-abs) holds for either.
  *   FP32   CUDA-core FFMA, fp32 operands, fp32 accumulate.
- *   F16X2  tcgen05 tensor cores: every fp32 operand v is split into fp16 (hi, lo) with
+ *   F16X2  wgmma tensor cores: every fp32 operand v is split into fp16 (hi, lo) with
  *          v ~= hi + lo (22-bit significand), the product is hi*hi + lo*hi + hi*lo
- *          with fp32 accumulation in TMEM (DESIGN.md "Precision").                          */
+ *          with fp32 accumulation (DESIGN.md "Precision").                                  */
 typedef enum raft_precision { RAFT_PREC_FP32 = 0, RAFT_PREC_F16X2 = 1 } raft_precision;
 
 /* model.py:10-30 (RAFT, BasicUpdateBlock) / model.py:173-188 (SmallRAFT, SmallUpdateBlock). */
@@ -254,8 +254,9 @@ void raft_b200_launch_count_reset(void);
  * of every iteration; _read waits for the last one and returns the summed durations of the most recent call.      */
 void raft_b200_profile_loop(int enable);
 int raft_b200_profile_read(float* lookup_ms, float* update_ms, int* iterations);
-/* Profiling aid: the next update-block launches of tensor-core layer `tc_layer` (-1 = off; 2000 = the correlation kernel) write clock64 stamps of
- * CTA 0 into `device_buf_2048` (4 x 512 int64: slot free / data landed / group retired / group drained).        */
+/* Profiling aid: the next per-layer launches (conv_tc_kernel: RAFT_B200_MEGA=0, or the k-th encoder convolution with
+ * tc_layer = 1000 + k) of tensor-core layer `tc_layer` (-1 = off) write clock64 stamps of CTA 0 into `device_buf_2048`
+ * ([0, 512): tile started, [512, 1024): tile's epilogue done, one entry per tile of the CTA).                        */
 void raft_b200_debug_timeline(int tc_layer, long long* device_buf_2048);
 
 #ifdef __cplusplus

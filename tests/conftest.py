@@ -10,7 +10,7 @@ for p in (ROOT, os.path.dirname(os.path.abspath(__file__))):
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a B200 (sm_100a) GPU; run with -m gpu on the GPU box')
+    config.addinivalue_line('markers', 'gpu: needs an H100 (sm_90a) GPU; run with -m gpu on a GPU machine')
 
 
 def pytest_collection_modifyitems(config, items):

@@ -163,7 +163,7 @@ def test_train_step_vs_oracle_autograd(variant, shape, iters):
     tr = model._trainer
     gnorm = math.sqrt(float((tr.flat.g.double() ** 2).sum()))
     assert gnorm == pytest.approx(norm_o, rel=1e-3), (gnorm, norm_o)
-    # Per variable and globally.  The two sides differ in arithmetic (tcgen05 fp16 hi/lo correlation and cuDNN convolutions vs
+    # Per variable and globally.  The two sides differ in arithmetic (tensor-core fp16 hi/lo correlation and PyTorch CUDA convolutions vs
     # CPU fp32, atomics in the lookup scatter) and the loss is only piecewise smooth in the coordinates (floor / ceil sampler),
     # so individual entries agree to a fraction of a percent of the tensor's scale, the whole gradient to 1e-2 in norm.
     num = den = 0.0

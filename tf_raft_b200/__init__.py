@@ -1,4 +1,4 @@
-"""tf_raft_b200 -- B200-native (sm_100a) RAFT forward/update hot path behind the Python API of
+"""tf_raft_b200 -- H100-native (sm_90a) RAFT forward/update hot path behind the Python API of
 daigo0927/tf-raft: `CorrBlock`, `BasicUpdateBlock` / `SmallUpdateBlock`, `RAFT` / `SmallRAFT`.
 
 Compute lives in libraft_b200.so (hand-written CUDA, C ABI in include/raft_b200.h); PyTorch supplies

@@ -10,7 +10,7 @@ import os
 import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# RAFT_B200_LIB: load another build of the same sources (kernel experiments, tools/epi_exp.sh); the default is the in-tree build.
+# RAFT_B200_LIB: load another build of the same sources (kernel experiments); the default is the in-tree build.
 LIB_PATH = os.environ.get('RAFT_B200_LIB') or os.path.join(_HERE, 'libraft_b200.so')
 
 PREC_FP32 = 0
@@ -23,7 +23,7 @@ _PRECISIONS = {'fp32': PREC_FP32, 'f16x2': PREC_F16X2, PREC_FP32: PREC_FP32, PRE
 
 
 def resolve_precision(precision=None):
-    """None -> $RAFT_B200_PRECISION or 'f16x2' (the tcgen05 path)."""
+    """None -> $RAFT_B200_PRECISION or 'f16x2' (the tensor-core path)."""
     if precision is None:
         precision = os.environ.get('RAFT_B200_PRECISION', 'f16x2')
     try:
@@ -104,7 +104,7 @@ def lib():
     if _lib is None:
         if not os.path.exists(LIB_PATH):
             raise ImportError(
-                f'{LIB_PATH} is missing: the sm_100a CUDA library has not been built. '
+                f'{LIB_PATH} is missing: the sm_90a CUDA library has not been built. '
                 'Run `python -c "import __graft_entry__ as g; g.build()"` (or `python -m tf_raft_b200.build`) '
                 'from the repository root. There is no CPU / PyTorch fallback for the RAFT hot path.')
         handle = ctypes.CDLL(LIB_PATH)
@@ -145,7 +145,7 @@ def require_cuda(*tensors):
         if t is None:
             continue
         if not t.is_cuda:
-            raise RuntimeError('tf_raft_b200 runs on CUDA tensors only (sm_100a); got a CPU tensor. '
+            raise RuntimeError('tf_raft_b200 runs on CUDA tensors only (sm_90a); got a CPU tensor. '
                                'There is no CPU fallback for this path.')
         if t.dtype != torch.float32 or not t.is_contiguous():
             raise RuntimeError('expected contiguous float32 tensors')
@@ -154,7 +154,7 @@ def require_cuda(*tensors):
 def f32c(t):
     """contiguous float32 view/copy of a CUDA tensor."""
     if not t.is_cuda:
-        raise RuntimeError('tf_raft_b200 runs on CUDA tensors only (sm_100a); got a CPU tensor. '
+        raise RuntimeError('tf_raft_b200 runs on CUDA tensors only (sm_90a); got a CPU tensor. '
                            'There is no CPU fallback for this path.')
     return t.to(torch.float32).contiguous()
 

@@ -82,7 +82,7 @@ static int corr_build_fp32(const float* f1, const float* f2, int B, int h, int w
 
 // Tensor-core path: level l = fmap1 . avgpool^l(fmap2)^T / sqrt(C).  Pooling is linear, so pooling
 // the 256-channel features (a few MB) before the GEMM equals pooling the N x N volume after it
-// (up to fp32 summation order) and every level is written exactly once, straight from TMEM.
+// (up to fp32 summation order) and every level is written exactly once, straight from the accumulator registers.
 // Two launches: corr_prep_kernel (pool + hi/lo split of both feature maps) and corr_tc_kernel (all levels).
 static int corr_build_tc(const float* f1, const float* f2, int B, int h, int w, int C, int levels, float* const pyr[],
                          void* ws, cudaStream_t st) {
@@ -148,16 +148,15 @@ static int corr_build_tc(const float* f1, const float* f2, int B, int h, int w, 
     const float m = frexpf(p.corr_div, &e);          // sqrt(C) = m * 2^e; m == 0.5 <=> exact power of two
     p.corr_mul = (m == 0.5f && p.corr_div * p.corr_div == (float)C) ? 1.0f / p.corr_div : 0.0f;
   }
-  if (g_dbg_layer == 2000) p.dbg = g_dbg_buf;
   int dev = 0;
   RAFT_CUDA_TRY(cudaGetDevice(&dev));
-  static unsigned long long attr_mask = 0;          // per-device attribute (benign race: idempotent)
-  if (!(attr_mask & (1ull << (dev & 63)))) {
+  static int num_sms[64] = {0};                     // per-device attribute and SM count (benign race: idempotent)
+  if (!num_sms[dev & 63]) {
     RAFT_CUDA_TRY(cudaFuncSetAttribute(corr_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kCorrSmemBytes));
-    attr_mask |= 1ull << (dev & 63);
+    RAFT_CUDA_TRY(cudaDeviceGetAttribute(&num_sms[dev & 63], cudaDevAttrMultiProcessorCount, dev));
   }
   const int ntiles = p.tile0[levels];
-  corr_tc_kernel<<<ntiles < kNumSMs ? ntiles : kNumSMs, kCorrThreads, kCorrSmemBytes, st>>>(p);
+  corr_tc_kernel<<<ntiles < num_sms[dev & 63] ? ntiles : num_sms[dev & 63], kTcThreads, kCorrSmemBytes, st>>>(p);
   RAFT_COUNT_LAUNCH();
   return raft_launch_status();
 }
@@ -417,20 +416,9 @@ static bool mega_enabled() {
   static const int v = [] { const char* e = getenv("RAFT_B200_MEGA"); return e ? atoi(e) : 1; }();
   return v != 0;
 }
-// CTA pairs (update_mega_kernel<true>) whenever the number of pixel tiles is even; RAFT_B200_PAIR=0 keeps single CTAs (A/B).
-static bool pair_enabled() {
-  static const int v = [] { const char* e = getenv("RAFT_B200_PAIR"); return e ? atoi(e) : 1; }();
-  return v != 0;
-}
 static int update_block_tc(UpdateCtx& c, float* h, float* delta, float* mask, float* adv_coords) {
   MegaPlan plan;
   c.plan = mega_enabled() ? &plan : nullptr;
-  {
-    int tw, th;
-    tc_pick_tile(c.w, c.h, &tw, &th);
-    const int mtiles = c.B * ceil_div(c.h, th) * ceil_div(c.w, tw);
-    plan.pair = pair_enabled() && (mtiles % 2 == 0) ? 1 : 0;
-  }
   const int st = update_core_tc(c, h, delta, mask, adv_coords);
   c.plan = nullptr;
   RAFT_TRY(st);
@@ -508,7 +496,7 @@ const char* raft_b200_strerror(int status) {
     case RAFT_ERR_BAD_ARG: return "bad argument (null pointer or unknown enum)";
     case RAFT_ERR_BAD_SHAPE: return "bad shape";
     case RAFT_ERR_WORKSPACE: return "workspace or prepared-weights buffer too small";
-    case RAFT_ERR_NO_DEVICE: return "no sm_100 CUDA device";
+    case RAFT_ERR_NO_DEVICE: return "no sm_90 CUDA device";
     case RAFT_ERR_DRIVER: return "cuTensorMapEncodeTiled unavailable or failed";
     case RAFT_ERR_UNSUPPORTED: return "unsupported configuration";
     default: return status > 0 ? cudaGetErrorString((cudaError_t)status) : "unknown raft_status";
@@ -523,9 +511,11 @@ int raft_b200_device_ok(int device) {
     (void)cudaGetLastError();
     return RAFT_ERR_NO_DEVICE;
   }
-  int major = 0;
-  if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device) != cudaSuccess) return RAFT_ERR_NO_DEVICE;
-  return major == 10 ? RAFT_OK : RAFT_ERR_NO_DEVICE;
+  int major = 0, minor = 0;
+  if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device) != cudaSuccess ||
+      cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, device) != cudaSuccess)
+    return RAFT_ERR_NO_DEVICE;
+  return major == 9 && minor == 0 ? RAFT_OK : RAFT_ERR_NO_DEVICE;       // the library holds sm_90a code only
 }
 
 void raft_b200_profile_loop(int enable) { g_prof.on = enable != 0; g_prof.n = 0; }

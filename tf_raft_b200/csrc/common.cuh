@@ -1,10 +1,12 @@
-// Shared device/host helpers for the sm_100a RAFT hot path: status codes, PTX wrappers for
-// mbarrier / TMA / tcgen05 / TMEM, fp16 hi-lo splitting.  No torch types anywhere.
+// Shared device/host helpers for the sm_90a RAFT hot path: status codes, PTX wrappers for
+// mbarrier / TMA / wgmma, fp16 hi-lo splitting.  No torch types anywhere.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include <type_traits>
 
 #include "../../include/raft_b200.h"
 
@@ -27,7 +29,7 @@ static inline int raft_launch_status() {
 
 namespace raft {
 
-constexpr int kNumSMs = 148;
+constexpr int kNumSMs = 132;         // H100 SXM; persistent kernels size their grids from the device attribute
 
 __host__ __device__ constexpr int ceil_div(int a, int b) { return (a + b - 1) / b; }
 __host__ __device__ constexpr int round_up(int a, int b) { return ceil_div(a, b) * b; }
@@ -38,13 +40,8 @@ __host__ __device__ constexpr int round_up(int a, int b) { return ceil_div(a, b)
 // ------------------------------------------------------------------------------------------
 __device__ __forceinline__ void split_f16(float v, __half& hi, __half& lo) {
   v = fminf(fmaxf(v, -65504.f), 65504.f);            // saturate instead of inf -> NaN downstream
-#if defined(RAFT_EPI_EXP) && (RAFT_EPI_EXP & 8)
-  hi = __ushort_as_half((unsigned short)(__float_as_uint(v) >> 16));      // experiment: no conversions
-  lo = __ushort_as_half((unsigned short)__float_as_uint(v));
-#else
   hi = __float2half_rn(v);
   lo = __float2half_rn(v - __half2float(hi));
-#endif
 }
 
 // Two values at once: the packed conversion (cvt.rn.f16x2.f32 -> F2FP.F16.F32.PACK_AB, ALU pipe) instead of two scalar F2F
@@ -52,16 +49,11 @@ __device__ __forceinline__ void split_f16(float v, __half& hi, __half& lo) {
 __device__ __forceinline__ void split_f16x2(float a, float b, uint32_t& hi2, uint32_t& lo2) {
   a = fminf(fmaxf(a, -65504.f), 65504.f);
   b = fminf(fmaxf(b, -65504.f), 65504.f);
-#if defined(RAFT_EPI_EXP) && (RAFT_EPI_EXP & 8)
-  hi2 = __float_as_uint(a) ^ (__float_as_uint(b) << 16);
-  lo2 = __float_as_uint(b) ^ (__float_as_uint(a) << 16);
-#else
   const __half2 h = __floats2half2_rn(a, b);
   const float2 hf = __half22float2(h);
   const __half2 l = __floats2half2_rn(a - hf.x, b - hf.y);
   hi2 = *reinterpret_cast<const uint32_t*>(&h);
   lo2 = *reinterpret_cast<const uint32_t*>(&l);
-#endif
 }
 
 __device__ __forceinline__ uint32_t pack_h2(__half a, __half b) {
@@ -72,7 +64,7 @@ __device__ __forceinline__ float sigmoidf_acc(float x) { return 1.0f / (1.0f + e
 
 #if defined(__CUDA_ARCH__)
 // ------------------------------------------------------------------------------------------
-// PTX wrappers (sm_100a)
+// PTX wrappers (sm_90a)
 // ------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
@@ -159,241 +151,102 @@ __device__ __forceinline__ void tma_load_5d(void* dst, const CUtensorMap* m, uin
       : "memory");
 }
 
-// --- tcgen05 / TMEM -----------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_holder, uint32_t ncols) {   // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_holder)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {        // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem], fp16 operands, fp32 accumulate; issued by ONE thread.
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                         uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// mbarrier arrives once every previously issued tcgen05.mma of this thread has completed
-// (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// --- CTA pairs (cta_group::2): two CTAs of a cluster share one M = 256 MMA -------------------------------------------
-// Each CTA stages its own 128 rows of A and its own HALF of the N rows of B; the leader (cluster rank 0) issues the MMAs for
-// both; each CTA's TMEM receives its 128 rows x N columns.  TMA loads of both CTAs signal the LEADER's mbarrier, commits are
-// multicast to the barriers of both CTAs (same shared-memory offset in each).  Mechanics checked by tools/pair_probe.cu.
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ uint32_t mapa_u32(uint32_t cta_addr, uint32_t rank) {   // shared::cta address -> shared::cluster of `rank`
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(cta_addr), "r"(rank));
-  return r;
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// wait that also acquires what ANOTHER CTA of the cluster released (remote arrive after st.shared::cluster)
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {
-  const long long t0 = clock64();
-  for (;;) {
-    uint32_t ok;
+// --- wgmma (sm_90a warpgroup MMA) ------------------------------------------------------------------------------------
+// D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, fp16 operands from shared memory, fp32 accumulators in the registers of the
+// four warps of a warpgroup.  Thread t of the warpgroup (warp w = t / 32, lane l) holds, for i in [0, N / 8),
+//   d[4i + 0, 1] = row 16w + l/4,     columns 8i + 2(l%4) + {0, 1}
+//   d[4i + 2, 3] = row 16w + l/4 + 8, the same columns.
+// scale_d == 0 starts a new accumulation (D = A * B).
+template <int N> struct Wgmma;
+template <> struct Wgmma<16> {
+  __device__ __forceinline__ static void mma(float (&d)[8], uint64_t a, uint64_t b, uint32_t scale_d) {
     asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n"
-        "selp.u32 %0, 1, 0, p;\n"
-        "}\n"
-        : "=r"(ok)
-        : "r"(smem_u32(bar)), "r"(parity)
-        : "memory");
-    if (ok) return;
-    if (clock64() - t0 > 8000000000LL) __trap();
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %10, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(a), "l"(b), "r"(scale_d));
   }
+};
+template <> struct Wgmma<32> {
+  __device__ __forceinline__ static void mma(float (&d)[16], uint64_t a, uint64_t b, uint32_t scale_d) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(a), "l"(b), "r"(scale_d));
+  }
+};
+template <> struct Wgmma<64> {
+  __device__ __forceinline__ static void mma(float (&d)[32], uint64_t a, uint64_t b, uint32_t scale_d) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(a), "l"(b), "r"(scale_d));
+  }
+};
+template <> struct Wgmma<96> {
+  __device__ __forceinline__ static void mma(float (&d)[48], uint64_t a, uint64_t b, uint32_t scale_d) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %50, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n96k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, %48, %49, p, 1, 1, 0, 0;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
+        : "l"(a), "l"(b), "r"(scale_d));
+  }
+};
+template <> struct Wgmma<128> {
+  __device__ __forceinline__ static void mma(float (&d)[64], uint64_t a, uint64_t b, uint32_t scale_d) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(a), "l"(b), "r"(scale_d));
+  }
+};
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// Orders the compiler's view of the accumulator registers around the asynchronous MMAs.
+template <int R>
+__device__ __forceinline__ void wgmma_fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void st_cluster_u32(uint32_t cluster_addr, uint32_t v) {
-  asm volatile("st.shared::cluster.u32 [%0], %1;" ::"r"(cluster_addr), "r"(v) : "memory");
-}
-__device__ __forceinline__ void tma2_load_4d(void* dst, const CUtensorMap* m, uint32_t leader_bar, int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, "
-      "%6}], [%2];" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(leader_bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void tma2_load_5d(void* dst, const CUtensorMap* m, uint32_t leader_bar, int c0, int c1, int c2, int c3,
-                                             int c4) {
-  asm volatile(
-      "cp.async.bulk.tensor.5d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, "
-      "%6, %7}], [%2];" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(leader_bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
-      : "memory");
-}
-__device__ __forceinline__ void tmem2_alloc(uint32_t* smem_holder, uint32_t ncols) {   // one warp of EACH CTA of the pair
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_holder)), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem2_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem2_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma2_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrives on the barrier at this shared-memory offset in BOTH CTAs of the pair once the issued MMAs have completed
-__device__ __forceinline__ void umma2_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                   smem_u32(bar)),
-               "h"((uint16_t)3)
-               : "memory");
-}
+
 // --- one 64-channel chunk of the three-pass product hi*hi + hi*lo + lo*hi ------------------------------------------------
-// The mainloops are bound by shared-memory bandwidth (DESIGN.md 3.2) and every MMA re-reads its A slice (4 KB) from shared
-// memory.  The tensor core has an A COLLECTOR buffer: `.collector::a::fill` keeps the slice, `.collector::a::lastuse` on the
-// next MMA reuses it without a shared-memory read (SASS: UTCHMMA ... .A_KEEP / .A_REUSE; measured, tools/mma_probe.cu: an
-// N = 64 MMA stream goes from 48 to 40 cycles per MMA, its issue floor).  So per K=16 slice hi*hi (fill) is followed directly
-// by hi*lo (lastuse), and the four lo*hi slices close the chunk: 8 A reads per chunk instead of 12.  All tensor-core kernels
-// issue their chunks through this routine, so their accumulation order -- and their results -- stay identical to each other.
-// RAFT_A_COLLECTOR=0 at compile time restores the round-1 order (hi*hi x4, lo*hi x4, hi*lo x4; A/B builds).
-#ifndef RAFT_A_COLLECTOR
-#define RAFT_A_COLLECTOR 1
-#endif
-#define RAFT_UMMA_ASM(GROUP, COLL)                                                                                    \
-  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"                                                            \
-               "tcgen05.mma.cta_group::" GROUP ".kind::f16" COLL " [%0], %1, %2, %3, p;\n}\n" ::"r"(d), "l"(a), "l"(b), \
-               "r"(idesc), "r"(acc)                                                                                   \
-               : "memory")
-template <bool kPair, int kColl>   // kColl: 0 plain, 1 fill, 2 lastuse
-__device__ __forceinline__ void umma_f16_c(uint32_t d, uint64_t a, uint64_t b, uint32_t idesc, uint32_t acc) {
-  if constexpr (kPair) {
-    if constexpr (kColl == 1) RAFT_UMMA_ASM("2", ".collector::a::fill");
-    else if constexpr (kColl == 2) RAFT_UMMA_ASM("2", ".collector::a::lastuse");
-    else RAFT_UMMA_ASM("2", "");
-  } else {
-    if constexpr (kColl == 1) RAFT_UMMA_ASM("1", ".collector::a::fill");
-    else if constexpr (kColl == 2) RAFT_UMMA_ASM("1", ".collector::a::lastuse");
-    else RAFT_UMMA_ASM("1", "");
-  }
-}
-// a_hi / a_lo / b_hi / b_lo: descriptors of the chunk's first K=16 slice (+2 per slice); first: the chunk opens an accumulation
-template <bool kPair>
-__device__ __forceinline__ void umma_chunk3(uint32_t d, uint64_t a_hi, uint64_t a_lo, uint64_t b_hi, uint64_t b_lo, uint32_t idesc,
-                                            bool first) {
-#if RAFT_A_COLLECTOR == 1
+// Per K=16 slice hi*hi then hi*lo, then the four lo*hi slices.  Every tensor-core kernel issues its chunks through this
+// routine, so their accumulation order -- and their results -- stay identical to each other.
+// a_hi / a_lo / b_hi / b_lo: descriptors of the chunk's first K=16 slice (+2 per slice: 32 bytes in 16-byte units);
+// first: the chunk opens an accumulation.  Issued by all 128 threads of a warpgroup.
+template <int N>
+__device__ __forceinline__ void wgmma_chunk3(float (&d)[N / 2], uint64_t a_hi, uint64_t a_lo, uint64_t b_hi, uint64_t b_lo,
+                                             bool first) {
 #pragma unroll
   for (int k = 0; k < 4; ++k) {
-    umma_f16_c<kPair, 1>(d, a_hi + 2 * k, b_hi + 2 * k, idesc, (!first || k > 0) ? 1u : 0u);
-    umma_f16_c<kPair, 2>(d, a_hi + 2 * k, b_lo + 2 * k, idesc, 1u);
+    Wgmma<N>::mma(d, a_hi + 2 * k, b_hi + 2 * k, (!first || k > 0) ? 1u : 0u);
+    Wgmma<N>::mma(d, a_hi + 2 * k, b_lo + 2 * k, 1u);
   }
 #pragma unroll
-  for (int k = 0; k < 4; ++k) umma_f16_c<kPair, 0>(d, a_lo + 2 * k, b_hi + 2 * k, idesc, 1u);
-#elif RAFT_A_COLLECTOR == 2      // (other pairings of the same products, kept for the parity study of the benchmark seed)
-#pragma unroll
-  for (int k = 0; k < 4; ++k) umma_f16_c<kPair, 0>(d, a_lo + 2 * k, b_hi + 2 * k, idesc, (!first || k > 0) ? 1u : 0u);
-#pragma unroll
-  for (int k = 0; k < 4; ++k) {
-    umma_f16_c<kPair, 1>(d, a_hi + 2 * k, b_hi + 2 * k, idesc, 1u);
-    umma_f16_c<kPair, 2>(d, a_hi + 2 * k, b_lo + 2 * k, idesc, 1u);
-  }
-#elif RAFT_A_COLLECTOR == 3
-#pragma unroll
-  for (int k = 0; k < 4; ++k) {
-    umma_f16_c<kPair, 1>(d, a_hi + 2 * k, b_hi + 2 * k, idesc, (!first || k > 0) ? 1u : 0u);
-    umma_f16_c<kPair, 2>(d, a_hi + 2 * k, b_lo + 2 * k, idesc, 1u);
-    umma_f16_c<kPair, 0>(d, a_lo + 2 * k, b_hi + 2 * k, idesc, 1u);
-  }
-#else
-#pragma unroll
-  for (int k = 0; k < 4; ++k) umma_f16_c<kPair, 0>(d, a_hi + 2 * k, b_hi + 2 * k, idesc, (!first || k > 0) ? 1u : 0u);
-#pragma unroll
-  for (int k = 0; k < 4; ++k) umma_f16_c<kPair, 0>(d, a_lo + 2 * k, b_hi + 2 * k, idesc, 1u);
-#pragma unroll
-  for (int k = 0; k < 4; ++k) umma_f16_c<kPair, 0>(d, a_hi + 2 * k, b_lo + 2 * k, idesc, 1u);
-#endif
+  for (int k = 0; k < 4; ++k) Wgmma<N>::mma(d, a_lo + 2 * k, b_hi + 2 * k, 1u);
 }
 
-// 32 lanes x 32 consecutive fp32 columns: thread i of the warp gets lane (base_lane + i).
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x8(uint32_t taddr, uint32_t (&r)[8]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// K-major, 128-byte-swizzled shared-memory operand descriptor (rows of 128 B, 8-row groups
-// 1024 B apart).  Fields as in the PTX ISA "matrix descriptor": start>>4 [0,14), LBO>>4
-// [16,30) (ignored for swizzled K-major; 1), SBO>>4 [32,46), version=1 [46,48), layout [61,64)=2.
+// K-major, 128-byte-swizzled shared-memory operand descriptor (rows of 128 B, 8-row groups 1024 B apart), the layout a
+// TMA box with CU_TENSOR_MAP_SWIZZLE_128B writes.  Fields as in the PTX ISA "matrix descriptor" of wgmma: start>>4 [0,14),
+// LBO>>4 [16,30) (unused for swizzled K-major; 1), SBO>>4 [32,46), base offset [49,52) = 0 (operands start on 1024-byte
+// boundaries), swizzle mode [62,64) = 1 (128 B).
 __device__ __forceinline__ uint64_t make_desc_sw128(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
   d |= (uint64_t)1 << 16;
   d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
 }
-// An operand may start `r` rows (r * 128 bytes) past a 1024-byte boundary of a TMA-written swizzled tile -- the kRow3
-// convolution reads the same 136-pixel activation row at 0 / 1 / 2 pixels offset.  MEASURED on B200 (round 2,
-// profiles/r02_row3_descriptor_ab.txt): the start address alone is right; the tensor core derives the swizzle phase from the
-// address bits, and additionally setting the descriptor's "matrix base offset" field [49,52) to (address >> 7) & 7 -- what the
-// PTX text suggests for unaligned starts -- gives wrong products.
-// kind::f16 instruction descriptor: D=f32 (bits 4-5 = 1), A=B=f16 (0), both K-major, N>>3 at
-// [17,23), M>>4 at [24,29).
-__device__ __forceinline__ uint32_t make_idesc_f16(int m, int n) {
-  return (1u << 4) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
+
+// Named barrier of one warpgroup (ids 1 and 2; 0 is __syncthreads).
+__device__ __forceinline__ void wg_sync(int wg) {
+  asm volatile("bar.sync %0, 128;" ::"r"(wg + 1) : "memory");
 }
 #endif  // __CUDA_ARCH__
 

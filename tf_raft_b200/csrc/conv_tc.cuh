@@ -1,25 +1,26 @@
-// tcgen05 implicit-GEMM kernel: one kernel serves the all-pairs correlation (a 1x1 "conv" whose
-// weights are the other image's features) and every stride-1 convolution of the update blocks.
+// wgmma implicit-GEMM kernel: one kernel serves every convolution of the encoders and the update blocks.
 //
 //   D[128 px, bn cout] = sum over (tap, 64-channel chunk) of  A_tap[128 px, 64] * W_tap[bn, 64]^T
 //
-// * A operand: a TH x TW pixel patch of an NHWC fp16 activation plane, fetched by ONE 4-D TMA box per
-//   (tap, chunk) at coordinates shifted by the tap offset; out-of-image rows/cols are zero-filled by
-//   the TMA unit, which *is* Keras 'same' padding -- no im2col buffer, no halo logic.
-// * B operand: packed weights [tap][cout][cin] fp16, one 3-D TMA box per (tap, chunk).
-// * Both operands land in shared memory K-major with the 128-byte swizzle and are consumed in place
-//   by tcgen05.mma (kind::f16, M=128, N=bn, K=16); the fp32 accumulator lives in TMEM.
-// * fp32-grade arithmetic from fp16 tensor cores: each operand is a (hi, lo) fp16 pair and every
-//   K step issues hi*hi, lo*hi, hi*lo into the same accumulator (DESIGN.md "Precision").
-// * Tensor-core fp32 accumulation truncates (measured: ~0.6 ulp of bias per K=16 step, all towards
-//   zero), so a 1920-deep GRU contraction issued as one 360-step chain is ~60x less accurate than an
-//   FFMA chain.  The K loop is therefore cut into groups of `group_chunks` 64-channel chunks; each
-//   group accumulates into one of two TMEM buffers (ping-pong) and is then promoted -- added in IEEE
-//   fp32 -- into per-thread register accumulators while the next group runs on the tensor core.
-// * Warp roles: warp 0 = TMA producer (one elected lane), warp 1 = TMEM allocator + MMA issuer (one
-//   elected lane), warps 2..9 = promotion + epilogue (TMEM -> registers, then fused bias / activation /
-//   GRU gating / hi-lo re-split -> global).  mbarrier rings: smem full/empty (producer <-> issuer),
-//   TMEM full/empty (issuer <-> promotion warps).
+// * A operand: a TH x TW pixel patch of an NHWC fp16 activation plane, fetched by ONE TMA box per (tap, chunk) at
+//   coordinates shifted by the tap offset; out-of-image rows/cols are zero-filled by the TMA unit, which *is* Keras
+//   'same' padding -- no im2col buffer, no halo logic.
+// * B operand: packed weights [tap][cout][cin] fp16, one TMA box per (tap, chunk).
+// * Both operands land in shared memory K-major with the 128-byte swizzle and are consumed in place by
+//   wgmma.mma_async (m64nNk16, fp16 x fp16 -> fp32 registers).
+// * fp32-grade arithmetic from fp16 tensor cores: each operand is a (hi, lo) fp16 pair and every K step issues hi*hi,
+//   hi*lo, lo*hi into the same accumulator (DESIGN.md "Precision").
+// * Tensor-core fp32 accumulation is not IEEE round-to-nearest, so a 1920-deep GRU contraction issued as one 360-step
+//   chain drifts far more than an FFMA chain.  The K loop is therefore cut into groups of `group_chunks` 64-channel
+//   chunks; each group accumulates into a fresh register tile that is then promoted -- added in IEEE fp32 -- into a
+//   second register tile.  Two register copies of a 64 x N accumulator per warpgroup bound N to kMaxTileN = 128; the
+//   host splits wider layers into column tiles.
+// * Warp roles: warps 0..7 = two consumer warpgroups (rows [0, 64) and [64, 128) of the tile: MMAs, promotion and the
+//   fused epilogue -- bias / activation / GRU gating / hi-lo re-split -> global, through a 64-column shared-memory
+//   staging tile so that each thread owns one pixel row); warp 8 = TMA producer (one elected lane; its warpgroup hands
+//   its registers to the consumers with setmaxnreg, so the two accumulator copies fit without spills).  mbarrier ring:
+//   full (producer -> consumers) / empty (consumers -> producer).  The producer runs up to nstages ahead, so the loads of
+//   tile i+1 overlap the epilogue of tile i.
 #pragma once
 #include <stdlib.h>
 
@@ -35,14 +36,17 @@ enum TcEpilogue : int {
 };
 enum TcAct : int { ACT_NONE = 0, ACT_RELU = 1 };
 
-constexpr int kEpiWarpsConv = 16;         // promotion/epilogue warps of the convolution instantiation (4 per TMEM lane quarter)
 constexpr int kTileM = 128;
 constexpr int kChunkK = 64;                       // fp16 elements per 128-byte swizzled row
 constexpr int kABytes = kTileM * kChunkK * 2;     // 16 KiB per A plane per stage
-constexpr int kEpiPatchBytes = 16 * 2048;         // EPI_GRU_Q: transposition patches of the 16 epilogue warps
-constexpr int kSmemBudget = 227 * 1024 - 2048;
-constexpr int kARow3Pixels = 136;                 // kRow3: activation box width (1 + 128 + 1 pixels, padded to a multiple of 8)
-constexpr int kARow3Bytes = 2 * kARow3Pixels * kChunkK * 2;   // hi + lo planes of one 136-pixel row chunk: 34 KB
+constexpr int kMaxTileN = 128;                    // accumulator columns per tile (two register copies per thread, see above)
+constexpr int kConsumerWGs = 2;                   // MMA + epilogue warpgroups: rows [0, 64) and [64, 128) of the tile
+constexpr int kConsumerWarps = 4 * kConsumerWGs;
+constexpr int kTcThreads = 128 * kConsumerWGs + 128;  // + a producer warpgroup: its first warp issues the TMA loads
+constexpr int kStageCols = 64;                    // epilogue staging: 64 rows x 64 fp32 columns per warpgroup
+constexpr int kStagingBytes = kConsumerWGs * 64 * kStageCols * 4;
+constexpr int kSmemMax = 227 * 1024;              // dynamic shared memory per block on sm_90
+constexpr int kSmemFixed = 1024 /*align slack*/ + kStagingBytes + 512 /*barriers, item queue*/;
 
 struct alignas(64) TcConvParams {
   CUtensorMap a_map[2];           // (hi, lo) plane pair of up to two channel-concatenated sources (K segments)
@@ -51,9 +55,9 @@ struct alignas(64) TcConvParams {
   int kh, kw, ph, pw;             // taps and 'same' padding (pad before)
   int stride;                     // 1 or 2: input pixel = output pixel * stride + tap - pad (TMA elementStrides)
   int B, H, W, TH, TW, tiles_x, tiles_y;
-  int bn, n_total;                // N per CTA (multiple of 16, <= 256); total valid output columns
+  int bn, n_total;                // N per CTA (multiple of 16, <= kMaxTileN); total valid output columns
   int n_tiles_n;                  // column tiles (tile id = n_tile * pixel_tiles + pixel_tile)
-  int nstages, stage_bytes, tmem_cols;
+  int nstages, stage_bytes;
   int group_chunks;               // K chunks per promotion group (accumulation chain = 12 * group_chunks MMAs)
   int mode, act;
   const float* bias;              // [n_total padded to bn multiple]; may be null
@@ -67,24 +71,15 @@ struct alignas(64) TcConvParams {
   const float* concat_src; int concat_n;   // EPI_LINEAR: fp32 (px, concat_n) appended at columns [n_total, n_total+concat_n)
   float* z; int hid;                       // GRU: z plane (px, hid) fp32
   float* h;                                // GRU: hidden state (px, hid) fp32, updated in place by EPI_GRU_Q
-  long long* dbg;                          // optional timeline of CTA 0 (tools/timeline.py): [4][512] clock64 stamps
+  long long* dbg;                          // optional timeline of CTA 0: [4][512] clock64 stamps
   // Programmatic dependent launch (default; RAFT_B200_PDL=0 disables): the launch carries the programmatic-serialization
   // attribute, so this grid's CTAs may be scheduled -- and run their prologue -- while the previous kernel in the stream
   // drains; every thread then executes griddepcontrol.wait before touching global memory.
   int pdl;
-  // kRow3 instantiation (3x3, stride 1, 1 x 128 pixel tiles, cout <= 96: the wide encoder layers).  The three taps of a
-  // kernel row read the SAME image row shifted by one pixel, so a stage holds ONE activation box of 136 pixels (x0-1 ..
-  // x0+134; 136 * 128 B = 17 KB per plane keeps the lo plane on a 1024-byte boundary) and ONE weight box with the row's
-  // three taps; tap dx issues its MMAs on the activation rows [dx, dx + 128) through a descriptor whose start is shifted by
-  // dx * 128 bytes.  3 + 3 boxes per 64-channel chunk instead of 9 + 9: these layers are bound by TMA box delivery.
-  int row3;
   // EPI_LINEAR with n_total == 2 (flow_head.conv2) inside the iteration loop: coords1 += delta_flow and
   // flow = coords1 - coords0 (model.py:102, :97) are applied by the thread that holds the pixel's two output columns.
   float* adv_coords;                       // (px, 2) coords1, updated in place; null = no fused advance
   float* adv_flow;                         // (px, 2) coords1 - pixel grid
-  // update_mega_kernel<true> only: the tile is one half of a CTA pair's M = 256 MMA; a stage holds this CTA's 128 activation
-  // rows and HALF of the bn weight rows (b_map's box is bn / 2 rows).
-  int pair;
 };
 
 #if defined(__CUDA_ARCH__)
@@ -92,33 +87,19 @@ struct alignas(64) TcConvParams {
 __device__ __forceinline__ float4 ld4(const float* p) { return *reinterpret_cast<const float4*>(p); }
 __device__ __forceinline__ float4 ldg4(const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
 __device__ __forceinline__ void st4(float* p, float4 v) { *reinterpret_cast<float4*>(p) = v; }
-// 32-byte global store (STG.256, sm_100): the thread-per-row epilogues write a full 32-byte sector per lane and instruction
-// instead of half of one -- half as many store instructions and LSU wavefronts for the same bytes.  `p` must be 32-byte aligned.
+// 32 bytes per lane as two 16-byte accesses (sm_90 has no 32-byte global load / store).  `p` must be 32-byte aligned.
 __device__ __forceinline__ void st8u(void* p, const uint32_t (&r)[8]) {
-#if defined(RAFT_EPI_EXP) && (RAFT_EPI_EXP & 1)
-  if (r[0] != 0x7fc12345u) return;          // experiment: no epilogue stores (tools/epi_exp.sh)
-#endif
-  asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(p), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]),
-               "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
+  reinterpret_cast<uint4*>(p)[0] = make_uint4(r[0], r[1], r[2], r[3]);
+  reinterpret_cast<uint4*>(p)[1] = make_uint4(r[4], r[5], r[6], r[7]);
 }
-// 32-byte loads: L2-coherent (tensors another CTA of the same grid may have written) and read-only forms.
+// L2-coherent (tensors another CTA of the same grid may have written) and read-only forms.
 __device__ __forceinline__ void ldcg8(const float* p, float (&r)[8]) {
-#if defined(RAFT_EPI_EXP) && (RAFT_EPI_EXP & 2)
-  if (p != nullptr) {                        // experiment: no epilogue operand loads
-#pragma unroll
-    for (int e = 0; e < 8; ++e) r[e] = 0.5f;
-    return;
-  }
-#endif
-  asm volatile("ld.global.cg.v8.f32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=f"(r[0]), "=f"(r[1]), "=f"(r[2]), "=f"(r[3]), "=f"(r[4]), "=f"(r[5]), "=f"(r[6]), "=f"(r[7])
-               : "l"(p));
+  const float4 a = __ldcg(reinterpret_cast<const float4*>(p)), b = __ldcg(reinterpret_cast<const float4*>(p) + 1);
+  r[0] = a.x; r[1] = a.y; r[2] = a.z; r[3] = a.w; r[4] = b.x; r[5] = b.y; r[6] = b.z; r[7] = b.w;
 }
 __device__ __forceinline__ void ldnc8(const float* p, float (&r)[8]) {
-  asm volatile("ld.global.nc.v8.f32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=f"(r[0]), "=f"(r[1]), "=f"(r[2]), "=f"(r[3]), "=f"(r[4]), "=f"(r[5]), "=f"(r[6]), "=f"(r[7])
-               : "l"(p));
+  const float4 a = __ldg(reinterpret_cast<const float4*>(p)), b = __ldg(reinterpret_cast<const float4*>(p) + 1);
+  r[0] = a.x; r[1] = a.y; r[2] = a.z; r[3] = a.w; r[4] = b.x; r[5] = b.y; r[6] = b.z; r[7] = b.w;
 }
 __device__ __forceinline__ void st8f(float* p, float a, float b, float c, float d, float e, float f, float g, float h) {
   const uint32_t r[8] = {__float_as_uint(a), __float_as_uint(b), __float_as_uint(c), __float_as_uint(d),
@@ -129,22 +110,16 @@ __device__ __forceinline__ void st8f(float* p, float a, float b, float c, float 
 // so they must not be served from this SM's L1 nor through the non-coherent path.
 __device__ __forceinline__ float4 ldcg4(const float* p) { return __ldcg(reinterpret_cast<const float4*>(p)); }
 
-#if defined(RAFT_EPI_EXP) && (RAFT_EPI_EXP & 4)
-__device__ __forceinline__ float fast_sigmoid(float x) { return x; }      // experiment: no MUFU
-#else
 __device__ __forceinline__ float fast_sigmoid(float x) { return __fdividef(1.0f, 1.0f + __expf(-x)); }
-#endif
 __device__ __forceinline__ float fast_tanh(float x) { return 1.0f - __fdividef(2.0f, 1.0f + __expf(2.0f * x)); }
 
 // ------------------------------------------------------------------------------------------------
 // Register-resident epilogue of one 32-column chunk of one pixel row (thread == row).
 //
-// Measured: with 227 KB of the unified L1/shared array configured as shared memory, per-thread LOCAL memory does not
-// stay in L1, so the earlier out-of-line routine (accumulators staged through a local buffer, rolled loops) paid an
-// L2 round trip per access: ~32-37 k cycles per tile regardless of the tile width.  Here nothing leaves registers:
-// the routine is inlined and specialised on the epilogue mode at compile time, loops are fully unrolled so the
-// independent 16-byte global loads (bias, h, z, residual) are all in flight together, and the activation math uses
-// the fast exp / reciprocal units (|error| ~1e-7, far inside the parity budget).
+// With 227 KB of the unified L1/shared array configured as shared memory, per-thread local memory does not stay in L1,
+// so nothing here leaves registers: the routine is inlined and specialised on the epilogue mode at compile time, loops
+// are fully unrolled so the independent 16-byte global loads (bias, h, z, residual) are all in flight together, and the
+// activation math uses the fast exp / reciprocal units (|error| ~1e-7, far inside the parity budget).
 // ------------------------------------------------------------------------------------------------
 template <int MODE>
 __device__ __forceinline__ void tc_epilogue_regs(const TcConvParams& p, float (&v)[32], size_t pix, int col, int ncol,
@@ -317,391 +292,224 @@ __device__ __forceinline__ void tc_epilogue_regs(const TcConvParams& p, float (&
 }
 
 // ------------------------------------------------------------------------------------------------
-// Coalesced GRU-q epilogue of a 32-row x 16-column accumulator block, AFTER transposition through shared memory:
-// lane l holds rows (l>>2) + 8k (k = 0..3) and columns col .. col+3 of the block, so every global access of a warp
-// touches 8 rows x 64 contiguous bytes instead of 32 rows x 16 bytes.  Measured on the thread-per-row form: the LSU
-// retires about one distinct 128-byte line per cycle, which made the epilogue of a 256-column tile cost 14-22 k cycles.
-// pixr[k] is the flat pixel index of row k (-1 = outside the image).
+// Shared by conv_tc_kernel and update_mega_kernel: the ring walk of one tile, its producer side and its consumer side.
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void store_split4(__half* hi, __half* lo, size_t o, bool aligned, const float (&v)[4]) {
-  uint32_t h01, l01, h23, l23;
-  split_f16x2(v[0], v[1], h01, l01);
-  split_f16x2(v[2], v[3], h23, l23);
-  if (aligned) {
-    *reinterpret_cast<uint2*>(hi + o) = make_uint2(h01, h23);
-    *reinterpret_cast<uint2*>(lo + o) = make_uint2(l01, l23);
-  } else {
-    const uint32_t hh[2] = {h01, h23}, ll[2] = {l01, l23};
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      hi[o + e] = __ushort_as_half((unsigned short)(hh[e >> 1] >> (16 * (e & 1))));
-      lo[o + e] = __ushort_as_half((unsigned short)(ll[e >> 1] >> (16 * (e & 1))));
-    }
-  }
+struct RingPos {            // next ring slot and the parity of every slot's use count (producer and consumers each keep one)
+  int slot;
+  uint32_t par;
+};
+
+__device__ __forceinline__ int ring_next(RingPos& r, int nst) {
+  const int s = r.slot;
+  r.slot = s + 1 == nst ? 0 : s + 1;
+  return s;
 }
 
-__device__ __forceinline__ void tc_epilogue_q_t(const TcConvParams& p, float (&v)[4][4], const int (&pixr)[4], int col,
-                                              float inv_scale) {
-  if (p.bias) {
-    const float4 bq = ldg4(p.bias + col);            // bias / affine arrays are zero-padded past the last column
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      v[k][0] = v[k][0] * inv_scale + bq.x; v[k][1] = v[k][1] * inv_scale + bq.y;
-      v[k][2] = v[k][2] * inv_scale + bq.z; v[k][3] = v[k][3] * inv_scale + bq.w;
-    }
-  } else {
-#pragma unroll
-    for (int k = 0; k < 4; ++k)
-#pragma unroll
-      for (int e = 0; e < 4; ++e) v[k][e] *= inv_scale;
-  }
+__device__ __forceinline__ int tc_total_chunks(const TcConvParams& c) {
+  return c.kh * c.kw * (c.seg_chunks[0] + (c.nseg > 1 ? c.seg_chunks[1] : 0));
+}
 
-  // h = (1-z)*h + z*tanh(v), in place
-  {
-    const bool h_vec = ((p.h_stride | p.h_c0) & 3) == 0;
-#pragma unroll
-    for (int k0 = 0; k0 < 4; k0 += 2) {                // two rows at a time: loads in flight together, registers bounded
-      float4 zv[2], hv[2];
-#pragma unroll
-      for (int kk = 0; kk < 2; ++kk) {
-        const bool ok = pixr[k0 + kk] >= 0;
-        zv[kk] = ok ? ldcg4(p.z + (size_t)pixr[k0 + kk] * p.hid + col) : make_float4(0.f, 0.f, 0.f, 0.f);
-        hv[kk] = ok ? ldcg4(p.h + (size_t)pixr[k0 + kk] * p.hid + col) : make_float4(0.f, 0.f, 0.f, 0.f);
-      }
-#pragma unroll
-      for (int kk = 0; kk < 2; ++kk) {
-        const int k = k0 + kk;
-        if (pixr[k] < 0) continue;
-        v[k][0] = (1.0f - zv[kk].x) * hv[kk].x + zv[kk].x * fast_tanh(v[k][0]);
-        v[k][1] = (1.0f - zv[kk].y) * hv[kk].y + zv[kk].y * fast_tanh(v[k][1]);
-        v[k][2] = (1.0f - zv[kk].z) * hv[kk].z + zv[kk].z * fast_tanh(v[k][2]);
-        v[k][3] = (1.0f - zv[kk].w) * hv[kk].w + zv[kk].w * fast_tanh(v[k][3]);
-        st4(p.h + (size_t)pixr[k] * p.hid + col, make_float4(v[k][0], v[k][1], v[k][2], v[k][3]));
-        store_split4(p.out_hi, p.out_lo, (size_t)pixr[k] * p.h_stride + p.h_c0 + col, h_vec, v[k]);
+// Producer: streams the (tap, chunk) stages of one tile.  claim != null: *claim = atomicAdd(next_item) just before the last
+// stage (late enough that the CTA is about to be free, early enough that the atomic hides behind the slot wait).
+__device__ __forceinline__ void tc_produce_tile(const TcConvParams& c, uint8_t* stages, uint64_t* full_bar, uint64_t* empty_bar,
+                                                RingPos& rp, int nt, int b, int ty, int tx, unsigned int* next_item = nullptr,
+                                                int* claim = nullptr) {
+  const int ntaps = c.kh * c.kw;
+  const int x0 = tx * c.TW * c.stride, y0 = ty * c.TH * c.stride, n0 = nt * c.bn;
+  int left = tc_total_chunks(c);
+  for (int tap = 0; tap < ntaps; ++tap) {
+    const int dy = tap / c.kw - c.ph, dx = tap % c.kw - c.pw;
+    int kc = 0;
+    for (int seg = 0; seg < c.nseg; ++seg) {
+      for (int ch = 0; ch < c.seg_chunks[seg]; ++ch, ++kc) {
+        if (--left == 0 && claim) *claim = (int)atomicAdd(next_item, 1u);
+        const int s = ring_next(rp, c.nstages);
+        mbar_wait(&empty_bar[s], ((rp.par >> s) & 1u) ^ 1u);
+        rp.par ^= 1u << s;
+        uint8_t* st = stages + (size_t)s * c.stage_bytes;
+        mbar_arrive_expect_tx(&full_bar[s], (uint32_t)c.stage_bytes);
+        // two boxes per stage: [A_hi | A_lo] and [B_hi | B_lo]
+        tma_load_5d(st, &c.a_map[seg], &full_bar[s], c.seg_c0[seg] + ch * kChunkK, x0 + dx, y0 + dy, b, 0);
+        tma_load_4d(st + 2 * kABytes, &c.b_map, &full_bar[s], kc * kChunkK, n0, tap, 0);
       }
     }
   }
 }
 
+// Staging tile of one warpgroup: 64 rows x 64 fp32, 16-byte groups XOR-swizzled by row (conflict-free row reads).
+__device__ __forceinline__ int stg_idx(int r, int c) { return r * kStageCols + ((((c >> 2) ^ (r & 7))) << 2) + (c & 3); }
+
+// Consumer side of one tile, all 128 threads of warpgroup `wg` (tid = thread index inside it): MMAs over the ring with
+// IEEE-fp32 promotion every group_chunks chunks, then the epilogue of the warpgroup's 64 rows.  N >= c.bn is the
+// instantiated MMA width (columns past bn read other shared memory and are discarded).
+template <int N>
+__device__ __forceinline__ void tc_consume_tile(const TcConvParams& c, uint8_t* stages, float* staging, uint64_t* full_bar,
+                                                uint64_t* empty_bar, RingPos& rp, int wg, int tid, int nt, int b, int ty,
+                                                int tx) {
+  const int lane = tid & 31, w = tid >> 5;
+  const int total = tc_total_chunks(c);
+  const uint32_t b_bytes = (uint32_t)(c.bn * kChunkK * 2);
+  float acc[N / 2], racc[N / 2];
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) acc[i] = racc[i] = 0.0f;
+  for (int done = 0; done < total;) {
+    const int gend = min(total, done + c.group_chunks);
+    for (int first = 1; done < gend; ++done, first = 0) {
+      const int s = ring_next(rp, c.nstages);
+      mbar_wait(&full_bar[s], (rp.par >> s) & 1u);
+      rp.par ^= 1u << s;
+      const uint32_t sa = smem_u32(stages + (size_t)s * c.stage_bytes);
+      const uint32_t arow = (uint32_t)wg * 64 * 128;
+      wgmma_fence_regs(acc);
+      wgmma_fence();
+      wgmma_chunk3<N>(acc, make_desc_sw128(sa + arow), make_desc_sw128(sa + kABytes + arow), make_desc_sw128(sa + 2 * kABytes),
+                      make_desc_sw128(sa + 2 * kABytes + b_bytes), first != 0);
+      wgmma_commit();
+      wgmma_wait_all();
+      wgmma_fence_regs(acc);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[s]);       // this warp's reads of the slot are complete
+    }
+#pragma unroll
+    for (int i = 0; i < N / 2; ++i) racc[i] += acc[i];   // IEEE fp32 promotion
+  }
+
+  // ---- epilogue: 64-column blocks through the staging tile; thread (row, half) then owns 32 columns of one pixel row ----
+  float* stg = staging + wg * 64 * kStageCols;
+  const int row = tid & 63, half = tid >> 6;
+  const int m = wg * 64 + row;
+  const int x = tx * c.TW + m % c.TW, y = ty * c.TH + m / c.TW;
+  const bool inside = x < c.W && y < c.H;
+  const size_t pix = ((size_t)b * c.H + y) * c.W + x;
+  const float inv_scale = c.inv_scale ? __ldg(c.inv_scale) : 1.0f;
+#pragma unroll
+  for (int cb = 0; cb < (N + kStageCols - 1) / kStageCols; ++cb) {
+    if (cb * kStageCols >= c.bn) break;
+    wg_sync(wg);                                       // the previous block's readers are done with the tile
+#pragma unroll
+    for (int i = cb * 8; i < min(cb * 8 + 8, N / 8); ++i) {
+      const int col = 8 * (i - cb * 8) + 2 * (lane & 3), r0 = 16 * w + (lane >> 2);
+      *reinterpret_cast<float2*>(stg + stg_idx(r0, col)) = make_float2(racc[4 * i], racc[4 * i + 1]);
+      *reinterpret_cast<float2*>(stg + stg_idx(r0 + 8, col)) = make_float2(racc[4 * i + 2], racc[4 * i + 3]);
+    }
+    wg_sync(wg);
+    const int c0 = cb * kStageCols + half * 32;
+    if (inside && c0 < c.bn) {
+      const int ncol = min(32, c.bn - c0);
+      float v[32];
+#pragma unroll
+      for (int q = 0; q < 8; ++q) {
+        const float4 t4 = *reinterpret_cast<const float4*>(stg + stg_idx(row, half * 32 + 4 * q));
+        v[4 * q] = t4.x; v[4 * q + 1] = t4.y; v[4 * q + 2] = t4.z; v[4 * q + 3] = t4.w;
+      }
+#pragma unroll
+      for (int j = 0; j < 32; ++j)
+        if (j >= ncol) v[j] = 0.0f;
+      if (c.mode == EPI_LINEAR) tc_epilogue_regs<EPI_LINEAR>(c, v, pix, nt * c.bn + c0, ncol, inv_scale);
+      else if (c.mode == EPI_GRU_ZR) tc_epilogue_regs<EPI_GRU_ZR>(c, v, pix, nt * c.bn + c0, ncol, inv_scale);
+      else tc_epilogue_regs<EPI_GRU_Q>(c, v, pix, nt * c.bn + c0, ncol, inv_scale);
+    }
+  }
+}
+
+// Instantiated MMA widths: bn (a multiple of 16, <= 128) rounds up to the next of these.
+template <class F>
+__device__ __forceinline__ void with_mma_n(int bn, F&& f) {
+  if (bn <= 16) f(std::integral_constant<int, 16>{});
+  else if (bn <= 32) f(std::integral_constant<int, 32>{});
+  else if (bn <= 64) f(std::integral_constant<int, 64>{});
+  else if (bn <= 96) f(std::integral_constant<int, 96>{});
+  else f(std::integral_constant<int, 128>{});
+}
+
+// Register split between the producer warpgroup and the two consumer warpgroups: 128 * 40 + 256 * 232 <= 64 K.
+__device__ __forceinline__ void regs_producer() { asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory"); }
+__device__ __forceinline__ void regs_consumer() { asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory"); }
+
+__device__ __forceinline__ void tc_decode_tile(const TcConvParams& c, int t, int& nt, int& b, int& ty, int& tx) {
+  const int mtiles = c.B * c.tiles_y * c.tiles_x;
+  nt = t / mtiles;
+  int mt = t - nt * mtiles;
+  tx = mt % c.tiles_x;
+  mt /= c.tiles_x;
+  ty = mt % c.tiles_y;
+  b = mt / c.tiles_y;
+}
 #endif
 
-// kRowEpi selects the epilogue form at compile time: thread-per-row registers (EPI_LINEAR, EPI_GRU_ZR) or transposed through
-// shared-memory patches (EPI_GRU_Q), so that neither costs the other registers or code.
-template <bool kRowEpi, bool kRow3 = false>
-__global__ void __launch_bounds__(64 + 32 * kEpiWarpsConv, 1) conv_tc_kernel(const __grid_constant__ TcConvParams p) {
+__global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_constant__ TcConvParams p) {
 #if defined(__CUDA_ARCH__)
-  // Persistent: CTA c processes output tiles c, c + gridDim.x, ...  A tile is (pixel tile, column tile).  All
-  // three roles walk the same tile sequence; the smem ring and the two TMEM buffers carry straight across
-  // tile boundaries, so the loads and MMAs of tile i+1 overlap the epilogue of tile i.
-  constexpr int kEpiWarps = kEpiWarpsConv;
+  // Persistent: CTA c processes output tiles c, c + gridDim.x, ...  A tile is (pixel tile, column tile).  Producer and
+  // consumers walk the same tile sequence; the ring carries straight across tile boundaries.
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int nst = p.nstages;
-  const int b_bytes = p.bn * kChunkK * 2;
-  uint8_t* stages = smem;                                     // ring of nst stages
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(stages + (size_t)nst * p.stage_bytes);
+  uint8_t* stages = smem;
+  float* staging = reinterpret_cast<float*>(stages + (size_t)nst * p.stage_bytes);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(staging) + kStagingBytes);
   uint64_t* empty_bar = full_bar + nst;
-  uint64_t* acc_full = empty_bar + nst;      // [2] issuer -> promotion warps
-  uint64_t* acc_empty = acc_full + 2;        // [2] promotion warps -> issuer
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(acc_empty + 2);
-  float* patches = reinterpret_cast<float*>(stages + (size_t)nst * p.stage_bytes + 256);   // transposition patches (GRU q)
 
   const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-
   const int mtiles = p.B * p.tiles_y * p.tiles_x;
   const int ntiles = mtiles * p.n_tiles_n;
-  const int ntaps = p.kh * p.kw;
-  const int chunks_per_tap = p.seg_chunks[0] + (p.nseg > 1 ? p.seg_chunks[1] : 0);
-  const int total = (kRow3 ? p.kh : ntaps) * chunks_per_tap;   // stages per tile (kRow3: one per kernel row and chunk)
-  const int gsz = p.group_chunks;
-  const int ngroups = (total + gsz - 1) / gsz;            // promotion groups per tile
-  const int nchunks32 = (p.bn + 31) >> 5;                 // 32-column accumulator chunks
-  constexpr int kParts = kEpiWarps / 4;                   // warps per TMEM lane quarter: each takes a slice of the columns
-  constexpr int kMaxCh = 8 / kParts;                      // accumulator chunks per thread (2)
-  const int chunks_per_part = (nchunks32 + kParts - 1) / kParts;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     for (int s = 0; s < nst; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&acc_full[i], 1);
-      mbar_init(&acc_empty[i], 4 * ((nchunks32 + chunks_per_part - 1) / chunks_per_part));   // one arrival per participating warp
+      mbar_init(&empty_bar[s], kConsumerWarps);
     }
     fence_mbar_init();
+  }
+  if (warp == kConsumerWarps && (threadIdx.x & 31) == 0) {
     prefetch_tmap(&p.a_map[0]);
     prefetch_tmap(&p.b_map);
     if (p.nseg > 1) prefetch_tmap(&p.a_map[1]);
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_holder, (uint32_t)p.tmem_cols);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_holder;
-  if (p.pdl && warp != 0) {
-    // barriers, TMEM and tensor-map prefetch above touch no global data; from here on the previous grid's results are
-    // read (and its inputs overwritten), so wait for it, then let the next grid in the stream start its own prologue.
-    // (Warp 0 = the producer thread waits further down, after it has started fetching the weights of the first stages.)
+  if (p.pdl) {
+    // barriers and tensor-map prefetch above touch no global data; from here on the previous grid's results are read
+    // (and its inputs overwritten), so wait for it, then let the next grid in the stream start its own prologue.
     asm volatile("griddepcontrol.wait;" ::: "memory");
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   }
 
-  if (warp == 0) {
+  RingPos rp{0, 0u};
+  if (warp >= kConsumerWarps) {
     // ===================== TMA producer =====================
-    if (elect_one()) {
-      int it = 0;
-      int npre = 0;                // stages whose weight box was issued before the dependency wait (PDL only)
-      if (p.pdl) {
-        // Convolution weights do not depend on the previous grid: fetch them for the first stages of this CTA's first
-        // tile while that grid is still draining, then wait, then fetch the activations.
-        if (!kRow3 && (int)blockIdx.x < ntiles) {
-          const int n0 = ((int)blockIdx.x / mtiles) * p.bn;
-          npre = min(nst, total);
-#pragma unroll 1
-          for (int i = 0; i < npre; ++i) {
-            mbar_arrive_expect_tx(&full_bar[i], (uint32_t)p.stage_bytes);
-            tma_load_4d(stages + (size_t)i * p.stage_bytes + 2 * kABytes, &p.b_map, &full_bar[i], (i % chunks_per_tap) * kChunkK,
-                        n0, i / chunks_per_tap, 0);
-          }
-        }
-        asm volatile("griddepcontrol.wait;" ::: "memory");
-        asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-      }
+    regs_producer();
+    if (warp == kConsumerWarps && elect_one()) {
       for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
-        const int nt = t / mtiles;
-        int mt = t - nt * mtiles;
-        const int tx = mt % p.tiles_x;
-        mt /= p.tiles_x;
-        const int ty = mt % p.tiles_y;
-        const int b = mt / p.tiles_y;
-        const int x0 = tx * p.TW * p.stride, y0 = ty * p.TH * p.stride, n0 = nt * p.bn;
-        if constexpr (kRow3) {
-          for (int ky = 0; ky < p.kh; ++ky) {
-            for (int ch = 0; ch < p.seg_chunks[0]; ++ch, ++it) {
-              const int s = it % nst;
-              mbar_wait(&empty_bar[s], ((uint32_t)(it / nst) & 1u) ^ 1u);
-              if (p.dbg && blockIdx.x == 0 && it < 512) p.dbg[it] = clock64();              // slot free
-              uint8_t* st = stages + (size_t)s * p.stage_bytes;
-              mbar_arrive_expect_tx(&full_bar[s], (uint32_t)p.stage_bytes);
-              tma_load_5d(st, &p.a_map[0], &full_bar[s], p.seg_c0[0] + ch * kChunkK, x0 - p.pw, y0 + ky - p.ph, b, 0);
-              tma_load_4d(st + kARow3Bytes, &p.b_map, &full_bar[s], ch * kChunkK, n0, ky * p.kw, 0);
-            }
-          }
-        } else {
-          for (int tap = 0; tap < ntaps; ++tap) {
-            const int dy = tap / p.kw - p.ph, dx = tap % p.kw - p.pw;
-            int kc = 0;
-            for (int seg = 0; seg < p.nseg; ++seg) {
-              for (int ch = 0; ch < p.seg_chunks[seg]; ++ch, ++kc, ++it) {
-                const int s = it % nst;
-                const uint32_t phase = (uint32_t)(it / nst) & 1u;
-                mbar_wait(&empty_bar[s], phase ^ 1u);
-                if (p.dbg && blockIdx.x == 0 && it < 512) p.dbg[it] = clock64();              // slot free
-                uint8_t* st = stages + (size_t)s * p.stage_bytes;
-                const int c = p.seg_c0[seg] + ch * kChunkK;
-#if defined(RAFT_TC_EXP) && (RAFT_TC_EXP & 6)        // mainloop experiments (tools/tc_exp.sh; run with RAFT_B200_PDL=0)
-                if (RAFT_TC_EXP & 2) {               // activations only
-                  mbar_arrive_expect_tx(&full_bar[s], (uint32_t)(2 * kABytes));
-                  tma_load_5d(st, &p.a_map[seg], &full_bar[s], c, x0 + dx, y0 + dy, b, 0);
-                } else {                             // weights only
-                  mbar_arrive_expect_tx(&full_bar[s], (uint32_t)(p.stage_bytes - 2 * kABytes));
-                  tma_load_4d(st + 2 * kABytes, &p.b_map, &full_bar[s], kc * kChunkK, n0, tap, 0);
-                }
-#else
-                if (it >= npre) mbar_arrive_expect_tx(&full_bar[s], (uint32_t)p.stage_bytes);
-                // two boxes per stage: [A_hi | A_lo] and [B_hi | B_lo] (TMA cost is per box, not per byte)
-                tma_load_5d(st, &p.a_map[seg], &full_bar[s], c, x0 + dx, y0 + dy, b, 0);
-                if (it >= npre) tma_load_4d(st + 2 * kABytes, &p.b_map, &full_bar[s], kc * kChunkK, n0, tap, 0);
-#endif
-              }
-            }
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    const uint32_t idesc = make_idesc_f16(kTileM, p.bn);
-    int it = 0, gg = 0;
-    for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
-      int done = 0;
-      for (int g = 0; g < ngroups; ++g, ++gg) {
-        const int buf = gg & 1;
-        mbar_wait(&acc_empty[buf], ((uint32_t)(gg >> 1) & 1u) ^ 1u);   // promotion warps drained this buffer
-        tc_fence_after();
-        if (p.dbg && blockIdx.x == 0 && gg < 256 && lane == 0) p.dbg[1024 + 256 + gg] = clock64();   // issuer owns the buffer
-        const uint32_t d_tmem = tmem_base + (uint32_t)(buf * p.bn);
-        const int gend = min(total, done + gsz);
-        for (int first = 1; done < gend; ++done, ++it, first = 0) {
-          const int s = it % nst;
-          const uint32_t phase = (uint32_t)(it / nst) & 1u;
-          mbar_wait(&full_bar[s], phase);
-          tc_fence_after();
-          if (p.dbg && blockIdx.x == 0 && it < 512 && lane == 0) p.dbg[512 + it] = clock64();   // data landed
-          if (elect_one()) {
-            const uint32_t sa = smem_u32(stages + (size_t)s * p.stage_bytes);
-            if constexpr (kRow3) {
-              // stage = [A hi: 136 rows | A lo: 136 rows | W hi: tap 0, 1, 2 | W lo: tap 0, 1, 2]
-#pragma unroll 1
-              for (int dx = 0; dx < 3; ++dx) {
-                const uint64_t a_hi = make_desc_sw128(sa + dx * 128);     // shifted start, base-offset field 0 (common.cuh)
-                const uint64_t a_lo = make_desc_sw128(sa + kARow3Bytes / 2 + dx * 128);
-                const uint64_t b_hi = make_desc_sw128(sa + kARow3Bytes + dx * b_bytes);
-                const uint64_t b_lo = make_desc_sw128(sa + kARow3Bytes + (3 + dx) * b_bytes);
-                umma_chunk3<false>(d_tmem, a_hi, a_lo, b_hi, b_lo, idesc, first != 0 && dx == 0);
-              }
-            } else {
-              const uint64_t a_hi = make_desc_sw128(sa);
-              const uint64_t a_lo = make_desc_sw128(sa + kABytes);
-              const uint64_t b_hi = make_desc_sw128(sa + 2 * kABytes);
-              const uint64_t b_lo = make_desc_sw128(sa + 2 * kABytes + b_bytes);
-#if defined(RAFT_TC_EXP) && (RAFT_TC_EXP & 1)        // experiment: no MMAs, only the commits
-              if (sa != 0xffffffffu) goto tc_exp_skip_mma;
-#endif
-              umma_chunk3<false>(d_tmem, a_hi, a_lo, b_hi, b_lo, idesc, first != 0);   // (+32 bytes per K=16 slice == +2 in 16-byte units)
-#if defined(RAFT_TC_EXP) && (RAFT_TC_EXP & 1)
-            tc_exp_skip_mma:;
-#endif
-            }
-            umma_commit(&empty_bar[s]);                      // frees the smem slot once these MMAs retire
-            if (done == gend - 1) umma_commit(&acc_full[buf]);   // group complete -> promotion warps
-          }
-          __syncwarp();
-        }
+        int nt, b, ty, tx;
+        tc_decode_tile(p, t, nt, b, ty, tx);
+        tc_produce_tile(p, stages, full_bar, empty_bar, rp, nt, b, ty, tx);
       }
     }
   } else {
-    // ===================== promotion + epilogue (warps 2..17) =====================
-    const int quarter = warp & 3;                    // TMEM lane quarter this warp may access
-    const int part_id = (warp - 2) >> 2;             // column slice of this warp within its lane quarter
-    const int chunk0 = part_id * chunks_per_part;
-    const int my_chunks = max(0, min(chunks_per_part, nchunks32 - chunk0));
-    const int m = quarter * 32 + lane;               // tile row == TMEM lane
-    const int xl = m % p.TW, yl = m / p.TW;
-    const float inv_scale = p.inv_scale ? __ldg(p.inv_scale) : 1.0f;
-    const uint32_t trow = tmem_base + ((uint32_t)(quarter * 32) << 16);
-
-    if (my_chunks > 0) {
-      int gg = 0;
+    // ===================== MMA + epilogue (warpgroups 0, 1) =====================
+    regs_consumer();
+    const int wg = warp >> 2, tid = threadIdx.x & 127;
+    with_mma_n(p.bn, [&](auto n) {
       for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
-        float racc[kMaxCh][32];
-#pragma unroll
-        for (int ci = 0; ci < kMaxCh; ++ci)
-#pragma unroll
-          for (int j = 0; j < 32; ++j) racc[ci][j] = 0.0f;
-
-        for (int g = 0; g < ngroups; ++g, ++gg) {
-          const int buf = gg & 1;
-          mbar_wait(&acc_full[buf], (uint32_t)(gg >> 1) & 1u);
-          tc_fence_after();
-          if (p.dbg && blockIdx.x == 0 && gg < 256 && warp == 2 && lane == 0) p.dbg[1024 + gg] = clock64();   // group retired
-#pragma unroll
-          for (int ci = 0; ci < kMaxCh; ++ci) {
-            if (ci < my_chunks) {
-              const int c0 = (chunk0 + ci) * 32;
-              uint32_t r[32];
-              if (p.bn - c0 >= 32) {
-                tmem_ld_32x32(trow + (uint32_t)(buf * p.bn + c0), r);
-              } else {
-                uint32_t r16[16];
-                tmem_ld_32x16(trow + (uint32_t)(buf * p.bn + c0), r16);
-#pragma unroll
-                for (int j = 0; j < 16; ++j) r[j] = r16[j];
-#pragma unroll
-                for (int j = 16; j < 32; ++j) r[j] = 0u;
-              }
-              tmem_ld_wait();
-#pragma unroll
-              for (int j = 0; j < 32; ++j) racc[ci][j] += __uint_as_float(r[j]);   // IEEE fp32 promotion
-            }
-          }
-          tc_fence_before();
-          __syncwarp();
-          if (p.dbg && blockIdx.x == 0 && gg < 256 && warp == 2 && lane == 0) p.dbg[1536 + gg] = clock64();   // group drained
-          if (lane == 0) mbar_arrive(&acc_empty[buf]);
-        }
-
-        // ---- epilogue of this tile (the issuer is already accumulating the next one) ----
-        const int nt = t / mtiles;
-        int mt = t - nt * mtiles;
-        const int tx = mt % p.tiles_x;
-        mt /= p.tiles_x;
-        const int ty = mt % p.tiles_y;
-        const int b = mt / p.tiles_y;
-        const int x = tx * p.TW + xl, y = ty * p.TH + yl;
-        if constexpr (kRowEpi) {    // thread-per-row register epilogue (EPI_LINEAR, EPI_GRU_ZR)
-          if (x < p.W && y < p.H) {
-            const size_t pix = ((size_t)b * p.H + y) * p.W + x;
-#pragma unroll
-            for (int ci = 0; ci < kMaxCh; ++ci) {
-              if (ci < my_chunks) {
-                const int c0 = (chunk0 + ci) * 32;
-                const int ncol = min(32, p.bn - c0);
-                if (p.mode == EPI_LINEAR) tc_epilogue_regs<EPI_LINEAR>(p, racc[ci], pix, nt * p.bn + c0, ncol, inv_scale);
-                else tc_epilogue_regs<EPI_GRU_ZR>(p, racc[ci], pix, nt * p.bn + c0, ncol, inv_scale);
-              }
-            }
-          }
-        } else {                           // EPI_GRU_Q: coalesced epilogue through a 32 x 16 transposition patch (measured:
-                                           // 13 k cycles vs 23 k thread-per-row; the other modes measured slower transposed)
-          float4* patch4 = reinterpret_cast<float4*>(patches + (warp - 2) * 512);
-          const int pix_own = (x < p.W && y < p.H) ? (int)(((size_t)b * p.H + y) * p.W + x) : -1;
-          int pixr[4];
-#pragma unroll
-          for (int k = 0; k < 4; ++k) pixr[k] = __shfl_sync(0xffffffffu, pix_own, (lane >> 2) + 8 * k);
-          const int c4 = lane & 3;
-          const int wsw = (lane >> 1) & 3, rsw = (lane >> 3) & 3;   // XOR swizzles: conflict-free 16-byte writes and reads
-#pragma unroll
-          for (int ci = 0; ci < kMaxCh; ++ci) {
-            if (ci < my_chunks) {
-#pragma unroll
-              for (int hh = 0; hh < 2; ++hh) {
-                const int c0 = (chunk0 + ci) * 32 + hh * 16;
-                if (c0 < p.bn) {
-                  __syncwarp();
-#pragma unroll
-                  for (int q = 0; q < 4; ++q)
-                    patch4[lane * 4 + (q ^ wsw)] = make_float4(racc[ci][hh * 16 + 4 * q], racc[ci][hh * 16 + 4 * q + 1],
-                                                               racc[ci][hh * 16 + 4 * q + 2], racc[ci][hh * 16 + 4 * q + 3]);
-                  __syncwarp();
-                  float v[4][4];
-#pragma unroll
-                  for (int k = 0; k < 4; ++k) {
-                    const float4 t4 = patch4[((lane >> 2) + 8 * k) * 4 + (c4 ^ rsw)];
-                    v[k][0] = t4.x; v[k][1] = t4.y; v[k][2] = t4.z; v[k][3] = t4.w;
-                  }
-                  const int col = nt * p.bn + c0 + 4 * c4;
-                  tc_epilogue_q_t(p, v, pixr, col, inv_scale);
-                }
-              }
-            }
-          }
-        }
-        if (p.dbg && blockIdx.x == 0 && warp == 2 && lane == 0) {
-          p.dbg[2047] = clock64();                                           // epilogue of the (last) tile done
+        int nt, b, ty, tx;
+        tc_decode_tile(p, t, nt, b, ty, tx);
+        if (p.dbg && blockIdx.x == 0 && threadIdx.x == 0) {
           const int tl = (t - (int)blockIdx.x) / (int)gridDim.x;
-          if (tl < 255) p.dbg[1536 + 256 + tl] = clock64();                   // ... of every tile
+          if (tl < 512) p.dbg[tl] = clock64();                               // tile started
+        }
+        tc_consume_tile<decltype(n)::value>(p, stages, staging, full_bar, empty_bar, rp, wg, tid, nt, b, ty, tx);
+        if (p.dbg && blockIdx.x == 0 && threadIdx.x == 0) {
+          const int tl = (t - (int)blockIdx.x) / (int)gridDim.x;
+          if (tl < 512) p.dbg[512 + tl] = clock64();                         // tile's epilogue done
         }
       }
-    }
+    });
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, (uint32_t)p.tmem_cols);
 #endif
 }
 
 // ------------------------------------------------------------------------------------------------
 // Host side
 // ------------------------------------------------------------------------------------------------
-inline bool tc_uses_patch(int mode) { return mode == EPI_GRU_Q; }
-
 inline void tc_pick_tile(int W, int H, int* tw, int* th) {
   // TW*TH = 128 with TW a power of two; minimise padded area, prefer wide tiles on ties.
   long best = -1;
@@ -716,22 +524,24 @@ inline void tc_pick_tile(int W, int H, int* tw, int* th) {
   }
 }
 
-// Fills the derived launch fields (tile grid, stages, TMEM columns) of `p`; returns bytes of
-// dynamic shared memory.  Caller has set bn, B, H, W, TH, TW.
+// Column tiling of a layer whose N per CTA exceeds kMaxTileN: the CTA's N is divided by the returned factor and the
+// number of column tiles multiplied by it (0: no such split keeps N a multiple of 16).
+inline int tc_n_split(int bn) {
+  const int f = ceil_div(bn, kMaxTileN);
+  return bn % (16 * f) == 0 ? f : 0;
+}
+
+// Fills the derived launch fields (tile grid, stages) of `p`; returns bytes of dynamic shared memory.  Caller has set
+// bn, B, H, W, TH, TW.
 inline int tc_finalize(TcConvParams& p) {
   p.tiles_x = ceil_div(p.W, p.TW);
   p.tiles_y = ceil_div(p.H, p.TH);
-  p.stage_bytes = 2 * kABytes + 2 * (p.pair ? p.bn / 2 : p.bn) * kChunkK * 2;
-  if (p.row3) p.stage_bytes = kARow3Bytes + 3 * 2 * p.bn * kChunkK * 2;
-  const int patch = tc_uses_patch(p.mode) ? kEpiPatchBytes : 0;   // 16 x 2 KB patches (GRU q)
-  int nst = (kSmemBudget - patch) / p.stage_bytes;
+  p.stage_bytes = 2 * kABytes + 2 * p.bn * kChunkK * 2;
+  int nst = (kSmemMax - kSmemFixed) / p.stage_bytes;
   if (nst > 8) nst = 8;
   p.nstages = nst;
-  int cols = 32;
-  while (cols < 2 * p.bn) cols <<= 1;           // two accumulator buffers (ping-pong promotion)
-  p.tmem_cols = cols;
   if (p.group_chunks <= 0) p.group_chunks = 2;
-  return nst * p.stage_bytes + 1024 /*align slack*/ + 256 /*barriers*/ + patch;
+  return nst * p.stage_bytes + kSmemFixed;
 }
 
 // RAFT_B200_PDL=0 disables programmatic dependent launch of the per-layer kernel (A/B timing).
@@ -740,40 +550,37 @@ inline bool tc_pdl_enabled() {
   return pdl != 0;
 }
 
-inline int tc_launch(TcConvParams& p, int n_tiles_n, cudaStream_t stream) {
-  if (p.bn % 16 != 0 || p.bn < 16 || p.bn > 256 || p.TW * p.TH != kTileM) return RAFT_ERR_BAD_SHAPE;
+inline int tc_check(const TcConvParams& p) {
+  if (p.bn % 16 != 0 || p.bn < 16 || p.bn > kMaxTileN || p.TW * p.TH != kTileM) return RAFT_ERR_BAD_SHAPE;
   if (p.mode != EPI_LINEAR && p.mode != EPI_GRU_ZR && p.mode != EPI_GRU_Q) return RAFT_ERR_UNSUPPORTED;
+  return RAFT_OK;
+}
+
+inline int tc_launch(TcConvParams& p, int n_tiles_n, cudaStream_t stream) {
+  RAFT_TRY(tc_check(p));
   if (p.stride < 1) p.stride = 1;
   const int smem = tc_finalize(p);
   if (p.nstages < 2) return RAFT_ERR_UNSUPPORTED;
-  // the attribute is per device: one bit per device ordinal (benign race: the calls are idempotent)
+  // the attribute and the SM count are per device: one entry per device ordinal (benign race: the calls are idempotent)
   int dev = 0;
   RAFT_CUDA_TRY(cudaGetDevice(&dev));
-  const unsigned long long dev_bit = 1ull << (dev & 63);
-  static unsigned long long attr_set_mask = 0;
-  if (!(attr_set_mask & dev_bit)) {
-    RAFT_CUDA_TRY(cudaFuncSetAttribute(conv_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    RAFT_CUDA_TRY(cudaFuncSetAttribute(conv_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    RAFT_CUDA_TRY(cudaFuncSetAttribute(conv_tc_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    attr_set_mask |= dev_bit;
+  static int num_sms[64] = {0};
+  if (!num_sms[dev & 63]) {
+    RAFT_CUDA_TRY(cudaFuncSetAttribute(conv_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax));
+    RAFT_CUDA_TRY(cudaDeviceGetAttribute(&num_sms[dev & 63], cudaDevAttrMultiProcessorCount, dev));
   }
   const int mtiles = p.B * p.tiles_y * p.tiles_x;
   p.n_tiles_n = n_tiles_n;
   const long ntiles = (long)mtiles * n_tiles_n;
-  const unsigned grid = (unsigned)(ntiles < kNumSMs ? ntiles : kNumSMs);   // one persistent CTA per SM
+  const unsigned grid = (unsigned)(ntiles < num_sms[dev & 63] ? ntiles : num_sms[dev & 63]);   // one persistent CTA per SM
   p.pdl = tc_pdl_enabled() ? 1 : 0;
-  const int threads = 64 + 32 * kEpiWarpsConv;
-  if (p.row3 && (p.mode != EPI_LINEAR || p.kh != 3 || p.kw != 3 || p.stride != 1 || p.TH != 1 || p.TW != kTileM || p.nseg != 1 ||
-                 p.bn % 8 != 0 || n_tiles_n != 1))
-    return RAFT_ERR_UNSUPPORTED;
-  void (*kern)(TcConvParams) = p.mode == EPI_GRU_Q ? conv_tc_kernel<false> : (p.row3 ? conv_tc_kernel<true, true> : conv_tc_kernel<true>);
   if (!p.pdl) {
-    kern<<<grid, threads, smem, stream>>>(p);
+    conv_tc_kernel<<<grid, kTcThreads, smem, stream>>>(p);
   } else {                                             // programmatic-serialization attribute: see the kernel prologue
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
     cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3((unsigned)threads);
+    cfg.blockDim = dim3((unsigned)kTcThreads);
     cfg.dynamicSmemBytes = (size_t)smem;
     cfg.stream = stream;
     cudaLaunchAttribute attr[1];
@@ -781,7 +588,7 @@ inline int tc_launch(TcConvParams& p, int n_tiles_n, cudaStream_t stream) {
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    RAFT_CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, p));
+    RAFT_CUDA_TRY(cudaLaunchKernelEx(&cfg, conv_tc_kernel, p));
   }
   return raft_launch_status();
 }

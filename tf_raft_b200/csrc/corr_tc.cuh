@@ -1,38 +1,31 @@
 // All-pairs correlation pyramid (tf_raft/layers/corr.py:100-114, 154-162) on the tensor cores: ONE persistent
-// warp-specialised tcgen05 kernel writes every level of the pyramid,
+// warp-specialised wgmma kernel writes every level of the pyramid,
 //
 //   pyr[l][b, q, n] = < fmap1[b, q, :], avgpool^l(fmap2)[b, n, :] > / sqrt(C)          (pooling is linear: the 256-channel
 //                                                                                       features are pooled, not the volume)
 // plus one preparation kernel that pools fmap2 and splits both feature maps into the fp16 (hi, lo) operand planes.
 //
 // Tile = 128 queries x bn <= 128 targets, K = C in 64-channel chunks of a 3-stage ring (64 KB stages), three fp16 passes
-// per chunk (hi*hi, lo*hi, hi*lo; fp32-grade, DESIGN.md section 4).  Accumulation chains are 24 MMAs long, exactly the
-// arithmetic of every other tensor-core layer: the K chunks are issued in groups of two, each group into its OWN 128-column
-// TMEM buffer, and the store warps add the group results in IEEE fp32 when they read them out ((0 + g0) + g1 + ...).  Four
-// TMEM buffers = two tiles in flight, so the MMAs of tile i+1 run while tile i is read out and stored.  (A single 48-MMA
-// chain per tile is inside the pyramid tolerance, but its ~1e-6 relative difference moved one query of the benchmark pair
-// across a discontinuity of the reference sampler at iteration 4 -- DESIGN.md section 4 -- so the chains stay at 24.)
-// Warp 0 = TMA producer, warp 1 = MMA issuer, warps 2..9 = read-out + store: each store warp owns 32 queries (its TMEM lane
-// quarter) x 64 columns, transposes 32 x 32 blocks through a swizzled 4 KB shared-memory patch and writes full 128-byte
-// lines of the pyramid rows.  The tile list runs over all levels (level 0 first), consecutive CTAs take consecutive query
-// tiles of the same target tile, so the target features are shared through L2.  Everything in the store path is inlined
-// and register-resident: the round-1 form of this epilogue lived in a non-inlined routine whose call made ptxas spill
-// accumulators to local memory (which, with 227 KB of the L1/shared array configured as shared memory, is an L2 round trip
-// per access).
+// per chunk (hi*hi, hi*lo, lo*hi; fp32-grade, DESIGN.md section 4).  Every chunk accumulates into a fresh register tile
+// (a 12-MMA chain) and the chunk results are added in IEEE fp32 ((0 + c0) + c1 + ...).  The pyramid feeds the sampler,
+// which is discontinuous at integer coordinates (DESIGN.md section 4), so the correlation takes the shortest chains:
+// with 24-MMA chains a query of the benchmark pair (448x512, seed 0/1) crosses a discontinuity at iteration 5 on the H100,
+// with 12 it stays within 3e-4 of the oracle.
+// Warps 0..7 = two consumer warpgroups (queries [0, 64) and [64, 128) of the tile): MMAs, then the scaled store straight
+// from the accumulator registers -- each lane writes 8-byte column pairs, a warp covers 8 rows x 32 contiguous bytes per
+// store, whole 32-byte sectors.  Warp 8 = TMA producer.  The tile list runs over all levels (level 0 first), consecutive
+// CTAs take consecutive query tiles of the same target tile, so the target features are shared through L2.
 #pragma once
 #include "conv_tc.cuh"
 #include "kernels.cuh"
 
 namespace raft {
 
-constexpr int kCorrStoreWarps = 8;
-constexpr int kCorrThreads = 64 + 32 * kCorrStoreWarps;
-constexpr int kCorrBn = 128;                                              // target columns per tile (one TMEM buffer)
+constexpr int kCorrBn = 128;                                              // target columns per tile
 constexpr int kCorrStageBytes = 2 * kABytes + 2 * kCorrBn * kChunkK * 2;  // 64 KB: A (hi|lo) 32 KB + B (hi|lo) up to 32 KB
 constexpr int kCorrStages = 3;
-constexpr int kCorrPatchBytes = kCorrStoreWarps * 4096;
-constexpr int kCorrSmemBytes = 1024 /*align slack*/ + kCorrStages * kCorrStageBytes + kCorrPatchBytes + 256 /*barriers*/;
-static_assert(kCorrSmemBytes <= 227 * 1024, "correlation kernel shared memory");
+constexpr int kCorrSmemBytes = 1024 /*align slack*/ + kCorrStages * kCorrStageBytes + 2048 /*MMA over-read, barriers*/;
+static_assert(kCorrSmemBytes <= kSmemMax, "correlation kernel shared memory");
 
 struct alignas(64) CorrTcParams {
   CUtensorMap a_map;                        // fmap1 (hi, lo): (C, N, 1, B, plane), box {64, 128, 1, 1, 2}
@@ -43,71 +36,109 @@ struct alignas(64) CorrTcParams {
   int levels, B, N, chunks;                 // chunks = C / 64
   int mtiles_img;                           // query tiles per image = ceil(N / 128)
   float corr_mul, corr_div;                 // 1/sqrt(C) when that is an exact power of two, else 0 and the divisor is used
-  long long* dbg;                           // optional clock64 timeline of CTA 0 (tools/timeline_corr.py): [4][512]
 };
 
-__global__ void __launch_bounds__(kCorrThreads, 1) corr_tc_kernel(const __grid_constant__ CorrTcParams p) {
+#if defined(__CUDA_ARCH__)
+// tile t -> (level, target tile, query tile): levels in order, query tile fastest
+__device__ __forceinline__ void corr_decode(const CorrTcParams& p, int t, int& l, int& nt, int& mt) {
+  l = 0;
+  while (l + 1 < p.levels && t >= p.tile0[l + 1]) ++l;
+  const int r = t - p.tile0[l];
+  const int mtiles = p.B * p.mtiles_img;
+  nt = r / mtiles;
+  mt = r - nt * mtiles;
+}
+
+template <int N>
+__device__ __forceinline__ void corr_consume_tile(const CorrTcParams& p, uint8_t* stages, uint64_t* full_bar, uint64_t* empty_bar,
+                                                  int& it, int wg, int tid, int l, int nt, int mt) {
+  const int lane = tid & 31, w = tid >> 5;
+  const int bn = p.bn[l], n2 = p.n2[l];
+  const uint32_t b_lo_off = (uint32_t)(bn * kChunkK * 2);
+  float acc[N / 2], racc[N / 2];
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) acc[i] = racc[i] = 0.0f;
+  for (int kc = 0; kc < p.chunks; ++kc, ++it) {
+    const int s = it % kCorrStages;
+    mbar_wait(&full_bar[s], (uint32_t)(it / kCorrStages) & 1u);
+    const uint32_t sa = smem_u32(stages + (size_t)s * kCorrStageBytes);
+    const uint32_t arow = (uint32_t)wg * 64 * 128;
+    wgmma_fence_regs(acc);
+    wgmma_fence();
+    wgmma_chunk3<N>(acc, make_desc_sw128(sa + arow), make_desc_sw128(sa + kABytes + arow), make_desc_sw128(sa + 2 * kABytes),
+                    make_desc_sw128(sa + 2 * kABytes + b_lo_off), true);
+    wgmma_commit();
+    wgmma_wait_all();
+    wgmma_fence_regs(acc);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty_bar[s]);
+#pragma unroll
+    for (int i = 0; i < N / 2; ++i) racc[i] += acc[i];     // IEEE fp32 sum of the 12-MMA chunk chains
+  }
+  // ---- store ----
+  const int b = mt / p.mtiles_img, m0 = (mt - b * p.mtiles_img) * kTileM, n0 = nt * bn;
+  const int col_end = min(n2, n0 + bn);
+  const bool vec = (n2 & 1) == 0;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int row = m0 + wg * 64 + 16 * w + (lane >> 2) + 8 * h;
+    if (row >= p.N) continue;
+    float* dst = p.out[l] + ((size_t)b * p.N + row) * n2;
+#pragma unroll
+    for (int i = 0; i < N / 8; ++i) {
+      const int col = n0 + 8 * i + 2 * (lane & 3);
+      float v0 = racc[4 * i + 2 * h], v1 = racc[4 * i + 2 * h + 1];
+      if (p.corr_mul != 0.0f) {
+        v0 *= p.corr_mul; v1 *= p.corr_mul;
+      } else {
+        v0 = __fdiv_rn(v0, p.corr_div); v1 = __fdiv_rn(v1, p.corr_div);
+      }
+      if (vec && col + 1 < col_end) {
+        *reinterpret_cast<float2*>(dst + col) = make_float2(v0, v1);
+      } else {
+        if (col < col_end) dst[col] = v0;
+        if (col + 1 < col_end) dst[col + 1] = v1;
+      }
+    }
+  }
+}
+#endif
+
+__global__ void __launch_bounds__(kTcThreads, 1) corr_tc_kernel(const __grid_constant__ CorrTcParams p) {
 #if defined(__CUDA_ARCH__)
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* stages = smem;
-  float* patches = reinterpret_cast<float*>(smem + kCorrStages * kCorrStageBytes);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kCorrStages * kCorrStageBytes + kCorrPatchBytes);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kCorrStages * kCorrStageBytes + 1024);   // (past the MMA over-read)
   uint64_t* empty_bar = full_bar + kCorrStages;
-  uint64_t* acc_full = empty_bar + kCorrStages;      // [2] issuer -> store warps: the buffer PAIR of a tile holds two groups
-  uint64_t* acc_empty = acc_full + 2;                // [2] store warps -> issuer: the pair has been read out
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(acc_empty + 2);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int mtiles = p.B * p.mtiles_img;
+  const int warp = threadIdx.x >> 5;
   const int ntiles = p.tile0[p.levels];
-  const int chunks = p.chunks;
-  const int npairs = (chunks + 3) >> 2;              // group pairs (4 K chunks) per tile: 1 for C <= 256
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     for (int s = 0; s < kCorrStages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&acc_full[i], 1);
-      mbar_init(&acc_empty[i], kCorrStoreWarps);
+      mbar_init(&empty_bar[s], kConsumerWarps);
     }
     fence_mbar_init();
     prefetch_tmap(&p.a_map);
     for (int l = 0; l < p.levels; ++l) prefetch_tmap(&p.b_map[l]);
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_holder, 512u);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_holder;
 
-  // tile t -> (level, target tile, query tile): levels in order, query tile fastest
-  auto decode = [&](int t, int& l, int& nt, int& mt) {
-    l = 0;
-    while (l + 1 < p.levels && t >= p.tile0[l + 1]) ++l;
-    const int r = t - p.tile0[l];
-    nt = r / mtiles;
-    mt = r - nt * mtiles;
-  };
-
-  if (warp == 0) {
+  if (warp >= kConsumerWarps) {
     // ===================== TMA producer =====================
-    if (elect_one()) {
+    regs_producer();
+    if (warp == kConsumerWarps && elect_one()) {
       int it = 0;
       for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
         int l, nt, mt;
-        decode(t, l, nt, mt);
+        corr_decode(p, t, l, nt, mt);
         const int b = mt / p.mtiles_img, m0 = (mt - b * p.mtiles_img) * kTileM, n0 = nt * p.bn[l];
         const uint32_t bytes = (uint32_t)(2 * kABytes + p.bn[l] * kChunkK * 4);
-        for (int kc = 0; kc < chunks; ++kc, ++it) {
+        for (int kc = 0; kc < p.chunks; ++kc, ++it) {
           const int s = it % kCorrStages;
           mbar_wait(&empty_bar[s], ((uint32_t)(it / kCorrStages) & 1u) ^ 1u);
-          if (p.dbg && blockIdx.x == 0 && it < 512) p.dbg[it] = clock64();
           uint8_t* st = stages + (size_t)s * kCorrStageBytes;
           mbar_arrive_expect_tx(&full_bar[s], bytes);
           tma_load_5d(st, &p.a_map, &full_bar[s], kc * kChunkK, m0, 0, b, 0);
@@ -115,148 +146,17 @@ __global__ void __launch_bounds__(kCorrThreads, 1) corr_tc_kernel(const __grid_c
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    int it = 0, uu = 0;                                // uu: uses of the buffer pairs (tile * npairs + pair)
+  } else {
+    // ===================== MMA + store (warpgroups 0, 1) =====================
+    regs_consumer();
+    const int wg = warp >> 2, tid = threadIdx.x & 127;
+    int it = 0;
     for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
       int l, nt, mt;
-      decode(t, l, nt, mt);
-      const int bn = p.bn[l];
-      const uint32_t idesc = make_idesc_f16(kTileM, bn);
-      const uint32_t b_lo_off = (uint32_t)(bn * kChunkK * 2);
-      int done = 0;
-      for (int gp = 0; gp < npairs; ++gp, ++uu) {
-        const int pr = uu & 1;                         // buffer pair: TMEM columns [256 pr, 256 pr + 256)
-        mbar_wait(&acc_empty[pr], ((uint32_t)(uu >> 1) & 1u) ^ 1u);          // store warps have read this pair out
-        tc_fence_after();
-        const int pend = min(chunks, done + 4);
-        for (; done < pend; ++done, ++it) {
-          const int s = it % kCorrStages;
-          const int g = (done >> 1) & 1;               // group inside the pair: chunks {0,1} -> buffer 0, {2,3} -> buffer 1
-          const uint32_t d_tmem = tmem_base + (uint32_t)(pr * 256 + g * 128);
-          const bool first = (done & 1) == 0;
-          mbar_wait(&full_bar[s], (uint32_t)(it / kCorrStages) & 1u);
-          tc_fence_after();
-          if (p.dbg && blockIdx.x == 0 && it < 512 && lane == 0) p.dbg[512 + it] = clock64();
-          if (elect_one()) {
-            const uint32_t sa = smem_u32(stages + (size_t)s * kCorrStageBytes);
-            const uint64_t a_hi = make_desc_sw128(sa), a_lo = make_desc_sw128(sa + kABytes);
-            const uint64_t b_hi = make_desc_sw128(sa + 2 * kABytes), b_lo = make_desc_sw128(sa + 2 * kABytes + b_lo_off);
-            umma_chunk3<false>(d_tmem, a_hi, a_lo, b_hi, b_lo, idesc, first != 0);
-            umma_commit(&empty_bar[s]);
-            if (done == pend - 1) umma_commit(&acc_full[pr]);
-          }
-          __syncwarp();
-        }
-      }
-    }
-  } else {
-    // ===================== read-out + store (warps 2..9) =====================
-    const int quarter = warp & 3;                    // TMEM lane quarter this warp may access
-    const int part = (warp - 2) >> 2;                // columns [part * 64, part * 64 + 64) of the tile
-    const uint32_t trow = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(part * 64);
-    float* patch = patches + (warp - 2) * 1024;
-    const int rsub = lane >> 3, q4 = lane & 7;
-    int uu = 0, tt = 0;
-    for (int t = blockIdx.x; t < ntiles; t += gridDim.x, ++tt) {
-      int l, nt, mt;
-      decode(t, l, nt, mt);
-      const int bn = p.bn[l], n2 = p.n2[l];
-      const int b = mt / p.mtiles_img, m0 = (mt - b * p.mtiles_img) * kTileM, n0 = nt * bn;
-      // 32-column blocks of this warp in this tile that hold columns of the level (warp-uniform)
-      const int nblk = max(0, min(2, (min(bn, n2 - n0) - part * 64 + 31) >> 5));
-
-      float racc[2][32];
-#pragma unroll
-      for (int ci = 0; ci < 2; ++ci)
-#pragma unroll
-        for (int j = 0; j < 32; ++j) racc[ci][j] = 0.0f;
-
-#pragma unroll 1
-      for (int gp = 0; gp < npairs; ++gp, ++uu) {
-        const int pr = uu & 1;
-        const int ng = min(2, ((chunks - 4 * gp) + 1) >> 1);               // groups in this pair (1 or 2)
-        mbar_wait(&acc_full[pr], (uint32_t)(uu >> 1) & 1u);
-        tc_fence_after();
-        if (p.dbg && blockIdx.x == 0 && gp == npairs - 1 && tt < 256 && warp == 2 && lane == 0) p.dbg[1024 + tt] = clock64();
-#pragma unroll
-        for (int g = 0; g < 2; ++g) {
-          if (g < ng) {
-#pragma unroll
-            for (int ci = 0; ci < 2; ++ci) {
-              if (ci < nblk) {
-                uint32_t r[32];
-                tmem_ld_32x32(trow + (uint32_t)(pr * 256 + g * 128 + ci * 32), r);
-                tmem_ld_wait();
-#pragma unroll
-                for (int j = 0; j < 32; ++j) racc[ci][j] += __uint_as_float(r[j]);   // IEEE fp32 sum of the 24-MMA groups
-              }
-            }
-          }
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&acc_empty[pr]);                        // the issuer may reuse the pair
-        if (p.dbg && blockIdx.x == 0 && gp == npairs - 1 && tt < 256 && warp == 2 && lane == 0) p.dbg[1536 + tt] = clock64();
-      }
-
-      // ---- store (the issuer is already two tiles ahead at most) ----
-      const int row_base = m0 + quarter * 32;                              // first query of this warp's 32 rows
-      float* dst0 = p.out[l] + ((size_t)b * p.N + row_base + rsub) * n2 + n0 + part * 64 + 4 * q4;
-      const int col_end = min(n2, n0 + bn);                                // bn need not be a multiple of 32: the last block
-                                                                           // of a tile stops at the tile's own last column
-      const bool vec = (n2 & 3) == 0 && (bn & 3) == 0;
-#pragma unroll
-      for (int ci = 0; ci < 2; ++ci) {
-        if (ci < nblk) {
-          __syncwarp();                                                    // previous block's readers are done with the patch
-#pragma unroll
-          for (int qq = 0; qq < 8; ++qq) {
-            float4 a4 = make_float4(racc[ci][4 * qq], racc[ci][4 * qq + 1], racc[ci][4 * qq + 2], racc[ci][4 * qq + 3]);
-            if (p.corr_mul != 0.0f) {
-              a4.x *= p.corr_mul; a4.y *= p.corr_mul; a4.z *= p.corr_mul; a4.w *= p.corr_mul;
-            } else {
-              a4.x = __fdiv_rn(a4.x, p.corr_div); a4.y = __fdiv_rn(a4.y, p.corr_div);
-              a4.z = __fdiv_rn(a4.z, p.corr_div); a4.w = __fdiv_rn(a4.w, p.corr_div);
-            }
-            *reinterpret_cast<float4*>(patch + lane * 32 + ((qq ^ (lane & 7)) << 2)) = a4;
-          }
-          __syncwarp();
-          const int col = n0 + part * 64 + ci * 32 + 4 * q4;
-          float* dst = dst0 + ci * 32;
-#pragma unroll
-          for (int i0 = 0; i0 < 8; i0 += 4) {                              // four 16-byte loads in flight, then four stores
-            float4 v[4];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const int rr = 4 * (i0 + i) + rsub;
-              v[i] = *reinterpret_cast<const float4*>(patch + rr * 32 + ((q4 ^ (rr & 7)) << 2));
-            }
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const int row = row_base + 4 * (i0 + i) + rsub;
-              if (row < p.N && col < col_end) {
-                float* d = dst + (size_t)(4 * (i0 + i)) * n2;
-                if (vec) {
-                  *reinterpret_cast<float4*>(d) = v[i];
-                } else {
-                  d[0] = v[i].x;
-                  if (col + 1 < col_end) d[1] = v[i].y;
-                  if (col + 2 < col_end) d[2] = v[i].z;
-                  if (col + 3 < col_end) d[3] = v[i].w;
-                }
-              }
-            }
-          }
-        }
-      }
-      if (p.dbg && blockIdx.x == 0 && warp == 2 && lane == 0 && tt < 255) p.dbg[1536 + 256 + tt] = clock64();
+      corr_decode(p, t, l, nt, mt);
+      with_mma_n(p.bn[l], [&](auto n) { corr_consume_tile<decltype(n)::value>(p, stages, full_bar, empty_bar, it, wg, tid, l, nt, mt); });
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, 512u);
 #endif
 }
 

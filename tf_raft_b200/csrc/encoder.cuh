@@ -190,9 +190,7 @@ struct EncCtx {
   int per_image;              // instance: one group per image; batch-training: one group
 };
 
-// y (npix, C) raw conv output -> normalised, activated, (+skip), re-split.  (Statistics partials from the convolution
-// epilogue and operand-swapped narrow layers were built and measured in round 2 -- both slower than this form
-// (profiles/README.md) -- and removed.)
+// y (npix, C) raw conv output -> normalised, activated, (+skip), re-split.
 inline int enc_norm_apply(const EncCtx& c, const EncNormSlot& ns, const float* y, size_t npix, int P, int relu,
                           const float* skip32, const __half* skip_hi, const __half* skip_lo, float* out32, __half* hi,
                           __half* lo) {
@@ -200,8 +198,8 @@ inline int enc_norm_apply(const EncCtx& c, const EncNormSlot& ns, const float* y
   const int Pg = c.per_image ? P : (int)npix;
   const float* gamma = reinterpret_cast<const float*>(c.prep + ns.gamma);
   const float* beta = reinterpret_cast<const float*>(c.prep + ns.beta);
-  // (Finalisation inside norm_stats_kernel by the last block of a group was measured twice -- +33 us per launch: the merge
-  //  of C channels by one block is serial where norm_final_kernel spreads it over G*C warps; profiles/README.md.)
+  // (Finalisation is a separate launch: inside norm_stats_kernel the merge of C channels by the last block of a group would
+  //  be serial, where norm_final_kernel spreads it over G*C warps.)
   norm_stats_kernel<<<dim3((unsigned)G, kNormSplit), 256, 0, c.st>>>(y, Pg, C, kNormSplit, c.W.part);
   norm_final_kernel<<<ceil_div(G * C * 32, 256), 256, 0, c.st>>>(c.W.part, G, C, kNormSplit, gamma, 1e-3f, c.W.mean, c.W.mult);
   norm_apply_kernel<<<grid_for(npix * (pad64(C) / 8)), 256, 0, c.st>>>(y, npix, P, C, c.per_image, c.W.mean, c.W.mult, beta, relu,
@@ -220,24 +218,12 @@ inline int enc_conv_tc(const EncCtx& c, const EncConvSlot& cs, const EncNormSlot
   int tw, th;
   tc_pick_tile(Wout, Hout, &tw, &th);
   if (tw * stride > 256) tw = 128 / stride, th = 128 / tw;
-  // Wide 3x3 stride-1 layers with few output channels (layer1 / layer2 of both encoders at >= 128 feature columns): one
-  // activation box and one weight box per kernel ROW (conv_tc.cuh kRow3).  RAFT_B200_ROW3=0 disables (A/B timing).
-  static const int row3_flag = [] { const char* e = getenv("RAFT_B200_ROW3"); return e ? atoi(e) : 1; }();
-  const bool row3 = row3_flag && cs.kh == 3 && cs.kw == 3 && stride == 1 && tw == kTileM && th == 1 && cs.cout_pad <= 96 &&
-                    cs.cout_pad % 8 == 0;
-  if (row3) {
-    RAFT_TRY(make_tmap_act2(&p.a_map[0], ahi, alo, c.N, Hin, Win, cs.cin_pad, kARow3Pixels, 1, 1));
-    RAFT_TRY(make_tmap_wgt3(&p.b_map, reinterpret_cast<const __half*>(c.prep + cs.hi),
-                            reinterpret_cast<const __half*>(c.prep + cs.lo), cs.kh * cs.kw, cs.cout_pad, cs.cin_pad, cs.cout_pad));
-    p.row3 = 1;
-    // (Keeping the nine taps of the 64-channel layers resident in shared memory was measured in round 2: slower, 489 vs 496
-    // pairs/s -- it leaves 68 KB of activation stages in flight against an HBM latency of ~3.1 k cycles.)
-  } else {
-    RAFT_TRY(make_tmap_act2(&p.a_map[0], ahi, alo, c.N, Hin, Win, cs.cin_pad, tw, th, stride));
-    RAFT_TRY(make_tmap_wgt2(&p.b_map, reinterpret_cast<const __half*>(c.prep + cs.hi),
-                            reinterpret_cast<const __half*>(c.prep + cs.lo), cs.kh * cs.kw, cs.cout_pad, cs.cin_pad,
-                            cs.cout_pad));
-  }
+  const int nsplit = tc_n_split(cs.cout_pad);          // layers wider than kMaxTileN run as more column tiles
+  if (!nsplit) return RAFT_ERR_BAD_SHAPE;
+  RAFT_TRY(make_tmap_act2(&p.a_map[0], ahi, alo, c.N, Hin, Win, cs.cin_pad, tw, th, stride));
+  RAFT_TRY(make_tmap_wgt2(&p.b_map, reinterpret_cast<const __half*>(c.prep + cs.hi),
+                          reinterpret_cast<const __half*>(c.prep + cs.lo), cs.kh * cs.kw, cs.cout_pad, cs.cin_pad,
+                          cs.cout_pad / nsplit));
   p.nseg = 1; p.seg_chunks[0] = cs.cin_pad / kChunkK; p.seg_c0[0] = 0;
   p.kh = cs.kh; p.kw = cs.kw; p.stride = stride;
   // Keras 'same': stride 1 -> (k-1)/2 before; stride 2 on even input -> total k-2, before = (k-2)/2 (0 for 3x3);
@@ -248,7 +234,7 @@ inline int enc_conv_tc(const EncCtx& c, const EncConvSlot& cs, const EncNormSlot
     p.ph = (tot_h > 0 ? tot_h : 0) / 2; p.pw = (tot_w > 0 ? tot_w : 0) / 2;
   }
   p.B = c.N; p.H = Hout; p.W = Wout; p.TH = th; p.TW = tw;
-  p.bn = cs.cout_pad; p.n_total = cs.cout;
+  p.bn = cs.cout_pad / nsplit; p.n_total = cs.cout;
   p.mode = EPI_LINEAR; p.out_scale = 1.0f;
   p.bias = reinterpret_cast<const float*>(c.prep + cs.bias);
   p.inv_scale = reinterpret_cast<const float*>(c.prep + cs.scale) + 1;
@@ -265,24 +251,18 @@ inline int enc_conv_tc(const EncCtx& c, const EncConvSlot& cs, const EncNormSlot
   } else {
     p.act = ACT_NONE; p.out_hi = nullptr; p.out_lo = nullptr;
   }
-  // (An L2 tensor prefetch of the next tile's activation boxes was measured in round 2: no effect, 494 vs 496 pairs/s -- the
-  //  ~3 k-cycle load latency of these layers is TMA service time, not HBM latency; profiles/README.md.)
   if (g_dbg_layer >= 1000 && g_dbg_count++ == g_dbg_layer - 1000) p.dbg = g_dbg_buf;   // timeline of the k-th encoder conv
   {
-    // Promotion group of the encoder convolutions: their contractions are short (K <= 1152, 18 chunks), so the fp32
-    // accumulator may stay in TMEM for 5 chunks (60 MMA steps) between IEEE promotions instead of the update block's 2
-    // (its K = 1920 GRU contractions feed a 12-iteration recurrence).  Measured: 433 -> 447 pairs/s, parity tests green.
+    // Promotion group of the encoder convolutions: their contractions are short (K <= 1152, 18 chunks), so the tensor-core
+    // accumulator may run for 5 chunks (60 MMA steps) between IEEE promotions instead of the update block's 2 (its
+    // K = 1920 GRU contractions feed a 12-iteration recurrence).
     static const int grp = [] { const char* e = getenv("RAFT_B200_ENC_GROUP"); return e ? atoi(e) : 5; }();
     if (grp > 0) p.group_chunks = grp;
-    if (row3) p.group_chunks = 2;       // a kRow3 stage carries three taps: 2 stages = 72 MMA steps per accumulation chain
   }
   ++g_launches;
-  return tc_launch(p, 1, c.st);
+  return tc_launch(p, nsplit, c.st);
 }
 
-// (Processing a large batch in groups of 2 or 4 images, so that a group's raw convolution output stays in L2 between the
-// convolution, the statistics pass and the normalise pass, was measured in round 2: 408 / 456 vs 482 pairs/s -- the
-// smaller launches cost more than the L2 hits save -- and removed.)
 inline int encoder_forward(int variant, int norm_type, int out_dim, const void* prepared, const float* images, int N,
                            int H, int W, int training, int image_norm, float* out, void* ws, size_t ws_bytes, cudaStream_t st) {
   EncCtx c;

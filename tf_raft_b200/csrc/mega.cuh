@@ -1,30 +1,25 @@
 // update_mega_kernel: every tensor-core layer of one update-block application (tf_raft/layers/update.py:143-153 -- motion
-// encoder, SepConvGRU / ConvGRU, flow head, mask head) in ONE persistent warp-specialised tcgen05 kernel.
+// encoder, SepConvGRU / ConvGRU, flow head, mask head) in ONE persistent warp-specialised wgmma kernel.
 //
-// The per-layer kernel (conv_tc.cuh) is launched 11 times per iteration; each launch pays its prologue (barriers, TMEM
-// allocation, first TMA round trip), exposes its 13-19 k-cycle epilogue with no next tile to hide behind (112 tiles on
-// 148 SMs at batch 4) and leaves a quarter of the chip idle.  Here the work list is (layer, tile) for all layers of the
-// block, in layer order; CTA c of the 148 walks items c, c + 148, ... with the same three roles as conv_tc_kernel:
-//   warp 0  TMA producer: before the first load of an item it waits for the tiles of the SOURCE layer(s) that cover the
-//           item's halo -- a per-(layer, tile) counter in global memory that the 16 epilogue warps of the producing CTA
-//           increment (release) after their stores -- then streams (tap, 64-channel chunk) stages as before;
-//   warp 1  single-thread tcgen05.mma issuer, ping-pong TMEM accumulators, IEEE-fp32 promotion groups of 2 chunks;
-//   warps 2..17  promotion + fused epilogue of the layer's mode (bias / ReLU / GRU gates / hi-lo re-split), then the
-//           item's completion counter.
-// The shared-memory ring and the TMEM buffers run straight across items, so the epilogue of one item overlaps the loads
-// and MMAs of the next (of another layer), and all 148 SMs stay busy.  Dependencies always point to earlier items of
-// the list and every CTA consumes its items in list order, so with all CTAs co-resident (1 per SM) the wait graph is
-// acyclic.  Activations written by generic-proxy stores and read back by TMA (async proxy) are ordered by
-// fence.proxy.async on both sides of the release / acquire pair; z and h, which epilogues re-read with ordinary loads,
-// are read through L2 (ld.global.cg).
+// The per-layer kernel (conv_tc.cuh) is launched 11 times per iteration; each launch pays its prologue and exposes its
+// epilogue with no next tile to hide behind.  Here the work list is (layer, tile) for all layers of the block, in layer
+// order; the CTAs (one per SM) claim items in list order with the same roles as conv_tc_kernel:
+//   warp 8  TMA producer: claims the items; before the first load of an item it waits for the tiles of the SOURCE
+//           layer(s) that cover the item's halo -- a per-(layer, tile) counter in global memory that the 8 consumer warps
+//           of the producing CTA increment (release) after their stores -- then streams (tap, 64-channel chunk) stages;
+//   warps 0..7  two consumer warpgroups: wgmma MMAs with IEEE-fp32 promotion groups, the fused epilogue of the layer's
+//           mode (bias / ReLU / GRU gates / hi-lo re-split), then the item's completion counter.
+// The shared-memory ring runs straight across items, so the epilogue of one item overlaps the loads of the next (of
+// another layer).  Dependencies always point to earlier items of the list and every CTA consumes its items in list
+// order, so with all CTAs co-resident (1 per SM) the wait graph is acyclic.  Activations written by generic-proxy stores
+// and read back by TMA (async proxy) are ordered by fence.proxy.async on both sides of the release / acquire pair; z and
+// h, which epilogues re-read with ordinary loads, are read through L2 (ld.global.cg).
 #pragma once
 #include "conv_tc.cuh"
 
 namespace raft {
 
 constexpr int kMegaMaxLayers = 14;
-constexpr int kMegaEpiWarps = 16;
-constexpr int kMegaThreads = 64 + 32 * kMegaEpiWarps;
 constexpr int kMegaMaxStages = 8;
 
 struct alignas(64) MegaLayer {
@@ -33,7 +28,7 @@ struct alignas(64) MegaLayer {
   int flag0;                      // first completion counter of this layer (n_tiles_n * pixel tiles of them)
   int ndep;
   int dep_layer[2];               // source layers (positions in MegaParams::layer)
-  int dep_ntile[2];               // column tile of the source that is read (-1: all of them)
+  int dep_nlo[2], dep_nhi[2];     // column tiles of the source that are read
   int dep_ry, dep_rx;             // halo of the dependency in tiles (>= 1: also covers the write-after-read hazards)
 };
 
@@ -42,10 +37,8 @@ struct alignas(64) MegaParams {
   int nlayers, nitems;
   unsigned int* flags;            // zeroed before the launch
   unsigned int* next_item;        // work-list cursor (zeroed with the flags): CTAs claim items with atomicAdd
-  long long* dbg;                 // optional schedule trace (tools/timeline_mega.py): [CTA][kMegaDbgItems][8] globaltimer stamps
 };
-constexpr int kMegaDbgItems = 16;
-constexpr int kMegaQueue = 16;    // per-CTA ring of claimed item numbers (producer -> issuer / epilogue warps)
+constexpr int kMegaQueue = 16;    // per-CTA ring of claimed item numbers (producer -> consumers)
 
 #if defined(__CUDA_ARCH__)
 __device__ __forceinline__ unsigned int ld_acquire_gpu(const unsigned int* p) {
@@ -57,152 +50,78 @@ __device__ __forceinline__ void red_release_gpu_add(unsigned int* p, unsigned in
   asm volatile("red.release.gpu.global.add.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
 __device__ __forceinline__ void fence_proxy_async_all() { asm volatile("fence.proxy.async;" ::: "memory"); }
-// schedule trace: compiled in only with -DRAFT_MEGA_TRACE (tools/timeline_mega.py loads such a build through RAFT_B200_LIB)
-#ifdef RAFT_MEGA_TRACE
-#define MEGA_STAMP(i) do { if (dbg) dbg[i] = global_ns(); } while (0)
-#else
-#define MEGA_STAMP(i) do { } while (0)
-#endif
-__device__ __forceinline__ long long global_ns() {
-  long long t;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-  return t;
-}
 
-template <bool kPair>
-__device__ __forceinline__ void mega_wait_q(uint64_t* bar, uint32_t parity) {     // item-number queue: filled by the leader CTA
-  if constexpr (kPair) mbar_wait_cluster(bar, parity); else mbar_wait(bar, parity);
-}
-// pair > 0: the item is a PAIR of consecutive pixel tiles (2j, 2j + 1) of one column tile; `rank` picks this CTA's half.
-__device__ __forceinline__ void mega_decode(const MegaParams& P, int item, int& L, int& nt, int& b, int& ty, int& tx, int pair = 0,
-                                            int rank = 0) {
-  L = 0;
+__device__ __forceinline__ int mega_layer_of(const MegaParams& P, int item) {
+  int L = 0;
   while (L + 1 < P.nlayers && item >= P.layer[L + 1].item0) ++L;
-  const TcConvParams& c = P.layer[L].c;
-  const int mtiles = c.B * c.tiles_y * c.tiles_x;
-  const int units = pair ? mtiles >> 1 : mtiles;
-  const int r = item - P.layer[L].item0;
-  nt = r / units;
-  int mt = r - nt * units;
-  if (pair) mt = 2 * mt + rank;
-  tx = mt % c.tiles_x;
-  mt /= c.tiles_x;
-  ty = mt % c.tiles_y;
-  b = mt / c.tiles_y;
+  return L;
 }
 #endif
 
-// kPair: launched in clusters of two CTAs; an item is a pair of pixel tiles computed by ONE M = 256 MMA stream
-// (tcgen05 cta_group::2) issued by the leader CTA.  Each CTA stages its own activation rows and half of the weight rows, so
-// the weights -- two thirds of the operand bytes of the 256-column layers -- cross the L2 -> SM fabric once per pair instead
-// of once per tile.  Everything downstream of the accumulators (promotion, epilogue, completion counters) is per CTA and
-// identical in both forms; so are the sums (same K order per accumulator).
-template <bool kPair>
-__global__ void __launch_bounds__(kMegaThreads, 1) update_mega_kernel(const __grid_constant__ MegaParams P) {
+__global__ void __launch_bounds__(kTcThreads, 1) update_mega_kernel(const __grid_constant__ MegaParams P) {
 #if defined(__CUDA_ARCH__)
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  constexpr int kRingBytes = kSmemBudget - kEpiPatchBytes - 1024;           // stages of the current layer live here
+  constexpr int kRingBytes = kSmemMax - kSmemFixed;                         // stages of the current layer live here
   uint8_t* stages = smem;
-  float* patches = reinterpret_cast<float*>(smem + kRingBytes);             // 16 x 2 KB transposition patches (GRU q)
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kRingBytes + kEpiPatchBytes);
+  float* staging = reinterpret_cast<float*>(smem + kRingBytes);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kRingBytes + kStagingBytes);
   uint64_t* empty_bar = full_bar + kMegaMaxStages;
-  uint64_t* acc_full = empty_bar + kMegaMaxStages;      // [2] issuer -> promotion warps
-  uint64_t* acc_empty = acc_full + 2;                   // [2] promotion warps -> issuer
-  uint64_t* q_bar = acc_empty + 2;                      // [kMegaQueue] producer -> consumers: item number published
+  uint64_t* q_bar = empty_bar + kMegaMaxStages;         // [kMegaQueue] producer -> consumers: item number published
   int* item_q = reinterpret_cast<int*>(q_bar + kMegaQueue);
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(item_q + kMegaQueue);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int rank = kPair ? (int)cluster_ctarank() : 0;       // 0 = leader: claims the items and issues the MMAs
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     for (int s = 0; s < kMegaMaxStages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&acc_full[i], 1);
-      mbar_init(&acc_empty[i], kMegaEpiWarps * (kPair ? 2 : 1));   // every epilogue warp (of both CTAs) arrives
+      mbar_init(&empty_bar[s], kConsumerWarps);
     }
     for (int i = 0; i < kMegaQueue; ++i) mbar_init(&q_bar[i], 1);
     fence_mbar_init();
   }
-  if (warp == 2 && lane < P.nlayers) {                   // descriptor fetches off the first stage of every layer
+  if (warp == 0 && lane < P.nlayers) {                   // descriptor fetches off the first stage of every layer
     const TcConvParams& c = P.layer[lane].c;
     prefetch_tmap(&c.a_map[0]);
     if (c.nseg > 1) prefetch_tmap(&c.a_map[1]);
     prefetch_tmap(&c.b_map);
   }
-  if (warp == 1) {
-    if constexpr (kPair) {
-      tmem2_alloc(tmem_holder, 512u);
-      tmem2_relinquish();
-    } else {
-      tmem_alloc(tmem_holder, 512u);
-      tmem_relinquish();
-    }
-  }
-  tc_fence_before();
-  if constexpr (kPair) cluster_sync_all(); else __syncthreads();   // (pair: the peer's barriers exist before anything targets them)
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_holder;
+  __syncthreads();
 
-  if (warp == 0) {
+  if (warp >= kConsumerWarps) {
     // ===================== TMA producer =====================
-    if (elect_one()) {
-      uint32_t par = 0, used = 0;          // per ring slot: parity of its use count, used since the last drain
-      int slot = 0, cur_nst = 0, cur_bytes = 0;
-      // (One producer thread and one issuer thread.  Round-robin producer warps, a separate weight-producer warp and two
-      //  MMA-issuing warps on alternate promotion groups were all built, validated bit-identical and measured within +-2 % of
-      //  this form -- profiles/README.md "what bounds the mainloop": shared-memory bandwidth, not issue.  Lesson kept from the
-      //  multi-warp forms: a thread that waits on the parity of a barrier must wait for EVERY phase of it, in order; skipping
-      //  the phases that belong to another warp lets a parity wait return one phase early, or never.)
+    regs_producer();
+    if (warp == kConsumerWarps && elect_one()) {
+      RingPos rp{0, 0u};
+      int cur_nst = 0, cur_bytes = 0;
       // Items are CLAIMED, not pre-assigned: a CTA that becomes free takes the lowest unclaimed item of the list (layer
       // order = priority order), so no CTA sits on a blocked item while a runnable one waits behind it in a fixed
       // per-CTA sequence.  Every dependency points to a lower item number, which some co-resident CTA has already claimed,
-      // so the wait graph stays acyclic.  The claimed number is handed to the other roles through item_q / q_bar.
-      int item = rank == 0 ? (int)atomicAdd(P.next_item, 1u) : 0;
+      // so the wait graph stays acyclic.  The claimed number is handed to the consumers through item_q / q_bar.
+      int item = (int)atomicAdd(P.next_item, 1u);
       for (int k = 0;; ++k) {
         const int qs = k & (kMegaQueue - 1);
-        if (rank == 0) {
-          const int pub = item < P.nitems ? item : -1;
-          item_q[qs] = pub;
-          mbar_arrive(&q_bar[qs]);                       // (release: the slot's item number is visible to the waiters)
-          if constexpr (kPair) {                         // ... and to the three roles of the peer CTA
-            st_cluster_u32(mapa_u32(smem_u32(&item_q[qs]), 1), (uint32_t)pub);
-            mbar_arrive_cluster(mapa_u32(smem_u32(&q_bar[qs]), 1));
-          }
-        } else {
-          mega_wait_q<kPair>(&q_bar[qs], (uint32_t)(k / kMegaQueue) & 1u);
-          item = item_q[qs];
-          if (item < 0) item = P.nitems;
-        }
+        item_q[qs] = item < P.nitems ? item : -1;
+        mbar_arrive(&q_bar[qs]);                         // (release: the slot's item number is visible to the waiters)
         if (item >= P.nitems) break;
-#ifdef RAFT_MEGA_TRACE
-        long long* dbg = (P.dbg && k < kMegaDbgItems) ? P.dbg + ((size_t)blockIdx.x * kMegaDbgItems + k) * 8 : nullptr;
-        if (dbg) { dbg[0] = item + 1; dbg[1] = global_ns(); }
-#endif
-        int nxt = P.nitems;
-        int L, nt, b, ty, tx;
-        mega_decode(P, item, L, nt, b, ty, tx, kPair, rank);
+        const int L = mega_layer_of(P, item);
         const MegaLayer& ML = P.layer[L];
         const TcConvParams& c = ML.c;
+        int nt, b, ty, tx;
+        tc_decode_tile(c, item - ML.item0, nt, b, ty, tx);
         // ---- dependencies: tiles of the source layers that cover this tile's halo ----
         if (ML.ndep > 0) {
           const int mtiles = c.B * c.tiles_y * c.tiles_x;
           for (int d = 0; d < ML.ndep; ++d) {
             const MegaLayer& SL = P.layer[ML.dep_layer[d]];
-            const int n_lo = ML.dep_ntile[d] < 0 ? 0 : ML.dep_ntile[d];
-            const int n_hi = ML.dep_ntile[d] < 0 ? SL.c.n_tiles_n - 1 : ML.dep_ntile[d];
-            for (int n = n_lo; n <= n_hi; ++n)
+            for (int n = ML.dep_nlo[d]; n <= ML.dep_nhi[d]; ++n)
               for (int yy = max(0, ty - ML.dep_ry); yy <= min(c.tiles_y - 1, ty + ML.dep_ry); ++yy)
                 for (int xx = max(0, tx - ML.dep_rx); xx <= min(c.tiles_x - 1, tx + ML.dep_rx); ++xx) {
                   const unsigned int* f = P.flags + SL.flag0 + n * mtiles + (b * c.tiles_y + yy) * c.tiles_x + xx;
-                  if (ld_acquire_gpu(f) < (unsigned)kMegaEpiWarps) {
+                  if (ld_acquire_gpu(f) < (unsigned)kConsumerWarps) {
                     const long long t0 = clock64();
-                    while (ld_acquire_gpu(f) < (unsigned)kMegaEpiWarps) {
+                    while (ld_acquire_gpu(f) < (unsigned)kConsumerWarps) {
                       __nanosleep(64);
                       if (clock64() - t0 > 8000000000LL) __trap();        // protocol bug -> trapped kernel, never a hang
                     }
@@ -211,232 +130,41 @@ __global__ void __launch_bounds__(kMegaThreads, 1) update_mega_kernel(const __gr
           }
           fence_proxy_async_all();          // acquired generic-proxy writes -> visible to the TMA loads issued below
         }
-        MEGA_STAMP(2);
         // ---- ring geometry: a layer with another stage size re-carves the ring once it has drained ----
         if (c.nstages != cur_nst || c.stage_bytes != cur_bytes) {
-          for (int s = 0; s < kMegaMaxStages; ++s)
-            if ((used >> s) & 1u) mbar_wait(&empty_bar[s], ((par >> s) & 1u) ^ 1u);   // MMAs of the slot's last use retired
-          used = 0;
-          slot = 0;
+          for (int s = 0; s < kMegaMaxStages; ++s)        // the last use of every slot has been consumed (an unused slot
+            mbar_wait(&empty_bar[s], ((rp.par >> s) & 1u) ^ 1u);   // passes at once: its parity wait names a past phase)
+          rp.slot = 0;
           cur_nst = c.nstages;
           cur_bytes = c.stage_bytes;
         }
-        MEGA_STAMP(3);
-        const int ntaps = c.kh * c.kw;
-        const int x0 = tx * c.TW * c.stride, y0 = ty * c.TH * c.stride, n0 = nt * c.bn;
-        int left = ntaps * (c.seg_chunks[0] + (c.nseg > 1 ? c.seg_chunks[1] : 0));
-        for (int tap = 0; tap < ntaps; ++tap) {
-          const int dy = tap / c.kw - c.ph, dx = tap % c.kw - c.pw;
-          int kc = 0;
-          for (int seg = 0; seg < c.nseg; ++seg) {
-            for (int ch = 0; ch < c.seg_chunks[seg]; ++ch, ++kc) {
-              // claim the next item while the last stage of this one is still to be loaded: late enough that the CTA is
-              // about to be free, early enough that the atomic's round trip hides behind the slot wait below
-              if (--left == 0 && rank == 0) nxt = (int)atomicAdd(P.next_item, 1u);
-              const int s = slot;
-              slot = slot + 1 == cur_nst ? 0 : slot + 1;
-              mbar_wait(&empty_bar[s], ((par >> s) & 1u) ^ 1u);
-              par ^= 1u << s;
-              used |= 1u << s;
-              uint8_t* st = stages + (size_t)s * cur_bytes;
-              if constexpr (kPair) {
-                // both CTAs' boxes complete on the LEADER's barrier, which expects the bytes of both stages
-                if (rank == 0) mbar_arrive_expect_tx(&full_bar[s], (uint32_t)(2 * cur_bytes));
-                const uint32_t lead = mapa_u32(smem_u32(&full_bar[s]), 0);
-                tma2_load_5d(st, &c.a_map[seg], lead, c.seg_c0[seg] + ch * kChunkK, x0 + dx, y0 + dy, b, 0);
-                tma2_load_4d(st + 2 * kABytes, &c.b_map, lead, kc * kChunkK, n0 + rank * (c.bn >> 1), tap, 0);
-              } else {
-                mbar_arrive_expect_tx(&full_bar[s], (uint32_t)cur_bytes);
-                tma_load_5d(st, &c.a_map[seg], &full_bar[s], c.seg_c0[seg] + ch * kChunkK, x0 + dx, y0 + dy, b, 0);
-                tma_load_4d(st + 2 * kABytes, &c.b_map, &full_bar[s], kc * kChunkK, n0, tap, 0);
-              }
-            }
-          }
-        }
-        MEGA_STAMP(4);
+        int nxt = P.nitems;
+        tc_produce_tile(c, stages, full_bar, empty_bar, rp, nt, b, ty, tx, P.next_item, &nxt);
         item = nxt;
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    uint32_t par = 0;
-    int slot = 0, cur_nst = 0, cur_bytes = 0, gg = 0;
-    for (int k = 0; rank == 0; ++k) {                    // (pair: the leader issues for both CTAs; the peer's warp 1 only
-      mega_wait_q<kPair>(&q_bar[k & (kMegaQueue - 1)], (uint32_t)(k / kMegaQueue) & 1u);   //  owns its half of the TMEM allocation)
+  } else {
+    // ===================== MMA + epilogue (warpgroups 0, 1) =====================
+    regs_consumer();
+    const int wg = warp >> 2, tid = threadIdx.x & 127;
+    RingPos rp{0, 0u};
+    int cur_nst = 0, cur_bytes = 0;
+    for (int k = 0;; ++k) {
+      mbar_wait(&q_bar[k & (kMegaQueue - 1)], (uint32_t)(k / kMegaQueue) & 1u);
       const int item = item_q[k & (kMegaQueue - 1)];
       if (item < 0) break;
-      int L, nt, b, ty, tx;
-      mega_decode(P, item, L, nt, b, ty, tx, kPair, 0);
-      const TcConvParams& c = P.layer[L].c;
+      const MegaLayer& ML = P.layer[mega_layer_of(P, item)];
+      const TcConvParams& c = ML.c;
       if (c.nstages != cur_nst || c.stage_bytes != cur_bytes) {
-        slot = 0;
+        rp.slot = 0;
         cur_nst = c.nstages;
         cur_bytes = c.stage_bytes;
       }
-      const uint32_t idesc = make_idesc_f16(kPair ? 2 * kTileM : kTileM, c.bn);
-      const uint32_t b_bytes = (uint32_t)((kPair ? c.bn >> 1 : c.bn) * kChunkK * 2);   // rows of B staged by this CTA
-      const int total = c.kh * c.kw * (c.seg_chunks[0] + (c.nseg > 1 ? c.seg_chunks[1] : 0));
-      const int gsz = c.group_chunks;
-      int done = 0;
-      while (done < total) {
-        const int buf = gg & 1;
-        mbar_wait(&acc_empty[buf], ((uint32_t)(gg >> 1) & 1u) ^ 1u);       // promotion warps drained this buffer
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(buf * 256);
-        const int gend = min(total, done + gsz);
-        for (int first = 1; done < gend; ++done, first = 0) {
-          const int s = slot;
-          slot = slot + 1 == cur_nst ? 0 : slot + 1;
-          mbar_wait(&full_bar[s], (par >> s) & 1u);
-          par ^= 1u << s;
-          tc_fence_after();
-          if (elect_one()) {
-            const uint32_t sa = smem_u32(stages + (size_t)s * cur_bytes);
-            const uint64_t a_hi = make_desc_sw128(sa), a_lo = make_desc_sw128(sa + kABytes);
-            const uint64_t b_hi = make_desc_sw128(sa + 2 * kABytes), b_lo = make_desc_sw128(sa + 2 * kABytes + b_bytes);
-            if constexpr (kPair) {
-              umma_chunk3<true>(d_tmem, a_hi, a_lo, b_hi, b_lo, idesc, first != 0);
-              umma2_commit(&empty_bar[s]);                     // frees the slot in BOTH CTAs once these MMAs retire
-              if (done == gend - 1) umma2_commit(&acc_full[buf]);   // group complete -> promotion warps of both CTAs
-            } else {
-              umma_chunk3<false>(d_tmem, a_hi, a_lo, b_hi, b_lo, idesc, first != 0);
-              umma_commit(&empty_bar[s]);                      // frees the smem slot once these MMAs retire
-              if (done == gend - 1) umma_commit(&acc_full[buf]);   // group complete -> promotion warps
-            }
-          }
-          __syncwarp();
-        }
-        ++gg;
-      }
-    }
-  } else {
-    // ===================== promotion + epilogue (warps 2..17) =====================
-    constexpr int kParts = kMegaEpiWarps / 4;        // warps per TMEM lane quarter: each takes a slice of the columns
-    constexpr int kMaxCh = 8 / kParts;               // 32-column accumulator chunks per thread (2)
-    const int quarter = warp & 3;                    // TMEM lane quarter this warp may access
-    const int part_id = (warp - 2) >> 2;
-    const int m = quarter * 32 + lane;               // tile row == TMEM lane
-    const uint32_t trow = tmem_base + ((uint32_t)(quarter * 32) << 16);
-    int gg = 0;
-    for (int k = 0;; ++k) {
-      mega_wait_q<kPair>(&q_bar[k & (kMegaQueue - 1)], (uint32_t)(k / kMegaQueue) & 1u);
-      const int item = item_q[k & (kMegaQueue - 1)];
-      if (item < 0) break;
-      int L = 0;
-      while (L + 1 < P.nlayers && item >= P.layer[L + 1].item0) ++L;
-      const MegaLayer& ML = P.layer[L];
-      const TcConvParams& c = ML.c;
-      const int nchunks32 = (c.bn + 31) >> 5;
-      const int chunks_per_part = (nchunks32 + kParts - 1) / kParts;
-      const int chunk0 = part_id * chunks_per_part;
-      const int my_chunks = max(0, min(chunks_per_part, nchunks32 - chunk0));
-      const int total = c.kh * c.kw * (c.seg_chunks[0] + (c.nseg > 1 ? c.seg_chunks[1] : 0));
-      const int ngroups = (total + c.group_chunks - 1) / c.group_chunks;
-
-      float racc[kMaxCh][32];
-#pragma unroll
-      for (int ci = 0; ci < kMaxCh; ++ci)
-#pragma unroll
-        for (int j = 0; j < 32; ++j) racc[ci][j] = 0.0f;
-
-#ifdef RAFT_MEGA_TRACE
-      long long* dbg = (P.dbg && k < kMegaDbgItems && warp == 2 && lane == 0) ? P.dbg + ((size_t)blockIdx.x * kMegaDbgItems + k) * 8 : nullptr;
-#endif
-#pragma unroll 1
-      for (int g = 0; g < ngroups; ++g, ++gg) {
-        const int buf = gg & 1;
-        mbar_wait(&acc_full[buf], (uint32_t)(gg >> 1) & 1u);
-        tc_fence_after();
-        if (g == 0) MEGA_STAMP(5);
-#pragma unroll
-        for (int ci = 0; ci < kMaxCh; ++ci) {
-          if (ci < my_chunks) {
-            const int c0 = (chunk0 + ci) * 32;
-#pragma unroll
-            for (int hh = 0; hh < 4; ++hh) {             // 8 columns at a time: the 64 accumulators leave few registers
-              if (c0 + hh * 8 < c.bn) {                  // (bn is a multiple of 16)
-                uint32_t r[8];
-                tmem_ld_32x8(trow + (uint32_t)(buf * 256 + c0 + hh * 8), r);
-                tmem_ld_wait();
-#pragma unroll
-                for (int j = 0; j < 8; ++j) racc[ci][hh * 8 + j] += __uint_as_float(r[j]);   // IEEE fp32 promotion
-              }
-            }
-          }
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) {
-          if (kPair && rank != 0) mbar_arrive_cluster(mapa_u32(smem_u32(&acc_empty[buf]), 0));   // the issuer lives in the leader
-          else mbar_arrive(&acc_empty[buf]);
-        }
-      }
-
-      MEGA_STAMP(6);
-      // ---- epilogue of this item (the issuer is already accumulating the next one) ----
-      // (tile coordinates are decoded here, not before the promotion loop: 64 accumulators leave few registers to carry them)
       int nt, b, ty, tx;
-      {
-        const int mtiles = c.B * c.tiles_y * c.tiles_x;
-        const int units = kPair ? mtiles >> 1 : mtiles;
-        const int r = item - ML.item0;
-        nt = r / units;
-        int mt = r - nt * units;
-        if (kPair) mt = 2 * mt + rank;
-        tx = mt % c.tiles_x;
-        mt /= c.tiles_x;
-        ty = mt % c.tiles_y;
-        b = mt / c.tiles_y;
-      }
-      const float inv_scale = c.inv_scale ? __ldg(c.inv_scale) : 1.0f;
-      const int xl = m % c.TW, yl = m / c.TW;
-      const int x = tx * c.TW + xl, y = ty * c.TH + yl;
-      if (c.mode != EPI_GRU_Q) {           // thread-per-row register epilogue (EPI_LINEAR, EPI_GRU_ZR)
-        if (x < c.W && y < c.H) {
-          const size_t pix = ((size_t)b * c.H + y) * c.W + x;
-#pragma unroll
-          for (int ci = 0; ci < kMaxCh; ++ci) {
-            if (ci < my_chunks) {
-              const int c0 = (chunk0 + ci) * 32;
-              const int ncol = min(32, c.bn - c0);
-              if (c.mode == EPI_LINEAR) tc_epilogue_regs<EPI_LINEAR>(c, racc[ci], pix, nt * c.bn + c0, ncol, inv_scale);
-              else tc_epilogue_regs<EPI_GRU_ZR>(c, racc[ci], pix, nt * c.bn + c0, ncol, inv_scale);
-            }
-          }
-        }
-      } else {                             // EPI_GRU_Q: coalesced epilogue through a 32 x 16 transposition patch
-        float4* patch4 = reinterpret_cast<float4*>(patches + (warp - 2) * 512);
-        const int pix_own = (x < c.W && y < c.H) ? (int)(((size_t)b * c.H + y) * c.W + x) : -1;
-        int pixr[4];
-#pragma unroll
-        for (int k = 0; k < 4; ++k) pixr[k] = __shfl_sync(0xffffffffu, pix_own, (lane >> 2) + 8 * k);
-        const int c4 = lane & 3;
-        const int wsw = (lane >> 1) & 3, rsw = (lane >> 3) & 3;   // XOR swizzles: conflict-free 16-byte writes and reads
-#pragma unroll
-        for (int ci = 0; ci < kMaxCh; ++ci) {
-          if (ci < my_chunks) {
-#pragma unroll
-            for (int hh = 0; hh < 2; ++hh) {
-              const int c0 = (chunk0 + ci) * 32 + hh * 16;
-              if (c0 < c.bn) {
-                __syncwarp();
-#pragma unroll
-                for (int q = 0; q < 4; ++q)
-                  patch4[lane * 4 + (q ^ wsw)] = make_float4(racc[ci][hh * 16 + 4 * q], racc[ci][hh * 16 + 4 * q + 1],
-                                                             racc[ci][hh * 16 + 4 * q + 2], racc[ci][hh * 16 + 4 * q + 3]);
-                __syncwarp();
-                float v[4][4];
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                  const float4 t4 = patch4[((lane >> 2) + 8 * k) * 4 + (c4 ^ rsw)];
-                  v[k][0] = t4.x; v[k][1] = t4.y; v[k][2] = t4.z; v[k][3] = t4.w;
-                }
-                tc_epilogue_q_t(c, v, pixr, nt * c.bn + c0 + 4 * c4, inv_scale);
-              }
-            }
-          }
-        }
-      }
+      tc_decode_tile(c, item - ML.item0, nt, b, ty, tx);
+      with_mma_n(c.bn, [&](auto n) {
+        tc_consume_tile<decltype(n)::value>(c, stages, staging, full_bar, empty_bar, rp, wg, tid, nt, b, ty, tx);
+      });
       // ---- publish: this warp's stores of the item are visible gpu-wide, to generic loads and to TMA ----
       __syncwarp();
       if (lane == 0) {
@@ -444,23 +172,10 @@ __global__ void __launch_bounds__(kMegaThreads, 1) update_mega_kernel(const __gr
         const int mtiles = c.B * c.tiles_y * c.tiles_x;
         red_release_gpu_add(P.flags + ML.flag0 + nt * mtiles + (b * c.tiles_y + ty) * c.tiles_x + tx, 1u);
       }
-      MEGA_STAMP(7);
     }
-  }
-
-  tc_fence_before();
-  if constexpr (kPair) {
-    cluster_sync_all();                  // no CTA leaves (or frees TMEM) while its peer may still signal it
-    if (warp == 1) tmem2_dealloc(tmem_base, 512u);
-  } else {
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, 512u);
   }
 #endif
 }
-
-extern int g_dbg_layer;            // timeline debugging (raft_b200_debug_timeline, api.cu)
-extern long long* g_dbg_buf;
 
 // ------------------------------------------------------------------------------------------------
 // Host side: the plan of one update-block application.
@@ -470,30 +185,25 @@ struct TcDeps { int n; int layer[2]; int ntile[2]; };            // by tensor-co
 struct MegaPlan {
   MegaParams P;
   int pos_of_layer[32];          // tensor-core layer id -> position in P.layer (-1: not planned)
+  int nsplit[kMegaMaxLayers];    // column tiles per column tile of the layer's table entry (tc_n_split)
   int nflags;
-  int pair;                      // 1: items are tile pairs for update_mega_kernel<true> (set before the layers are added)
   MegaPlan() {
     memset(&P, 0, sizeof(P));
     for (int i = 0; i < 32; ++i) pos_of_layer[i] = -1;
     nflags = 0;
-    pair = 0;
   }
 };
 
-inline int mega_flag_words(int B, int tiles) { return kMegaMaxLayers * 3 * B * tiles + 1; }   // upper bound used by the workspace layout
+inline int mega_flag_words(int B, int tiles) { return kMegaMaxLayers * 6 * B * tiles + 1; }   // upper bound used by the workspace layout
 
-// Appends a planned layer (p complete except for the launch fields).  Mirrors the checks of tc_launch().
-inline int mega_add(MegaPlan& M, int layer_id, TcConvParams& p, int n_tiles_n, const TcDeps& deps) {
+// Appends a planned layer (p complete except for the launch fields).  Mirrors the checks of tc_launch().  nsplit: the
+// layer's column tiles are its table's column tiles split nsplit ways, so a dependency on table tile j reads tiles
+// [j * nsplit, (j + 1) * nsplit).
+inline int mega_add(MegaPlan& M, int layer_id, TcConvParams& p, int n_tiles_n, int nsplit, const TcDeps& deps) {
   if (M.P.nlayers >= kMegaMaxLayers || layer_id < 0 || layer_id >= 32) return RAFT_ERR_UNSUPPORTED;
-  if (p.bn % 16 != 0 || p.bn < 16 || p.bn > 256 || p.TW * p.TH != kTileM) return RAFT_ERR_BAD_SHAPE;
-  if (p.mode != EPI_LINEAR && p.mode != EPI_GRU_ZR && p.mode != EPI_GRU_Q) return RAFT_ERR_UNSUPPORTED;
+  RAFT_TRY(tc_check(p));
   if (p.stride < 1) p.stride = 1;
-  p.pair = M.pair;
-  if (M.pair && (p.bn < 32 || ((p.B * ceil_div(p.H, p.TH) * ceil_div(p.W, p.TW)) & 1))) return RAFT_ERR_BAD_SHAPE;
-  const int saved_mode = p.mode;
-  p.mode = EPI_GRU_Q;                      // reserve the transposition patches whatever the layer's mode (one smem layout)
   tc_finalize(p);
-  p.mode = saved_mode;
   if (p.nstages < 2) return RAFT_ERR_UNSUPPORTED;
   if (p.nstages > kMegaMaxStages) p.nstages = kMegaMaxStages;
   p.n_tiles_n = n_tiles_n;
@@ -508,14 +218,17 @@ inline int mega_add(MegaPlan& M, int layer_id, TcConvParams& p, int n_tiles_n, c
     const int pos = M.pos_of_layer[deps.layer[d]];
     if (pos < 0) return RAFT_ERR_BAD_ARG;            // a source layer must be planned before its consumer
     ML.dep_layer[d] = pos;
-    ML.dep_ntile[d] = deps.ntile[d];
+    const int f = M.nsplit[pos];
+    ML.dep_nlo[d] = deps.ntile[d] < 0 ? 0 : deps.ntile[d] * f;
+    ML.dep_nhi[d] = deps.ntile[d] < 0 ? M.P.layer[pos].c.n_tiles_n - 1 : deps.ntile[d] * f + f - 1;
   }
   ML.dep_ry = ceil_div(p.ph > 0 ? p.ph : 1, p.TH);
   ML.dep_rx = ceil_div(p.pw > 0 ? p.pw : 1, p.TW);
   if (ML.dep_ry < 1) ML.dep_ry = 1;
   if (ML.dep_rx < 1) ML.dep_rx = 1;
   M.pos_of_layer[layer_id] = M.P.nlayers;
-  M.P.nitems += (M.pair ? mtiles / 2 : mtiles) * n_tiles_n;
+  M.nsplit[M.P.nlayers] = nsplit;
+  M.P.nitems += mtiles * n_tiles_n;
   M.nflags += mtiles * n_tiles_n;
   ++M.P.nlayers;
   return RAFT_OK;
@@ -526,41 +239,18 @@ inline int mega_launch(MegaPlan& M, unsigned int* flags, size_t flag_words, bool
   if ((size_t)M.nflags + 1 > flag_words) return RAFT_ERR_WORKSPACE;
   M.P.flags = flags;
   M.P.next_item = flags + M.nflags;
-  M.P.dbg = g_dbg_layer == 3000 ? g_dbg_buf : nullptr;      // raft_b200_debug_timeline(3000, buf of 148 * 16 * 8 int64)
   int dev = 0;
   RAFT_CUDA_TRY(cudaGetDevice(&dev));
-  static unsigned long long attr_mask = 0;          // per-device attribute (benign race: idempotent)
-  if (!(attr_mask & (1ull << (dev & 63)))) {
-    RAFT_CUDA_TRY(cudaFuncSetAttribute(update_mega_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    RAFT_CUDA_TRY(cudaFuncSetAttribute(update_mega_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    attr_mask |= 1ull << (dev & 63);
+  static int num_sms[64] = {0};                     // per-device attribute and SM count (benign race: idempotent)
+  if (!num_sms[dev & 63]) {
+    RAFT_CUDA_TRY(cudaFuncSetAttribute(update_mega_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax));
+    RAFT_CUDA_TRY(cudaDeviceGetAttribute(&num_sms[dev & 63], cudaDevAttrMultiProcessorCount, dev));
   }
   if (zero_flags) RAFT_CUDA_TRY(cudaMemsetAsync(flags, 0, ((size_t)M.nflags + 1) * sizeof(unsigned int), stream));
   // Items wait on items claimed by other CTAs: every claimed item is held by a RUNNING CTA, so the wait graph is acyclic
   // whatever the number of co-resident CTAs; one CTA per SM (shared memory), never more CTAs than SMs.
-  static int num_sms[64] = {0};
-  if (!num_sms[dev & 63]) RAFT_CUDA_TRY(cudaDeviceGetAttribute(&num_sms[dev & 63], cudaDevAttrMultiProcessorCount, dev));
-  const int smem = kSmemBudget + 1024;
-  if (!M.pair) {
-    const int grid = M.P.nitems < num_sms[dev & 63] ? M.P.nitems : num_sms[dev & 63];
-    update_mega_kernel<false><<<grid, kMegaThreads, smem, stream>>>(M.P);
-    return raft_launch_status();
-  }
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  const int pairs = M.P.nitems < num_sms[dev & 63] / 2 ? M.P.nitems : num_sms[dev & 63] / 2;
-  cfg.gridDim = dim3((unsigned)(2 * pairs));
-  cfg.blockDim = dim3((unsigned)kMegaThreads);
-  cfg.dynamicSmemBytes = (size_t)smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  RAFT_CUDA_TRY(cudaLaunchKernelEx(&cfg, update_mega_kernel<true>, M.P));
+  const int grid = M.P.nitems < num_sms[dev & 63] ? M.P.nitems : num_sms[dev & 63];
+  update_mega_kernel<<<grid, kTcThreads, kSmemMax, stream>>>(M.P);
   return raft_launch_status();
 }
 

@@ -44,9 +44,8 @@ inline int make_tmap_f16(CUtensorMap* out, const void* base, int rank, const uin
   return r == CUDA_SUCCESS ? 0 : RAFT_ERR_DRIVER;
 }
 
-// Measured on B200 (tools/tma_probe.cu, timelines in profiles/): one TMA box costs about max(616 cycles, bytes / 53 B/clk)
-// and an SM serves its boxes one after another, whatever their number in flight.  The hi and lo planes of every operand
-// are therefore fetched by ONE box: the plane index is an extra tensor dimension whose stride is (lo - hi) bytes.
+// The hi and lo planes of every operand are fetched by ONE box (TMA cost is per box more than per byte): the plane index
+// is an extra tensor dimension whose stride is (lo - hi) bytes.
 // Activation planes: rank-5 map (C, W, H, B, plane), box {64, tw*s, th*s, 1, 2} -> smem [hi 128 rows | lo 128 rows].
 inline int make_tmap_act2(CUtensorMap* out, const __half* hi, const __half* lo, int B, int H, int W, int cstride, int tw,
                           int th, int stride = 1) {
@@ -68,17 +67,6 @@ inline int make_tmap_wgt2(CUtensorMap* out, const __half* hi, const __half* lo, 
   uint64_t dims[4] = {(uint64_t)cin_pad, (uint64_t)cout_pad, (uint64_t)taps, 2};
   uint64_t str[3] = {(uint64_t)cin_pad * 2, (uint64_t)cout_pad * cin_pad * 2, (uint64_t)pstride};
   uint32_t box[4] = {64, (uint32_t)bn, 1, 2};
-  return make_tmap_f16(out, hi, 4, dims, str, box);
-}
-
-// Weight planes, three taps (one kernel row) per box: box {64, bn, 3, 2} -> smem [hi: tap 0 | tap 1 | tap 2][lo: ...].
-inline int make_tmap_wgt3(CUtensorMap* out, const __half* hi, const __half* lo, int taps, int cout_pad, int cin_pad,
-                          int bn) {
-  const ptrdiff_t pstride = reinterpret_cast<const char*>(lo) - reinterpret_cast<const char*>(hi);
-  if (pstride <= 0 || (pstride & 15)) return RAFT_ERR_BAD_ARG;
-  uint64_t dims[4] = {(uint64_t)cin_pad, (uint64_t)cout_pad, (uint64_t)taps, 2};
-  uint64_t str[3] = {(uint64_t)cin_pad * 2, (uint64_t)cout_pad * cin_pad * 2, (uint64_t)pstride};
-  uint32_t box[4] = {64, (uint32_t)bn, 3, 2};
   return make_tmap_f16(out, hi, 4, dims, str, box);
 }
 

@@ -46,7 +46,7 @@ struct TcLayerSpec {
   int kh, kw;
   int cin_pad, cout_pad;       // packed dims
   int nrange, r_src0[2], r_n[2], r_dst0[2];   // cin remap
-  int bn, ntn;                 // N per CTA, N tiles
+  int bn, ntn;                 // N per column tile, column tiles (launch_tc_layer splits bn > kMaxTileN further)
   int flatten;                 // 1: (kh,kw,cin) flattened into the channel axis -- the layer runs as a 1x1 conv on im2col planes
 };
 
@@ -274,11 +274,10 @@ inline int launch_tc_layer(const UpdateCtx& c, int layer, int nseg, const TcSeg*
   if (chunks * kChunkK != L.cin_pad) return RAFT_ERR_BAD_SHAPE;
   const __half* whi = reinterpret_cast<const __half*>(c.prepared + c.PL.tc_hi[layer]);
   const __half* wlo = reinterpret_cast<const __half*>(c.prepared + c.PL.tc_lo[layer]);
-  // pair plan (update_mega_kernel<true>): each CTA of a pair stages half of the weight rows; the pair's N is at least 32
-  // (rows past cout_pad are out of bounds of the map and arrive as zeros)
-  const bool pair = c.plan && c.plan->pair;
-  const int bn = pair && L.bn < 32 ? 32 : L.bn;
-  RAFT_TRY(make_tmap_wgt2(&p.b_map, whi, wlo, L.kh * L.kw, L.cout_pad, L.cin_pad, pair ? bn / 2 : bn));
+  const int nsplit = tc_n_split(L.bn);                // layers wider than kMaxTileN run as more column tiles
+  if (!nsplit) return RAFT_ERR_BAD_SHAPE;
+  const int bn = L.bn / nsplit;
+  RAFT_TRY(make_tmap_wgt2(&p.b_map, whi, wlo, L.kh * L.kw, L.cout_pad, L.cin_pad, bn));
   p.kh = L.kh; p.kw = L.kw; p.ph = (L.kh - 1) / 2; p.pw = (L.kw - 1) / 2;
   p.B = c.B; p.H = c.h; p.W = c.w; p.TH = th; p.TW = tw;
   p.bn = bn;
@@ -290,9 +289,10 @@ inline int launch_tc_layer(const UpdateCtx& c, int layer, int nseg, const TcSeg*
     static const int grp = [] { const char* e = getenv("RAFT_B200_UPD_GROUP"); return e ? atoi(e) : 0; }();
     if (grp > 0) p.group_chunks = grp;
   }
-  if (c.plan) return mega_add(*c.plan, layer, p, ntn > 0 ? ntn : L.ntn, deps);
+  const int n_tiles_n = (ntn > 0 ? ntn : L.ntn) * nsplit;
+  if (c.plan) return mega_add(*c.plan, layer, p, n_tiles_n, nsplit, deps);
   RAFT_COUNT_LAUNCH();
-  return tc_launch(p, ntn > 0 ? ntn : L.ntn, c.stream);
+  return tc_launch(p, n_tiles_n, c.stream);
 }
 
 }  // namespace raft

@@ -66,7 +66,7 @@ class CorrBlock:
     """Reference corr.py:99-162.  Plain class; the constructor builds the whole pyramid.
 
     Attributes as in the reference: fmap1, fmap2, num_levels, radius, corr_pyramid (list of
-    `num_levels` tensors (B*h*w, h>>l, w>>l, 1)).  `precision` ('f16x2' tcgen05 path, or 'fp32'
+    `num_levels` tensors (B*h*w, h>>l, w>>l, 1)).  `precision` ('f16x2' tensor-core path, or 'fp32'
     CUDA-core path) is a keyword-only extra.
     """
 

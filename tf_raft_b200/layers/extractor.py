@@ -1,7 +1,7 @@
 """Feature / context encoders -- host-side mirror of tf_raft/layers/extractor.py (SURVEY.md 8(f) rank 1).
 
 backend='native' (default): one call into libraft_b200.so (raft_b200_encoder_forward): every convolution on
-the tcgen05 kernel, stride-2 convolutions via TMA elementStrides, norms as fused epilogues (BatchNorm in
+the wgmma kernel, stride-2 convolutions via TMA elementStrides, norms as fused epilogues (BatchNorm in
 inference) or deterministic reduction kernels (InstanceNorm).
 backend='torch': IEEE-fp32 cuDNN convolutions through PyTorch with the reference's TensorFlow semantics
 restated (Keras 'same' padding incl. the asymmetric stride-2 case, eps = 1e-3 norms) -- kept as an

@@ -3,7 +3,7 @@
 (tfa AdamW + CyclicalLearningRate) and the scale function of tf_raft/training.py:10-15.
 
 What runs where (DESIGN.md "Training"):
-* correlation pyramid forward: the tcgen05 kernels of the inference path (CorrBlock); backward: two fp32 GEMMs per level;
+* correlation pyramid forward: the wgmma kernels of the inference path (CorrBlock); backward: two fp32 GEMMs per level;
 * pyramid lookup forward AND backward (d/d coords -- the reference does not detach coords1, model.py:102 -- and the
   scatter of d/d pyramid): hand-written CUDA (raft_b200_corr_lookup / raft_b200_corr_lookup_backward);
 * global-norm clipping + AdamW on ONE flat fp32 parameter / gradient / moment buffer: hand-written CUDA
@@ -12,8 +12,9 @@ What runs where (DESIGN.md "Training"):
   clipping (global norm of the reduced gradient, as a single-device step on the global batch would compute), and the
   per-channel batch statistics of the context encoder's BatchNorm layers all-reduced in forward and backward (SyncBN:
   the single-device reference normalises over the global batch);
-* convolutions, norms, gates, convex upsampling and the loss in the backward-capable form: IEEE-fp32 cuDNN / elementwise
-  kernels through torch.autograd -- library code, stated as such; the hand-written tensor-core kernels are forward-only.
+* convolutions, norms, gates, convex upsampling and the loss in the backward-capable form: IEEE-fp32 PyTorch CUDA kernels
+  through torch.autograd, with cuDNN switched off for the step (see Trainer.step) -- library code, stated as such; the
+  hand-written tensor-core kernels are forward-only.
 """
 import math
 
@@ -163,7 +164,7 @@ class _Lookup(torch.autograd.Function):
 
 
 class _CorrPyramid(torch.autograd.Function):
-    """CorrBlock.__init__: forward = the tcgen05 correlation kernels; backward = fp32 GEMMs on the pooled features
+    """CorrBlock.__init__: forward = the wgmma correlation kernels; backward = fp32 GEMMs on the pooled features
     (level l = fmap1 . avgpool^l(fmap2)^T / sqrt(C), so d fmap1 = sum_l dP_l . pool^l(fmap2) / sqrt(C) and
     d pool^l(fmap2) = dP_l^T . fmap1 / sqrt(C), un-pooled through the 2x2 means)."""
 
@@ -355,11 +356,20 @@ class Trainer:
         image1 = image1.to(torch.float32)
         image2 = image2.to(torch.float32)
         self.flat.zero_grad()
-        preds = self.graph.forward(image1, image2, self.model.iters)           # model.py:131 (training=True)
-        loss = loss_fn([flow_gt, valid], preds)                                # :132
-        # tape.gradient (:133).  Each rank's loss is the mean over ITS shard: the mean over the global batch is the
-        # average of the shard means (equal shard sizes), so gradients are summed over ranks and divided by the world size.
-        loss.backward()
+        # cuDNN off for the forward AND the backward of the step: on the H100 its algorithm choice for the small encoder's
+        # convolutions gives feature-encoder gradients ~10x further from an IEEE-fp32 autograd step than PyTorch's own
+        # (im2col + IEEE GEMM) convolutions -- up to 5 % of a tensor's largest entry (tests/test_train.py).
+        cudnn_enabled = torch.backends.cudnn.enabled
+        torch.backends.cudnn.enabled = False
+        try:
+            preds = self.graph.forward(image1, image2, self.model.iters)       # model.py:131 (training=True)
+            loss = loss_fn([flow_gt, valid], preds)                            # :132
+            # tape.gradient (:133).  Each rank's loss is the mean over ITS shard: the mean over the global batch is the
+            # average of the shard means (equal shard sizes), so gradients are summed over ranks and divided by the world
+            # size.
+            loss.backward()
+        finally:
+            torch.backends.cudnn.enabled = cudnn_enabled
         if self.world > 1:
             dist.all_reduce(self.flat.g, op=dist.ReduceOp.SUM)                 # ONE flat NCCL all-reduce per step
             self.flat.g.div_(self.world)

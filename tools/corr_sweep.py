@@ -42,7 +42,7 @@ def main():
             break
         n = g * g
         pyr_bytes = 4 * sum(n * (g >> l) * (g >> l) for l in range(4))
-        if pyr_bytes > 100e9:
+        if pyr_bytes > 0.8 * torch.cuda.get_device_properties(0).total_memory:
             print(f'{g:4d}: pyramid {pyr_bytes/1e9:.0f} GB does not fit')
             continue
         gen = torch.Generator().manual_seed(g)
