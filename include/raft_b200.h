@@ -9,14 +9,17 @@
  * Conventions
  *   - every pointer is DEVICE memory, dense row-major, NHWC, float32 unless stated;
  *     coordinates are (x, y) in the last dimension, exactly as in the reference;
- *   - the caller owns every buffer; the library never allocates or frees device memory and
- *     keeps no global mutable state beyond once-initialised function attributes and the
- *     resolved driver entry point for cuTensorMapEncodeTiled;
+ *   - the caller owns every buffer; the library never allocates or frees device memory;
+ *   - its global state is the per-thread launch counter (raft_b200_launch_count), the
+ *     process-wide loop profiler (raft_b200_profile_loop, off by default) and caches filled
+ *     once: kernel shared-memory attributes, SM counts and the resolved driver entry point
+ *     for cuTensorMapEncodeTiled;
  *   - every call is asynchronous on `stream` (a cudaStream_t passed as void*); nothing
  *     synchronises the device, so a sequence of calls can be captured into a CUDA graph;
  *   - return value: 0 = ok, < 0 = raft_status (argument / shape / workspace error, detected on
  *     the host before anything is launched), > 0 = cudaError_t of a failed launch;
- *   - re-entrant across host threads as long as streams and buffers differ;
+ *   - re-entrant across host threads as long as streams and buffers differ and the loop
+ *     profiler is off;
  *   - there is NO CPU path: without an sm_90 device every compute entry point returns
  *     RAFT_ERR_NO_DEVICE or the CUDA error.
  */
@@ -30,7 +33,7 @@
 extern "C" {
 #endif
 
-#define RAFT_B200_ABI_VERSION 1
+#define RAFT_B200_ABI_VERSION 2
 #define RAFT_MAX_LEVELS 8
 
 typedef enum raft_status {
@@ -38,7 +41,7 @@ typedef enum raft_status {
   RAFT_ERR_BAD_ARG = -1,     /* null pointer, unknown enum value                          */
   RAFT_ERR_BAD_SHAPE = -2,   /* non-positive dims, C not a multiple of 8, level too small */
   RAFT_ERR_WORKSPACE = -3,   /* workspace / prepared-weights buffer too small             */
-  RAFT_ERR_NO_DEVICE = -4,   /* no CUDA device of compute capability 10.x                 */
+  RAFT_ERR_NO_DEVICE = -4,   /* no CUDA device of compute capability 9.0                  */
   RAFT_ERR_DRIVER = -5,      /* cuTensorMapEncodeTiled unavailable or rejected a map       */
   RAFT_ERR_UNSUPPORTED = -6  /* valid request this build does not implement               */
 } raft_status;
@@ -56,7 +59,7 @@ typedef enum raft_variant { RAFT_VARIANT_BASIC = 0, RAFT_VARIANT_SMALL = 1 } raf
 
 const char* raft_b200_strerror(int status);
 int raft_b200_abi_version(void);
-/* 0 if device `device` can run the kernels (compute capability 10.x), else RAFT_ERR_NO_DEVICE. */
+/* 0 if device `device` can run the kernels (compute capability 9.0), else RAFT_ERR_NO_DEVICE.  */
 int raft_b200_device_ok(int device);
 
 /* ---------------------------------------------------------------------------------------------
@@ -254,10 +257,6 @@ void raft_b200_launch_count_reset(void);
  * of every iteration; _read waits for the last one and returns the summed durations of the most recent call.      */
 void raft_b200_profile_loop(int enable);
 int raft_b200_profile_read(float* lookup_ms, float* update_ms, int* iterations);
-/* Profiling aid: the next per-layer launches (conv_tc_kernel: RAFT_B200_MEGA=0, or the k-th encoder convolution with
- * tc_layer = 1000 + k) of tensor-core layer `tc_layer` (-1 = off) write clock64 stamps of CTA 0 into `device_buf_2048`
- * ([0, 512): tile started, [512, 1024): tile's epilogue done, one entry per tile of the CTA).                        */
-void raft_b200_debug_timeline(int tc_layer, long long* device_buf_2048);
 
 #ifdef __cplusplus
 }

@@ -36,7 +36,8 @@ def test_pyramid_sizes_match_survey(L):
     assert sum(sizes) == 272957440 + 0 or abs(sum(sizes) / 1e6 - 272.96) < 0.01
 
 
-def test_host_side_argument_errors(L):
+def test_host_side_argument_errors_and_abi_version(L):
+    """ABI version 2: raft_b200_debug_timeline was removed from the header."""
     from tf_raft_b200 import _lib
     sizes = (ctypes.c_size_t * 8)()
     assert L.raft_b200_corr_pyramid_sizes(1, 8, 8, 0, sizes) == -1          # levels out of range
@@ -50,7 +51,7 @@ def test_host_side_argument_errors(L):
     assert L.raft_b200_update_prepared_bytes(0, 196, 1, ctypes.byref(nbytes)) == -2
     assert L.raft_b200_update_prepared_bytes(1, 196, 0, ctypes.byref(nbytes)) == 0
     assert 'shape' in _lib.strerror(-2) and _lib.strerror(0) == 'ok'
-    assert L.raft_b200_abi_version() == 1
+    assert L.raft_b200_abi_version() == 2
 
 
 def test_no_device_is_reported_not_emulated(L):

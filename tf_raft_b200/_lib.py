@@ -64,7 +64,6 @@ _SIGNATURES = {
     'raft_b200_device_ok': (_i, [_i]),
     'raft_b200_launch_count': (ctypes.c_longlong, []),
     'raft_b200_launch_count_reset': (None, []),
-    'raft_b200_debug_timeline': (None, [_i, _vp]),
     'raft_b200_profile_loop': (None, [_i]),
     'raft_b200_profile_read': (_i, [ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_float), ctypes.POINTER(_i)]),
     'raft_b200_corr_pyramid_sizes': (_i, [_i, _i, _i, _i, ctypes.POINTER(_sz)]),
@@ -112,7 +111,7 @@ def lib():
             fn = getattr(handle, name)
             fn.restype = res
             fn.argtypes = args
-        if handle.raft_b200_abi_version() != 1:
+        if handle.raft_b200_abi_version() != 2:
             raise ImportError('libraft_b200.so ABI version mismatch; rebuild it')
         _lib = handle
     return _lib

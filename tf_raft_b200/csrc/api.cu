@@ -1,6 +1,8 @@
 // extern "C" entry points of libraft_b200.so (see include/raft_b200.h for the contract and the
 // reference file:line each one replaces).  Host code only decides shapes and launches kernels;
 // there is no CPU compute path.
+#include <stdlib.h>
+
 #include <algorithm>
 
 #include "corr_tc.cuh"
@@ -9,9 +11,6 @@
 
 namespace raft {
 thread_local long long g_launches = 0;
-int g_dbg_layer = -1;
-long long* g_dbg_buf = nullptr;
-int g_dbg_count = 0;               // encoder convolutions launched since the timeline was armed (tc_layer >= 1000)
 
 static int check_dims(int B, int h, int w) { return (B > 0 && h > 0 && w > 0) ? 0 : RAFT_ERR_BAD_SHAPE; }
 
@@ -148,15 +147,9 @@ static int corr_build_tc(const float* f1, const float* f2, int B, int h, int w, 
     const float m = frexpf(p.corr_div, &e);          // sqrt(C) = m * 2^e; m == 0.5 <=> exact power of two
     p.corr_mul = (m == 0.5f && p.corr_div * p.corr_div == (float)C) ? 1.0f / p.corr_div : 0.0f;
   }
-  int dev = 0;
-  RAFT_CUDA_TRY(cudaGetDevice(&dev));
-  static int num_sms[64] = {0};                     // per-device attribute and SM count (benign race: idempotent)
-  if (!num_sms[dev & 63]) {
-    RAFT_CUDA_TRY(cudaFuncSetAttribute(corr_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kCorrSmemBytes));
-    RAFT_CUDA_TRY(cudaDeviceGetAttribute(&num_sms[dev & 63], cudaDevAttrMultiProcessorCount, dev));
-  }
-  const int ntiles = p.tile0[levels];
-  corr_tc_kernel<<<ntiles < num_sms[dev & 63] ? ntiles : num_sms[dev & 63], kTcThreads, kCorrSmemBytes, st>>>(p);
+  unsigned grid = 0;
+  RAFT_TRY(persistent_grid<corr_tc_kernel>(kCorrSmemBytes, p.tile0[levels], &grid));
+  corr_tc_kernel<<<grid, kTcThreads, kCorrSmemBytes, st>>>(p);
   RAFT_COUNT_LAUNCH();
   return raft_launch_status();
 }
@@ -534,11 +527,6 @@ int raft_b200_profile_read(float* lookup_ms, float* update_ms, int* iterations) 
 }
 
 long long raft_b200_launch_count(void) { return g_launches; }
-void raft_b200_debug_timeline(int tc_layer, long long* device_buf_2048) {
-  g_dbg_layer = tc_layer;
-  g_dbg_count = 0;
-  g_dbg_buf = device_buf_2048;
-}
 void raft_b200_launch_count_reset(void) { g_launches = 0; }
 
 int raft_b200_corr_pyramid_sizes(int B, int h, int w, int levels, size_t bytes_per_level[]) {

@@ -22,8 +22,6 @@
 //   full (producer -> consumers) / empty (consumers -> producer).  The producer runs up to nstages ahead, so the loads of
 //   tile i+1 overlap the epilogue of tile i.
 #pragma once
-#include <stdlib.h>
-
 #include "common.cuh"
 #include "tmap.cuh"
 
@@ -71,11 +69,6 @@ struct alignas(64) TcConvParams {
   const float* concat_src; int concat_n;   // EPI_LINEAR: fp32 (px, concat_n) appended at columns [n_total, n_total+concat_n)
   float* z; int hid;                       // GRU: z plane (px, hid) fp32
   float* h;                                // GRU: hidden state (px, hid) fp32, updated in place by EPI_GRU_Q
-  long long* dbg;                          // optional timeline of CTA 0: [4][512] clock64 stamps
-  // Programmatic dependent launch (default; RAFT_B200_PDL=0 disables): the launch carries the programmatic-serialization
-  // attribute, so this grid's CTAs may be scheduled -- and run their prologue -- while the previous kernel in the stream
-  // drains; every thread then executes griddepcontrol.wait before touching global memory.
-  int pdl;
   // EPI_LINEAR with n_total == 2 (flow_head.conv2) inside the iteration loop: coords1 += delta_flow and
   // flow = coords1 - coords0 (model.py:102, :97) are applied by the thread that holds the pixel's two output columns.
   float* adv_coords;                       // (px, 2) coords1, updated in place; null = no fused advance
@@ -292,7 +285,12 @@ __device__ __forceinline__ void tc_epilogue_regs(const TcConvParams& p, float (&
 }
 
 // ------------------------------------------------------------------------------------------------
-// Shared by conv_tc_kernel and update_mega_kernel: the ring walk of one tile, its producer side and its consumer side.
+// The shared-memory ring of all three tensor-core kernels (conv_tc_kernel, update_mega_kernel, corr_tc_kernel).  A slot
+// holds one 64-channel chunk of both operands, [A_hi | A_lo | B_hi | B_lo]; full[s] completes on the slot's TMA bytes,
+// empty[s] on one arrival per consumer warp.
+// The geometry arguments (slot_bytes, nst, tx, group_chunks) are taken by reference: update_mega_kernel passes fields of
+// its parameter block at a run-time layer index, and a reference lets them be re-read after each barrier wait instead of
+// held in registers across the loop (its producer warpgroup runs in 40 registers; held, they add spills).
 // ------------------------------------------------------------------------------------------------
 struct RingPos {            // next ring slot and the parity of every slot's use count (producer and consumers each keep one)
   int slot;
@@ -305,6 +303,66 @@ __device__ __forceinline__ int ring_next(RingPos& r, int nst) {
   return s;
 }
 
+// Thread 0, before the CTA-wide barrier that precedes the first use; the caller then issues fence_mbar_init().
+__device__ __forceinline__ void ring_init(uint64_t* full_bar, uint64_t* empty_bar, int nst) {
+  for (int s = 0; s < nst; ++s) {
+    mbar_init(&full_bar[s], 1);
+    mbar_init(&empty_bar[s], kConsumerWarps);
+  }
+}
+
+struct RingSlot {
+  uint8_t* data;
+  uint64_t* full;           // the barrier the slot's TMA loads complete on
+};
+
+// Producer: waits for the next slot to be free and arms its full barrier for `tx` bytes of TMA loads.
+__device__ __forceinline__ RingSlot ring_acquire(uint8_t* stages, const int& slot_bytes, const int& nst, uint64_t* full_bar,
+                                                 uint64_t* empty_bar, RingPos& rp, const int& tx) {
+  const int s = ring_next(rp, nst);
+  mbar_wait(&empty_bar[s], ((rp.par >> s) & 1u) ^ 1u);
+  rp.par ^= 1u << s;
+  mbar_arrive_expect_tx(&full_bar[s], (uint32_t)tx);
+  return RingSlot{stages + (size_t)s * slot_bytes, &full_bar[s]};
+}
+
+// Consumer, all 128 threads of warpgroup `wg` (rows [64 wg, 64 wg + 64) of the A tile): the MMAs of `total` consecutive
+// slots, promoted -- added in IEEE fp32 into racc -- every `group_chunks` chunks, each group accumulating into a fresh
+// register tile.  N is the instantiated MMA width; b_lo_off is the byte offset of B_lo behind B_hi.
+template <int N>
+__device__ __forceinline__ void ring_mma(float (&racc)[N / 2], uint8_t* stages, const int& slot_bytes, const int& nst,
+                                         uint64_t* full_bar, uint64_t* empty_bar, RingPos& rp, int wg, uint32_t b_lo_off,
+                                         int total, const int& group_chunks) {
+  const int lane = threadIdx.x & 31;
+  float acc[N / 2];
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) acc[i] = racc[i] = 0.0f;
+  for (int done = 0; done < total;) {
+    const int gend = min(total, done + group_chunks);
+    for (int first = 1; done < gend; ++done, first = 0) {
+      const int s = ring_next(rp, nst);
+      mbar_wait(&full_bar[s], (rp.par >> s) & 1u);
+      rp.par ^= 1u << s;
+      const uint32_t sa = smem_u32(stages + (size_t)s * slot_bytes);
+      const uint32_t arow = (uint32_t)wg * 64 * 128;
+      wgmma_fence_regs(acc);
+      wgmma_fence();
+      wgmma_chunk3<N>(acc, make_desc_sw128(sa + arow), make_desc_sw128(sa + kABytes + arow), make_desc_sw128(sa + 2 * kABytes),
+                      make_desc_sw128(sa + 2 * kABytes + b_lo_off), first != 0);
+      wgmma_commit();
+      wgmma_wait_all();
+      wgmma_fence_regs(acc);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[s]);       // this warp's reads of the slot are complete
+    }
+#pragma unroll
+    for (int i = 0; i < N / 2; ++i) racc[i] += acc[i];   // IEEE fp32 promotion
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
+// Shared by conv_tc_kernel and update_mega_kernel: the ring walk of one convolution tile, producer and consumer side.
+// ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ int tc_total_chunks(const TcConvParams& c) {
   return c.kh * c.kw * (c.seg_chunks[0] + (c.nseg > 1 ? c.seg_chunks[1] : 0));
 }
@@ -323,14 +381,10 @@ __device__ __forceinline__ void tc_produce_tile(const TcConvParams& c, uint8_t* 
     for (int seg = 0; seg < c.nseg; ++seg) {
       for (int ch = 0; ch < c.seg_chunks[seg]; ++ch, ++kc) {
         if (--left == 0 && claim) *claim = (int)atomicAdd(next_item, 1u);
-        const int s = ring_next(rp, c.nstages);
-        mbar_wait(&empty_bar[s], ((rp.par >> s) & 1u) ^ 1u);
-        rp.par ^= 1u << s;
-        uint8_t* st = stages + (size_t)s * c.stage_bytes;
-        mbar_arrive_expect_tx(&full_bar[s], (uint32_t)c.stage_bytes);
+        const RingSlot st = ring_acquire(stages, c.stage_bytes, c.nstages, full_bar, empty_bar, rp, c.stage_bytes);
         // two boxes per stage: [A_hi | A_lo] and [B_hi | B_lo]
-        tma_load_5d(st, &c.a_map[seg], &full_bar[s], c.seg_c0[seg] + ch * kChunkK, x0 + dx, y0 + dy, b, 0);
-        tma_load_4d(st + 2 * kABytes, &c.b_map, &full_bar[s], kc * kChunkK, n0, tap, 0);
+        tma_load_5d(st.data, &c.a_map[seg], st.full, c.seg_c0[seg] + ch * kChunkK, x0 + dx, y0 + dy, b, 0);
+        tma_load_4d(st.data + 2 * kABytes, &c.b_map, st.full, kc * kChunkK, n0, tap, 0);
       }
     }
   }
@@ -339,7 +393,7 @@ __device__ __forceinline__ void tc_produce_tile(const TcConvParams& c, uint8_t* 
 // Staging tile of one warpgroup: 64 rows x 64 fp32, 16-byte groups XOR-swizzled by row (conflict-free row reads).
 __device__ __forceinline__ int stg_idx(int r, int c) { return r * kStageCols + ((((c >> 2) ^ (r & 7))) << 2) + (c & 3); }
 
-// Consumer side of one tile, all 128 threads of warpgroup `wg` (tid = thread index inside it): MMAs over the ring with
+// Consumer side of one tile, all 128 threads of warpgroup `wg` (tid = thread index inside it): the ring's MMAs with
 // IEEE-fp32 promotion every group_chunks chunks, then the epilogue of the warpgroup's 64 rows.  N >= c.bn is the
 // instantiated MMA width (columns past bn read other shared memory and are discarded).
 template <int N>
@@ -347,32 +401,9 @@ __device__ __forceinline__ void tc_consume_tile(const TcConvParams& c, uint8_t* 
                                                 uint64_t* empty_bar, RingPos& rp, int wg, int tid, int nt, int b, int ty,
                                                 int tx) {
   const int lane = tid & 31, w = tid >> 5;
-  const int total = tc_total_chunks(c);
-  const uint32_t b_bytes = (uint32_t)(c.bn * kChunkK * 2);
-  float acc[N / 2], racc[N / 2];
-#pragma unroll
-  for (int i = 0; i < N / 2; ++i) acc[i] = racc[i] = 0.0f;
-  for (int done = 0; done < total;) {
-    const int gend = min(total, done + c.group_chunks);
-    for (int first = 1; done < gend; ++done, first = 0) {
-      const int s = ring_next(rp, c.nstages);
-      mbar_wait(&full_bar[s], (rp.par >> s) & 1u);
-      rp.par ^= 1u << s;
-      const uint32_t sa = smem_u32(stages + (size_t)s * c.stage_bytes);
-      const uint32_t arow = (uint32_t)wg * 64 * 128;
-      wgmma_fence_regs(acc);
-      wgmma_fence();
-      wgmma_chunk3<N>(acc, make_desc_sw128(sa + arow), make_desc_sw128(sa + kABytes + arow), make_desc_sw128(sa + 2 * kABytes),
-                      make_desc_sw128(sa + 2 * kABytes + b_bytes), first != 0);
-      wgmma_commit();
-      wgmma_wait_all();
-      wgmma_fence_regs(acc);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&empty_bar[s]);       // this warp's reads of the slot are complete
-    }
-#pragma unroll
-    for (int i = 0; i < N / 2; ++i) racc[i] += acc[i];   // IEEE fp32 promotion
-  }
+  float racc[N / 2];
+  ring_mma<N>(racc, stages, c.stage_bytes, c.nstages, full_bar, empty_bar, rp, wg, (uint32_t)(c.bn * kChunkK * 2),
+              tc_total_chunks(c), c.group_chunks);
 
   // ---- epilogue: 64-column blocks through the staging tile; thread (row, half) then owns 32 columns of one pixel row ----
   float* stg = staging + wg * 64 * kStageCols;
@@ -454,10 +485,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
   const int ntiles = mtiles * p.n_tiles_n;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < nst; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], kConsumerWarps);
-    }
+    ring_init(full_bar, empty_bar, nst);
     fence_mbar_init();
   }
   if (warp == kConsumerWarps && (threadIdx.x & 31) == 0) {
@@ -466,12 +494,11 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
     if (p.nseg > 1) prefetch_tmap(&p.a_map[1]);
   }
   __syncthreads();
-  if (p.pdl) {
-    // barriers and tensor-map prefetch above touch no global data; from here on the previous grid's results are read
-    // (and its inputs overwritten), so wait for it, then let the next grid in the stream start its own prologue.
-    asm volatile("griddepcontrol.wait;" ::: "memory");
-    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  }
+  // Launched with programmatic dependent launch (tc_launch): the barriers and tensor-map prefetch above touch no global
+  // data and overlap the previous kernel's tail; from here on its results are read (and its inputs overwritten), so wait
+  // for it, then let the next grid in the stream start its own prologue.
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 
   RingPos rp{0, 0u};
   if (warp >= kConsumerWarps) {
@@ -492,15 +519,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
       for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
         int nt, b, ty, tx;
         tc_decode_tile(p, t, nt, b, ty, tx);
-        if (p.dbg && blockIdx.x == 0 && threadIdx.x == 0) {
-          const int tl = (t - (int)blockIdx.x) / (int)gridDim.x;
-          if (tl < 512) p.dbg[tl] = clock64();                               // tile started
-        }
         tc_consume_tile<decltype(n)::value>(p, stages, staging, full_bar, empty_bar, rp, wg, tid, nt, b, ty, tx);
-        if (p.dbg && blockIdx.x == 0 && threadIdx.x == 0) {
-          const int tl = (t - (int)blockIdx.x) / (int)gridDim.x;
-          if (tl < 512) p.dbg[512 + tl] = clock64();                         // tile's epilogue done
-        }
       }
     });
   }
@@ -540,19 +559,31 @@ inline int tc_finalize(TcConvParams& p) {
   int nst = (kSmemMax - kSmemFixed) / p.stage_bytes;
   if (nst > 8) nst = 8;
   p.nstages = nst;
-  if (p.group_chunks <= 0) p.group_chunks = 2;
   return nst * p.stage_bytes + kSmemFixed;
 }
 
-// RAFT_B200_PDL=0 disables programmatic dependent launch of the per-layer kernel (A/B timing).
-inline bool tc_pdl_enabled() {
-  static const int pdl = [] { const char* e = getenv("RAFT_B200_PDL"); return e ? atoi(e) : 1; }();
-  return pdl != 0;
-}
-
+// group_chunks has no default: every caller states its promotion group (a precision decision, DESIGN.md section 4).
 inline int tc_check(const TcConvParams& p) {
   if (p.bn % 16 != 0 || p.bn < 16 || p.bn > kMaxTileN || p.TW * p.TH != kTileM) return RAFT_ERR_BAD_SHAPE;
   if (p.mode != EPI_LINEAR && p.mode != EPI_GRU_ZR && p.mode != EPI_GRU_Q) return RAFT_ERR_UNSUPPORTED;
+  if (p.group_chunks < 1) return RAFT_ERR_BAD_ARG;
+  return RAFT_OK;
+}
+
+// Grid of a persistent tensor-core kernel: one CTA per SM, never more CTAs than work items.  The first call for a kernel
+// on a device raises the kernel's dynamic shared-memory limit to `smem` and caches the device's SM count (one entry per
+// kernel and device ordinal; benign race: the calls are idempotent).
+template <auto Kernel>
+inline int persistent_grid(int smem, long items, unsigned* grid) {
+  static int num_sms[64] = {0};
+  int dev = 0;
+  RAFT_CUDA_TRY(cudaGetDevice(&dev));
+  int& sms = num_sms[dev & 63];
+  if (!sms) {
+    RAFT_CUDA_TRY(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    RAFT_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  }
+  *grid = (unsigned)(items < sms ? items : sms);
   return RAFT_OK;
 }
 
@@ -561,35 +592,21 @@ inline int tc_launch(TcConvParams& p, int n_tiles_n, cudaStream_t stream) {
   if (p.stride < 1) p.stride = 1;
   const int smem = tc_finalize(p);
   if (p.nstages < 2) return RAFT_ERR_UNSUPPORTED;
-  // the attribute and the SM count are per device: one entry per device ordinal (benign race: the calls are idempotent)
-  int dev = 0;
-  RAFT_CUDA_TRY(cudaGetDevice(&dev));
-  static int num_sms[64] = {0};
-  if (!num_sms[dev & 63]) {
-    RAFT_CUDA_TRY(cudaFuncSetAttribute(conv_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax));
-    RAFT_CUDA_TRY(cudaDeviceGetAttribute(&num_sms[dev & 63], cudaDevAttrMultiProcessorCount, dev));
-  }
-  const int mtiles = p.B * p.tiles_y * p.tiles_x;
   p.n_tiles_n = n_tiles_n;
-  const long ntiles = (long)mtiles * n_tiles_n;
-  const unsigned grid = (unsigned)(ntiles < num_sms[dev & 63] ? ntiles : num_sms[dev & 63]);   // one persistent CTA per SM
-  p.pdl = tc_pdl_enabled() ? 1 : 0;
-  if (!p.pdl) {
-    conv_tc_kernel<<<grid, kTcThreads, smem, stream>>>(p);
-  } else {                                             // programmatic-serialization attribute: see the kernel prologue
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3((unsigned)kTcThreads);
-    cfg.dynamicSmemBytes = (size_t)smem;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    RAFT_CUDA_TRY(cudaLaunchKernelEx(&cfg, conv_tc_kernel, p));
-  }
+  unsigned grid = 0;
+  RAFT_TRY(persistent_grid<conv_tc_kernel>(kSmemMax, (long)p.B * p.tiles_y * p.tiles_x * n_tiles_n, &grid));
+  cudaLaunchConfig_t cfg;                              // programmatic-serialization attribute: see the kernel prologue
+  memset(&cfg, 0, sizeof(cfg));
+  cfg.gridDim = dim3(grid);
+  cfg.blockDim = dim3((unsigned)kTcThreads);
+  cfg.dynamicSmemBytes = (size_t)smem;
+  cfg.stream = stream;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  RAFT_CUDA_TRY(cudaLaunchKernelEx(&cfg, conv_tc_kernel, p));
   return raft_launch_status();
 }
 

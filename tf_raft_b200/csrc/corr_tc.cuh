@@ -6,8 +6,9 @@
 // plus one preparation kernel that pools fmap2 and splits both feature maps into the fp16 (hi, lo) operand planes.
 //
 // Tile = 128 queries x bn <= 128 targets, K = C in 64-channel chunks of a 3-stage ring (64 KB stages), three fp16 passes
-// per chunk (hi*hi, hi*lo, lo*hi; fp32-grade, DESIGN.md section 4).  Every chunk accumulates into a fresh register tile
-// (a 12-MMA chain) and the chunk results are added in IEEE fp32 ((0 + c0) + c1 + ...).  The pyramid feeds the sampler,
+// per chunk (hi*hi, hi*lo, lo*hi; fp32-grade, DESIGN.md section 4).  The ring and its MMA loop are the convolutions'
+// (ring_acquire / ring_mma, conv_tc.cuh) with a promotion group of one chunk: every chunk accumulates into a fresh register
+// tile (a 12-MMA chain) and the chunk results are added in IEEE fp32 ((0 + c0) + c1 + ...).  The pyramid feeds the sampler,
 // which is discontinuous at integer coordinates (DESIGN.md section 4), so the correlation takes the shortest chains:
 // with 24-MMA chains a query of the benchmark pair (448x512, seed 0/1) crosses a discontinuity at iteration 5 on the H100,
 // with 12 it stays within 3e-4 of the oracle.
@@ -51,30 +52,12 @@ __device__ __forceinline__ void corr_decode(const CorrTcParams& p, int t, int& l
 
 template <int N>
 __device__ __forceinline__ void corr_consume_tile(const CorrTcParams& p, uint8_t* stages, uint64_t* full_bar, uint64_t* empty_bar,
-                                                  int& it, int wg, int tid, int l, int nt, int mt) {
+                                                  RingPos& rp, int wg, int tid, int l, int nt, int mt) {
   const int lane = tid & 31, w = tid >> 5;
   const int bn = p.bn[l], n2 = p.n2[l];
-  const uint32_t b_lo_off = (uint32_t)(bn * kChunkK * 2);
-  float acc[N / 2], racc[N / 2];
-#pragma unroll
-  for (int i = 0; i < N / 2; ++i) acc[i] = racc[i] = 0.0f;
-  for (int kc = 0; kc < p.chunks; ++kc, ++it) {
-    const int s = it % kCorrStages;
-    mbar_wait(&full_bar[s], (uint32_t)(it / kCorrStages) & 1u);
-    const uint32_t sa = smem_u32(stages + (size_t)s * kCorrStageBytes);
-    const uint32_t arow = (uint32_t)wg * 64 * 128;
-    wgmma_fence_regs(acc);
-    wgmma_fence();
-    wgmma_chunk3<N>(acc, make_desc_sw128(sa + arow), make_desc_sw128(sa + kABytes + arow), make_desc_sw128(sa + 2 * kABytes),
-                    make_desc_sw128(sa + 2 * kABytes + b_lo_off), true);
-    wgmma_commit();
-    wgmma_wait_all();
-    wgmma_fence_regs(acc);
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&empty_bar[s]);
-#pragma unroll
-    for (int i = 0; i < N / 2; ++i) racc[i] += acc[i];     // IEEE fp32 sum of the 12-MMA chunk chains
-  }
+  float racc[N / 2];                                   // promotion group 1: IEEE fp32 sum of the 12-MMA chunk chains
+  ring_mma<N>(racc, stages, int{kCorrStageBytes}, int{kCorrStages}, full_bar, empty_bar, rp, wg, (uint32_t)(bn * kChunkK * 2),
+              p.chunks, 1);
   // ---- store ----
   const int b = mt / p.mtiles_img, m0 = (mt - b * p.mtiles_img) * kTileM, n0 = nt * bn;
   const int col_end = min(n2, n0 + bn);
@@ -116,33 +99,27 @@ __global__ void __launch_bounds__(kTcThreads, 1) corr_tc_kernel(const __grid_con
   const int ntiles = p.tile0[p.levels];
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < kCorrStages; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], kConsumerWarps);
-    }
+    ring_init(full_bar, empty_bar, kCorrStages);
     fence_mbar_init();
     prefetch_tmap(&p.a_map);
     for (int l = 0; l < p.levels; ++l) prefetch_tmap(&p.b_map[l]);
   }
   __syncthreads();
 
+  RingPos rp{0, 0u};
   if (warp >= kConsumerWarps) {
     // ===================== TMA producer =====================
     regs_producer();
     if (warp == kConsumerWarps && elect_one()) {
-      int it = 0;
       for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
         int l, nt, mt;
         corr_decode(p, t, l, nt, mt);
         const int b = mt / p.mtiles_img, m0 = (mt - b * p.mtiles_img) * kTileM, n0 = nt * p.bn[l];
-        const uint32_t bytes = (uint32_t)(2 * kABytes + p.bn[l] * kChunkK * 4);
-        for (int kc = 0; kc < p.chunks; ++kc, ++it) {
-          const int s = it % kCorrStages;
-          mbar_wait(&empty_bar[s], ((uint32_t)(it / kCorrStages) & 1u) ^ 1u);
-          uint8_t* st = stages + (size_t)s * kCorrStageBytes;
-          mbar_arrive_expect_tx(&full_bar[s], bytes);
-          tma_load_5d(st, &p.a_map, &full_bar[s], kc * kChunkK, m0, 0, b, 0);
-          tma_load_4d(st + 2 * kABytes, &p.b_map[l], &full_bar[s], kc * kChunkK, n0, b, 0);
+        const int bytes = 2 * kABytes + p.bn[l] * kChunkK * 4;     // slots are a fixed 64 KB; B fills bn rows of them
+        for (int kc = 0; kc < p.chunks; ++kc) {
+          const RingSlot st = ring_acquire(stages, int{kCorrStageBytes}, int{kCorrStages}, full_bar, empty_bar, rp, bytes);
+          tma_load_5d(st.data, &p.a_map, st.full, kc * kChunkK, m0, 0, b, 0);
+          tma_load_4d(st.data + 2 * kABytes, &p.b_map[l], st.full, kc * kChunkK, n0, b, 0);
         }
       }
     }
@@ -150,11 +127,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) corr_tc_kernel(const __grid_con
     // ===================== MMA + store (warpgroups 0, 1) =====================
     regs_consumer();
     const int wg = warp >> 2, tid = threadIdx.x & 127;
-    int it = 0;
     for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
       int l, nt, mt;
       corr_decode(p, t, l, nt, mt);
-      with_mma_n(p.bn[l], [&](auto n) { corr_consume_tile<decltype(n)::value>(p, stages, full_bar, empty_bar, it, wg, tid, l, nt, mt); });
+      with_mma_n(p.bn[l], [&](auto n) { corr_consume_tile<decltype(n)::value>(p, stages, full_bar, empty_bar, rp, wg, tid, l, nt, mt); });
     }
   }
 #endif

@@ -251,14 +251,10 @@ inline int enc_conv_tc(const EncCtx& c, const EncConvSlot& cs, const EncNormSlot
   } else {
     p.act = ACT_NONE; p.out_hi = nullptr; p.out_lo = nullptr;
   }
-  if (g_dbg_layer >= 1000 && g_dbg_count++ == g_dbg_layer - 1000) p.dbg = g_dbg_buf;   // timeline of the k-th encoder conv
-  {
-    // Promotion group of the encoder convolutions: their contractions are short (K <= 1152, 18 chunks), so the tensor-core
-    // accumulator may run for 5 chunks (60 MMA steps) between IEEE promotions instead of the update block's 2 (its
-    // K = 1920 GRU contractions feed a 12-iteration recurrence).
-    static const int grp = [] { const char* e = getenv("RAFT_B200_ENC_GROUP"); return e ? atoi(e) : 5; }();
-    if (grp > 0) p.group_chunks = grp;
-  }
+  // Promotion group of the encoder convolutions: their contractions are short (K <= 1152, 18 chunks), so the tensor-core
+  // accumulator may run for 5 chunks (60 MMA steps) between IEEE promotions instead of the update block's 2 (its
+  // K = 1920 GRU contractions feed a 12-iteration recurrence).
+  p.group_chunks = 5;
   ++g_launches;
   return tc_launch(p, nsplit, c.st);
 }

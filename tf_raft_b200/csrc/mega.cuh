@@ -74,10 +74,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) update_mega_kernel(const __grid
   const int lane = threadIdx.x & 31;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < kMegaMaxStages; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], kConsumerWarps);
-    }
+    ring_init(full_bar, empty_bar, kMegaMaxStages);
     for (int i = 0; i < kMegaQueue; ++i) mbar_init(&q_bar[i], 1);
     fence_mbar_init();
   }
@@ -207,7 +204,6 @@ inline int mega_add(MegaPlan& M, int layer_id, TcConvParams& p, int n_tiles_n, i
   if (p.nstages < 2) return RAFT_ERR_UNSUPPORTED;
   if (p.nstages > kMegaMaxStages) p.nstages = kMegaMaxStages;
   p.n_tiles_n = n_tiles_n;
-  p.pdl = 0;
   MegaLayer& ML = M.P.layer[M.P.nlayers];
   ML.c = p;
   const int mtiles = p.B * p.tiles_y * p.tiles_x;
@@ -239,17 +235,11 @@ inline int mega_launch(MegaPlan& M, unsigned int* flags, size_t flag_words, bool
   if ((size_t)M.nflags + 1 > flag_words) return RAFT_ERR_WORKSPACE;
   M.P.flags = flags;
   M.P.next_item = flags + M.nflags;
-  int dev = 0;
-  RAFT_CUDA_TRY(cudaGetDevice(&dev));
-  static int num_sms[64] = {0};                     // per-device attribute and SM count (benign race: idempotent)
-  if (!num_sms[dev & 63]) {
-    RAFT_CUDA_TRY(cudaFuncSetAttribute(update_mega_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax));
-    RAFT_CUDA_TRY(cudaDeviceGetAttribute(&num_sms[dev & 63], cudaDevAttrMultiProcessorCount, dev));
-  }
-  if (zero_flags) RAFT_CUDA_TRY(cudaMemsetAsync(flags, 0, ((size_t)M.nflags + 1) * sizeof(unsigned int), stream));
   // Items wait on items claimed by other CTAs: every claimed item is held by a RUNNING CTA, so the wait graph is acyclic
   // whatever the number of co-resident CTAs; one CTA per SM (shared memory), never more CTAs than SMs.
-  const int grid = M.P.nitems < num_sms[dev & 63] ? M.P.nitems : num_sms[dev & 63];
+  unsigned grid = 0;
+  RAFT_TRY(persistent_grid<update_mega_kernel>(kSmemMax, M.P.nitems, &grid));
+  if (zero_flags) RAFT_CUDA_TRY(cudaMemsetAsync(flags, 0, ((size_t)M.nflags + 1) * sizeof(unsigned int), stream));
   update_mega_kernel<<<grid, kTcThreads, kSmemMax, stream>>>(M.P);
   return raft_launch_status();
 }

@@ -10,9 +10,6 @@
 namespace raft {
 
 extern thread_local long long g_launches;
-extern int g_dbg_layer;            // timeline debugging (raft_b200_debug_timeline)
-extern long long* g_dbg_buf;
-extern int g_dbg_count;
 #define RAFT_COUNT_LAUNCH() (++::raft::g_launches)
 
 // ------------------------------------------------------------------------------------------------
@@ -284,11 +281,9 @@ inline int launch_tc_layer(const UpdateCtx& c, int layer, int nseg, const TcSeg*
   p.bias = reinterpret_cast<const float*>(c.prepared + c.PL.tc_bias[layer]);
   p.inv_scale = reinterpret_cast<const float*>(c.prepared + c.PL.tc_scale[layer]) + 1;
   if (p.out_scale == 0.0f) p.out_scale = 1.0f;
-  if (g_dbg_layer == layer) p.dbg = g_dbg_buf;
-  {   // promotion group of the update-block layers (default 2, see conv_tc.cuh); RAFT_B200_UPD_GROUP overrides for experiments
-    static const int grp = [] { const char* e = getenv("RAFT_B200_UPD_GROUP"); return e ? atoi(e) : 0; }();
-    if (grp > 0) p.group_chunks = grp;
-  }
+  // Promotion group of the update-block layers: 2 chunks (24-MMA chains).  Their K = 1920 GRU contractions feed a
+  // 12-iteration recurrence (DESIGN.md section 4).
+  p.group_chunks = 2;
   const int n_tiles_n = (ntn > 0 ? ntn : L.ntn) * nsplit;
   if (c.plan) return mega_add(*c.plan, layer, p, n_tiles_n, nsplit, deps);
   RAFT_COUNT_LAUNCH();
