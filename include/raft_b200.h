@@ -249,7 +249,7 @@ int raft_b200_forward_loop(int variant, const void* prepared, const float* const
                            int B, int h, int w, void* workspace, size_t workspace_bytes, int precision,
                            void* stream);
 
-/* Number of kernels the most recent call on this host thread launched (bench.py's gpu_launches). */
+/* Number of kernels launched on this host thread since the last raft_b200_launch_count_reset (bench.py's gpu_launches). */
 long long raft_b200_launch_count(void);
 void raft_b200_launch_count_reset(void);
 /* Profiling aid for bench.py's roofline objects: while enabled, raft_b200_forward_loop (F16X2, <= 64 iterations, not

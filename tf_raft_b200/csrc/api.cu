@@ -13,6 +13,8 @@ namespace raft {
 thread_local long long g_launches = 0;
 
 static int check_dims(int B, int h, int w) { return (B > 0 && h > 0 && w > 0) ? 0 : RAFT_ERR_BAD_SHAPE; }
+static int check_variant(int v) { return (v == RAFT_VARIANT_BASIC || v == RAFT_VARIANT_SMALL) ? 0 : RAFT_ERR_BAD_ARG; }
+static int check_precision(int p) { return (p == RAFT_PREC_FP32 || p == RAFT_PREC_F16X2) ? 0 : RAFT_ERR_BAD_ARG; }
 
 // Per-kernel timing of raft_b200_forward_loop for bench.py's roofline objects: CUDA events on the launching stream around
 // the lookup and around the update-block kernel(s) of every iteration (raft_b200_profile_loop / _read).  Off by default;
@@ -63,16 +65,12 @@ static int corr_build_fp32(const float* f1, const float* f2, int B, int h, int w
                            cudaStream_t st) {
   const int N = h * w;
   dim3 grid((unsigned)ceil_div(N, 64), (unsigned)ceil_div(N, 64), (unsigned)B);
-  corr_fp32_kernel<<<grid, 256, 0, st>>>(f1, f2, pyr[0], N, C, sqrtf((float)C));
-  RAFT_COUNT_LAUNCH();
-  RAFT_TRY(raft_launch_status());
+  RAFT_TRY(launch(corr_fp32_kernel, grid, 256, 0, st, f1, f2, pyr[0], N, C, sqrtf((float)C)));
   int lh = h, lw = w;
   for (int l = 1; l < levels; ++l) {        // corr.py:112-114: pool the volume itself
     const size_t M = (size_t)B * N;
     const size_t total = M * (lh / 2) * (lw / 2);
-    avgpool2x2_kernel<<<grid_for(total), 256, 0, st>>>(pyr[l - 1], pyr[l], M, lh, lw, 1);
-    RAFT_COUNT_LAUNCH();
-    RAFT_TRY(raft_launch_status());
+    RAFT_TRY(launch(avgpool2x2_kernel, grid_for(total), 256, 0, st, pyr[l - 1], pyr[l], M, lh, lw, 1));
     lh /= 2;
     lw /= 2;
   }
@@ -98,28 +96,24 @@ static int corr_build_tc(const float* f1, const float* f2, int B, int h, int w, 
     q.patches_x = ceil_div(w, 8); q.patches_y = ceil_div(h, 8);
     q.npatch = B * q.patches_x * q.patches_y;
     const int split_blocks = (int)std::min<size_t>((npix * C / 4 + 127) / 128, (size_t)kNumSMs * 8);
-    corr_prep_kernel<<<q.npatch + split_blocks, 128, 0, st>>>(q);
-    RAFT_COUNT_LAUNCH();
+    RAFT_TRY(launch(corr_prep_kernel, q.npatch + split_blocks, 128, 0, st, q));
   } else {                                   // deeper pyramids: generic pooling / split kernels, level by level
-    split_plane_kernel<<<grid_for(npix * C), 256, 0, st>>>(f1, C, 0, C, C, W.f1_hi, W.f1_lo, C, 0, npix, 1.0f);
-    RAFT_COUNT_LAUNCH();
+    RAFT_TRY(launch(split_plane_kernel, grid_for(npix * C), 256, 0, st, f1, C, 0, C, C, W.f1_hi, W.f1_lo, C, 0, npix, 1.0f));
     int lh = h, lw = w;
     const float* src = f2;
     for (int l = 0; l < levels; ++l) {
       if (l > 0) {
         const size_t total = (size_t)B * (lh / 2) * (lw / 2) * C;
-        avgpool2x2_kernel<<<grid_for(total), 256, 0, st>>>(src, W.f2_lvl[l], (size_t)B, lh, lw, C);
-        RAFT_COUNT_LAUNCH();
+        RAFT_TRY(launch(avgpool2x2_kernel, grid_for(total), 256, 0, st, src, W.f2_lvl[l], (size_t)B, lh, lw, C));
         src = W.f2_lvl[l];
         lh /= 2;
         lw /= 2;
       }
       const size_t np2 = (size_t)B * lh * lw;
-      split_plane_kernel<<<grid_for(np2 * C), 256, 0, st>>>(src, C, 0, C, C, W.f2_hi[l], W.f2_lo[l], C, 0, np2, 1.0f);
-      RAFT_COUNT_LAUNCH();
+      RAFT_TRY(launch(split_plane_kernel, grid_for(np2 * C), 256, 0, st, src, C, 0, C, C, W.f2_hi[l], W.f2_lo[l], C, 0, np2,
+                      1.0f));
     }
   }
-  RAFT_TRY(raft_launch_status());
 
   CorrTcParams p;
   memset(&p, 0, sizeof(p));
@@ -149,9 +143,7 @@ static int corr_build_tc(const float* f1, const float* f2, int B, int h, int w, 
   }
   unsigned grid = 0;
   RAFT_TRY(persistent_grid<corr_tc_kernel>(kCorrSmemBytes, p.tile0[levels], &grid));
-  corr_tc_kernel<<<grid, kTcThreads, kCorrSmemBytes, st>>>(p);
-  RAFT_COUNT_LAUNCH();
-  return raft_launch_status();
+  return launch(corr_tc_kernel, grid, kTcThreads, kCorrSmemBytes, st, p);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -162,12 +154,9 @@ static int gru_fp32(const UpdateCtx& c, float* h, int iz, int ir, int iq, int hi
   const size_t n = (size_t)c.B * c.h * c.w * hid;
   RAFT_TRY(simt2(c, iz, h, hid, hid, W.x, xs, xn, W.z, hid, SACT_SIGMOID));
   RAFT_TRY(simt2(c, ir, h, hid, hid, W.x, xs, xn, W.r, hid, SACT_SIGMOID));
-  gru_rh_kernel<<<grid_for(n), 256, 0, c.stream>>>(W.r, h, W.rh, n);
-  RAFT_COUNT_LAUNCH();
+  RAFT_TRY(launch(gru_rh_kernel, grid_for(n), 256, 0, c.stream, W.r, h, W.rh, n));
   RAFT_TRY(simt2(c, iq, W.rh, hid, hid, W.x, xs, xn, W.q, hid, SACT_TANH));
-  gru_update_kernel<<<grid_for(n), 256, 0, c.stream>>>(W.z, W.q, h, n);
-  RAFT_COUNT_LAUNCH();
-  return raft_launch_status();
+  return launch(gru_update_kernel, grid_for(n), 256, 0, c.stream, W.z, W.q, h, n);
 }
 
 static int update_core_fp32(const UpdateCtx& c, float* h, float* delta, float* mask) {
@@ -180,8 +169,7 @@ static int update_core_fp32(const UpdateCtx& c, float* h, float* delta, float* m
     RAFT_TRY(simt1(c, BF1, W.flow, 2, 0, 2, W.flo1, 128, 0, SACT_RELU));                // :100
     RAFT_TRY(simt1(c, BF2, W.flo1, 128, 0, 128, W.cf, 256, 192, SACT_RELU));            // :101,104
     RAFT_TRY(simt1(c, BCV, W.cf, 256, 0, 256, W.x, 256, 128, SACT_RELU));               // :105
-    copy_channels_kernel<<<grid_for(npix * 2), 256, 0, c.stream>>>(W.flow, 2, 0, W.x, 256, 254, 2, npix);   // :106
-    RAFT_COUNT_LAUNCH();
+    RAFT_TRY(launch(copy_channels_kernel, grid_for(npix * 2), 256, 0, c.stream, W.flow, 2, 0, W.x, 256, 254, 2, npix));  // :106
     RAFT_TRY(gru_fp32(c, h, BZ1, BR1, BQ1, 128, 256, 256));                             // :53-58
     RAFT_TRY(gru_fp32(c, h, BZ2, BR2, BQ2, 128, 256, 256));                             // :60-65
     RAFT_TRY(simt1(c, BFH1, h, 128, 0, 128, W.fm, 512, 0, SACT_RELU));                  // :14
@@ -195,8 +183,7 @@ static int update_core_fp32(const UpdateCtx& c, float* h, float* delta, float* m
     RAFT_TRY(simt1(c, SF1, W.flow, 2, 0, 2, W.flo1, 64, 0, SACT_RELU));                 // :81
     RAFT_TRY(simt1(c, SF2, W.flo1, 64, 0, 64, W.cf, 128, 96, SACT_RELU));               // :82-83
     RAFT_TRY(simt1(c, SCV, W.cf, 128, 0, 128, W.x, d.c_x, 64, SACT_RELU));              // :84
-    copy_channels_kernel<<<grid_for(npix * 2), 256, 0, c.stream>>>(W.flow, 2, 0, W.x, d.c_x, 144, 2, npix);  // :85
-    RAFT_COUNT_LAUNCH();
+    RAFT_TRY(launch(copy_channels_kernel, grid_for(npix * 2), 256, 0, c.stream, W.flow, 2, 0, W.x, d.c_x, 144, 2, npix));  // :85
     RAFT_TRY(gru_fp32(c, h, SZ, SR, SQ, 96, d.c_x, 146));                               // :26-35
     RAFT_TRY(simt1(c, SFH1, h, 96, 0, 96, W.fm, 128, 0, SACT_RELU));
     RAFT_TRY(simt1(c, SFH2, W.fm, 128, 0, 128, delta, 2, 0, SACT_NONE));
@@ -251,8 +238,7 @@ static int flow_branch_basic_tc(const UpdateCtx& c, int part) {
   if (part == 0) {  // convf1 7x7 2->128 + relu: K = 98 -> gather the window into 128-channel planes, run as a 1x1 GEMM
     const size_t npix = (size_t)c.B * c.h * c.w;
     if (!c.fim_ready) {              // (the iteration loop's lookup kernel has already produced the planes)
-      flow_im2col_kernel<<<grid_for(npix * 128), 256, 0, c.stream>>>(W.flow, c.B, c.h, c.w, W.fim_hi, W.fim_lo);
-      RAFT_COUNT_LAUNCH();
+      RAFT_TRY(launch(flow_im2col_kernel, grid_for(npix * 128), 256, 0, c.stream, W.flow, c.B, c.h, c.w, W.fim_hi, W.fim_lo));
     }
     tc_params_init(p, EPI_LINEAR, ACT_RELU, 128);
     p.out_hi = W.flo1_hi; p.out_lo = W.flo1_lo; p.h_stride = d.s_flo1;
@@ -325,8 +311,8 @@ static int update_core_tc(const UpdateCtx& c, float* h, float* delta, float* mas
     {  // convf1 7x7 2->64 + relu via im2col + 1x1 GEMM
       const size_t npix = (size_t)c.B * c.h * c.w;
       if (!c.fim_ready) {
-        flow_im2col_kernel<<<grid_for(npix * 128), 256, 0, c.stream>>>(W.flow, c.B, c.h, c.w, W.fim_hi, W.fim_lo);
-        RAFT_COUNT_LAUNCH();
+        RAFT_TRY(launch(flow_im2col_kernel, grid_for(npix * 128), 256, 0, c.stream, W.flow, c.B, c.h, c.w, W.fim_hi,
+                        W.fim_lo));
       }
       tc_params_init(p, EPI_LINEAR, ACT_RELU, 64);
       p.out_hi = W.flo1_hi; p.out_lo = W.flo1_lo; p.h_stride = d.s_flo1;
@@ -372,24 +358,19 @@ static int update_begin(const UpdateCtx& c, const float* h, const float* inp) {
   const size_t npix = (size_t)c.B * c.h * c.w;
   if (c.precision == RAFT_PREC_F16X2) {
     RAFT_CUDA_TRY(cudaMemsetAsync(W.f16_begin, 0, W.f16_bytes, c.stream));
-    split_plane_kernel<<<grid_for(npix * d.ctx), 256, 0, c.stream>>>(inp, d.ctx, 0, d.ctx, d.ctx, W.x_hi, W.x_lo, d.s_x,
-                                                                      0, npix, 1.0f);
-    RAFT_COUNT_LAUNCH();
-    split_plane_kernel<<<grid_for(npix * d.hid), 256, 0, c.stream>>>(h, d.hid, 0, d.hid, d.hid, W.h_hi, W.h_lo, d.s_h, 0,
-                                                                      npix, 1.0f);
-    RAFT_COUNT_LAUNCH();
-  } else {
-    RAFT_CUDA_TRY(cudaMemsetAsync(W.x, 0, npix * d.c_x * sizeof(float), c.stream));
-    copy_channels_kernel<<<grid_for(npix * d.ctx), 256, 0, c.stream>>>(inp, d.ctx, 0, W.x, d.c_x, 0, d.ctx, npix);
-    RAFT_COUNT_LAUNCH();
+    RAFT_TRY(launch(split_plane_kernel, grid_for(npix * d.ctx), 256, 0, c.stream, inp, d.ctx, 0, d.ctx, d.ctx, W.x_hi, W.x_lo,
+                    d.s_x, 0, npix, 1.0f));
+    return launch(split_plane_kernel, grid_for(npix * d.hid), 256, 0, c.stream, h, d.hid, 0, d.hid, d.hid, W.h_hi, W.h_lo,
+                  d.s_h, 0, npix, 1.0f);
   }
-  return raft_launch_status();
+  RAFT_CUDA_TRY(cudaMemsetAsync(W.x, 0, npix * d.c_x * sizeof(float), c.stream));
+  return launch(copy_channels_kernel, grid_for(npix * d.ctx), 256, 0, c.stream, inp, d.ctx, 0, W.x, d.c_x, 0, d.ctx, npix);
 }
 
 static int make_ctx(UpdateCtx& c, int variant, const void* prepared, int B, int h, int w, void* ws, size_t ws_bytes,
                     int precision, void* stream) {
-  if (variant != RAFT_VARIANT_BASIC && variant != RAFT_VARIANT_SMALL) return RAFT_ERR_BAD_ARG;
-  if (precision != RAFT_PREC_FP32 && precision != RAFT_PREC_F16X2) return RAFT_ERR_BAD_ARG;
+  RAFT_TRY(check_variant(variant));
+  RAFT_TRY(check_precision(precision));
   if (!prepared || !ws) return RAFT_ERR_BAD_ARG;
   RAFT_TRY(check_dims(B, h, w));
   c.variant = variant; c.precision = precision; c.B = B; c.h = h; c.w = w;
@@ -416,7 +397,6 @@ static int update_block_tc(UpdateCtx& c, float* h, float* delta, float* mask, fl
   c.plan = nullptr;
   RAFT_TRY(st);
   if (!mega_enabled()) return 0;
-  RAFT_COUNT_LAUNCH();
   return mega_launch(plan, c.W.mega_flags, c.W.mega_flag_words, true, c.stream);
 }
 
@@ -433,9 +413,8 @@ static int update_once(int variant, const void* prepared, const float* net, cons
   RAFT_CUDA_TRY(cudaMemcpyAsync(c.W.flow, flow, npix * 2 * sizeof(float), cudaMemcpyDeviceToDevice, c.stream));
   RAFT_TRY(update_begin(c, net_out, inp));
   if (precision == RAFT_PREC_F16X2) {
-    split_plane_kernel<<<grid_for(npix * d.s_corr), 256, 0, c.stream>>>(corr, d.corr_ch, 0, d.corr_ch, d.s_corr,
-                                                                         c.W.corr_hi, c.W.corr_lo, d.s_corr, 0, npix, 1.0f);
-    RAFT_COUNT_LAUNCH();
+    RAFT_TRY(launch(split_plane_kernel, grid_for(npix * d.s_corr), 256, 0, c.stream, corr, d.corr_ch, 0, d.corr_ch, d.s_corr,
+                    c.W.corr_hi, c.W.corr_lo, d.s_corr, 0, npix, 1.0f));
     return update_block_tc(c, net_out, delta, mask, nullptr);
   }
   RAFT_CUDA_TRY(cudaMemcpyAsync(c.W.corr, corr, npix * d.corr_ch * sizeof(float), cudaMemcpyDeviceToDevice, c.stream));
@@ -465,15 +444,11 @@ static int lookup_launch(const float* const pyr[], const float* coords, int B, i
   p.im_flow = im_flow; p.im_hi = im_hi; p.im_lo = im_lo; p.im_B = B; p.im_h = h; p.im_w = w;
   const size_t nwork = (size_t)p.nq * levels;
   static const int gather = [] { const char* e = getenv("RAFT_B200_LOOKUP_GATHER"); return e ? atoi(e) : 0; }();   // A/B: force the generic kernel
-  if (gather || !lookup_win_launch(p, levels, radius, st)) {       // window kernel for the model's (radius, levels); else generic
-    corr_lookup_kernel<<<grid_for(nwork * 32, 256, kNumSMs * 32), 256, 0, st>>>(p);
-    if (im_flow) {
-      flow_im2col_kernel<<<grid_for((size_t)p.nq * 128), 256, 0, st>>>(im_flow, B, h, w, im_hi, im_lo);
-      RAFT_COUNT_LAUNCH();
-    }
-  }
-  RAFT_COUNT_LAUNCH();
-  return raft_launch_status();
+  const LookupKernel win = gather ? nullptr : lookup_win_kernel(p, levels, radius);   // the model's (radius, levels)
+  if (win) return launch(win, grid_for(nwork * 32, 256, kNumSMs * 4), 256, 0, st, p);   // 4 resident blocks per SM: one wave
+  RAFT_TRY(launch(corr_lookup_kernel, grid_for(nwork * 32, 256, kNumSMs * 32), 256, 0, st, p));
+  if (!im_flow) return RAFT_OK;
+  return launch(flow_im2col_kernel, grid_for((size_t)p.nq * 128), 256, 0, st, im_flow, B, h, w, im_hi, im_lo);
 }
 
 }  // namespace raft
@@ -595,9 +570,7 @@ int raft_b200_corr_lookup_backward(const float* const pyr[], const float* coords
   p.coords = coords; p.gout = grad_out; p.gout_stride = levels * side * side; p.gcoords = grad_coords;
   p.nq = B * h * w; p.levels = levels; p.radius = radius;
   const size_t nwork = (size_t)p.nq * levels;
-  corr_lookup_bwd_kernel<<<grid_for(nwork * 32, 256, kNumSMs * 32), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
-  RAFT_COUNT_LAUNCH();
-  return raft_launch_status();
+  return launch(corr_lookup_bwd_kernel, grid_for(nwork * 32, 256, kNumSMs * 32), 256, 0, reinterpret_cast<cudaStream_t>(stream), p);
 }
 
 int raft_b200_sumsq(const float* g, size_t n, float* partials, size_t npartials, float* out, void* stream) {
@@ -605,43 +578,35 @@ int raft_b200_sumsq(const float* g, size_t n, float* partials, size_t npartials,
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   int blocks = (int)std::min<size_t>(std::min<size_t>(npartials, (size_t)kNumSMs * 4), (n + 255) / 256);
   if (blocks < 1) blocks = 1;
-  sumsq_partial_kernel<<<blocks, 256, 0, st>>>(g, n, partials);
-  sumsq_final_kernel<<<1, 256, 0, st>>>(partials, blocks, out);
-  g_launches += 2;
-  return raft_launch_status();
+  RAFT_TRY(launch(sumsq_partial_kernel, blocks, 256, 0, st, g, n, partials));
+  return launch(sumsq_final_kernel, 1, 256, 0, st, partials, blocks, out);
 }
 
 int raft_b200_adamw_step(float* param, const float* grad, float* m, float* v, size_t n, const float* sumsq, float clip_norm,
                          float lr_t, float beta1, float beta2, float epsilon, float weight_decay, void* stream) {
   if (!param || !grad || !m || !v || (clip_norm > 0.0f && !sumsq)) return RAFT_ERR_BAD_ARG;
-  adamw_kernel<<<grid_for(n), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(param, grad, m, v, n, sumsq, clip_norm, lr_t,
-                                                                             beta1, beta2, epsilon, weight_decay);
-  RAFT_COUNT_LAUNCH();
-  return raft_launch_status();
+  return launch(adamw_kernel, grid_for(n), 256, 0, reinterpret_cast<cudaStream_t>(stream), param, grad, m, v, n, sumsq,
+                clip_norm, lr_t, beta1, beta2, epsilon, weight_decay);
 }
 
 int raft_b200_bilinear_sampler(const float* image, const float* coords, int M, int H, int W, int P, float* out,
                                void* stream) {
   if (!image || !coords || !out) return RAFT_ERR_BAD_ARG;
   if (M < 1 || H < 1 || W < 1 || P < 1) return RAFT_ERR_BAD_SHAPE;
-  bilinear_sampler_kernel<<<grid_for((size_t)M * P), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(image, coords, M,
-                                                                                                      H, W, P, out);
-  RAFT_COUNT_LAUNCH();
-  return raft_launch_status();
+  return launch(bilinear_sampler_kernel, grid_for((size_t)M * P), 256, 0, reinterpret_cast<cudaStream_t>(stream), image,
+                coords, M, H, W, P, out);
 }
 
 int raft_b200_coords_grid(int B, int h, int w, float* out, void* stream) {
   if (!out) return RAFT_ERR_BAD_ARG;
   RAFT_TRY(check_dims(B, h, w));
-  coords_grid_kernel<<<grid_for((size_t)B * h * w), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(out, B, h, w);
-  RAFT_COUNT_LAUNCH();
-  return raft_launch_status();
+  return launch(coords_grid_kernel, grid_for((size_t)B * h * w), 256, 0, reinterpret_cast<cudaStream_t>(stream), out, B, h, w);
 }
 
 int raft_b200_update_prepared_bytes(int variant, int corr_channels, int precision, size_t* bytes) {
   if (!bytes) return RAFT_ERR_BAD_ARG;
-  if (variant != RAFT_VARIANT_BASIC && variant != RAFT_VARIANT_SMALL) return RAFT_ERR_BAD_ARG;
-  if (precision != RAFT_PREC_FP32 && precision != RAFT_PREC_F16X2) return RAFT_ERR_BAD_ARG;
+  RAFT_TRY(check_variant(variant));
+  RAFT_TRY(check_precision(precision));
   if (corr_channels != variant_dims(variant).corr_ch) return RAFT_ERR_BAD_SHAPE;
   *bytes = prepared_layout(variant, precision).total;
   return RAFT_OK;
@@ -650,8 +615,8 @@ int raft_b200_update_prepared_bytes(int variant, int corr_channels, int precisio
 int raft_b200_update_prepare(int variant, const void* weights, void* prepared, size_t prepared_bytes, int precision,
                              void* stream) {
   if (!weights || !prepared) return RAFT_ERR_BAD_ARG;
-  if (variant != RAFT_VARIANT_BASIC && variant != RAFT_VARIANT_SMALL) return RAFT_ERR_BAD_ARG;
-  if (precision != RAFT_PREC_FP32 && precision != RAFT_PREC_F16X2) return RAFT_ERR_BAD_ARG;
+  RAFT_TRY(check_variant(variant));
+  RAFT_TRY(check_precision(precision));
   const PreparedLayout L = prepared_layout(variant, precision);
   if (L.total > prepared_bytes) return RAFT_ERR_WORKSPACE;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
@@ -673,41 +638,8 @@ int raft_b200_update_prepare(int variant, const void* weights, void* prepared, s
     const TcLayerSpec* tl = tc_layers(variant);
     for (int li = 0; li < n_tc_layers(variant); ++li) {
       const TcLayerSpec& T = tl[li];
-      unsigned int* amax = reinterpret_cast<unsigned int*>(base + L.tc_absmax[li]);
-      float* scale = reinterpret_cast<float*>(base + L.tc_scale[li]);
-      for (int s = 0; s < T.nsrc; ++s) {
-        const int ci = T.src[s];
-        const size_t nw = (size_t)cd[ci].kh * cd[ci].kw * cd[ci].cin * cd[ci].cout;
-        absmax_kernel<<<grid_for(nw), 256, 0, st>>>(convs[ci].kernel, nw, amax);
-        RAFT_COUNT_LAUNCH();
-      }
-      weight_scale_kernel<<<1, 1, 0, st>>>(amax, scale);
-      RAFT_COUNT_LAUNCH();
-      int cout_off = 0;
-      for (int s = 0; s < T.nsrc; ++s) {
-        const int ci = T.src[s];
-        PackParams pp;
-        memset(&pp, 0, sizeof(pp));
-        pp.w = convs[ci].kernel;
-        pp.kh = cd[ci].kh; pp.kw = cd[ci].kw; pp.cin = cd[ci].cin; pp.cout = cd[ci].cout;
-        if (T.flatten) { pp.cin = pp.kh * pp.kw * pp.cin; pp.kh = pp.kw = 1; }   // HWIO is already [tap*cin + c][cout]
-        pp.hi = reinterpret_cast<__half*>(base + L.tc_hi[li]);
-        pp.lo = reinterpret_cast<__half*>(base + L.tc_lo[li]);
-        pp.cout_pad = T.cout_pad; pp.cin_pad = T.cin_pad; pp.cout_off = cout_off;
-        pp.nrange = T.nrange;
-        for (int r = 0; r < T.nrange; ++r) {
-          pp.r_src0[r] = T.r_src0[r];
-          pp.r_n[r] = T.r_n[r];
-          pp.r_dst0[r] = T.r_dst0[r];
-        }
-        pp.scale = scale;
-        const size_t nw = (size_t)cd[ci].kh * cd[ci].kw * cd[ci].cin * cd[ci].cout;
-        pack_weights_kernel<<<grid_for(nw), 256, 0, st>>>(pp);
-        RAFT_COUNT_LAUNCH();
-        RAFT_CUDA_TRY(cudaMemcpyAsync(base + L.tc_bias[li] + cout_off * sizeof(float), convs[ci].bias,
-                                      cd[ci].cout * sizeof(float), cudaMemcpyDeviceToDevice, st));
-        cout_off += cd[ci].cout;
-      }
+      const raft_conv* src[2] = {&convs[T.src[0]], T.nsrc > 1 ? &convs[T.src[1]] : nullptr};
+      RAFT_TRY(tc_pack_weights(base, L.tc[li], src, T.nsrc, &T.cin_map, T.flatten != 0, st));
     }
   }
   return raft_launch_status();
@@ -715,8 +647,8 @@ int raft_b200_update_prepare(int variant, const void* weights, void* prepared, s
 
 int raft_b200_update_workspace_bytes(int variant, int B, int h, int w, int precision, size_t* bytes) {
   if (!bytes) return RAFT_ERR_BAD_ARG;
-  if (variant != RAFT_VARIANT_BASIC && variant != RAFT_VARIANT_SMALL) return RAFT_ERR_BAD_ARG;
-  if (precision != RAFT_PREC_FP32 && precision != RAFT_PREC_F16X2) return RAFT_ERR_BAD_ARG;
+  RAFT_TRY(check_variant(variant));
+  RAFT_TRY(check_precision(precision));
   RAFT_TRY(check_dims(B, h, w));
   *bytes = workspace_layout(nullptr, variant, B, h, w, precision).total;
   return RAFT_OK;
@@ -740,22 +672,20 @@ int raft_b200_upsample_convex(const float* flow, const float* mask, int B, int h
   if (!flow || !mask || !out) return RAFT_ERR_BAD_ARG;
   RAFT_TRY(check_dims(B, h, w));
   const size_t npix = (size_t)B * h * w;
-  upsample_convex_kernel<<<grid_for(npix, 4, kNumSMs * 32), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(flow, mask,
-                                                                                                            B, h, w, out);
-  RAFT_COUNT_LAUNCH();
-  return raft_launch_status();
+  return launch(upsample_convex_kernel, grid_for(npix, 4, kNumSMs * 32), 256, 0, reinterpret_cast<cudaStream_t>(stream), flow,
+                mask, B, h, w, out);
 }
 
 int raft_b200_upflow8(const float* flow, int B, int h, int w, float* out, void* stream) {
   if (!flow || !out) return RAFT_ERR_BAD_ARG;
   RAFT_TRY(check_dims(B, h, w));
-  upflow8_kernel<<<grid_for((size_t)B * h * w * 64), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(flow, B, h, w, out);
-  RAFT_COUNT_LAUNCH();
-  return raft_launch_status();
+  return launch(upflow8_kernel, grid_for((size_t)B * h * w * 64), 256, 0, reinterpret_cast<cudaStream_t>(stream), flow, B, h,
+                w, out);
 }
 
 int raft_b200_encoder_prepared_bytes(int variant, int out_dim, size_t* bytes) {
-  if (!bytes || (variant != RAFT_VARIANT_BASIC && variant != RAFT_VARIANT_SMALL)) return RAFT_ERR_BAD_ARG;
+  if (!bytes) return RAFT_ERR_BAD_ARG;
+  RAFT_TRY(check_variant(variant));
   if (out_dim < 32 || out_dim > 256 || out_dim % 32) return RAFT_ERR_BAD_SHAPE;
   *bytes = enc_layout(variant, out_dim).total;
   return RAFT_OK;
@@ -763,14 +693,16 @@ int raft_b200_encoder_prepared_bytes(int variant, int out_dim, size_t* bytes) {
 
 int raft_b200_encoder_prepare(int variant, int norm_type, int out_dim, const raft_encoder_weights* weights,
                               void* prepared, size_t prepared_bytes, void* stream) {
-  if (!weights || !prepared || (variant != RAFT_VARIANT_BASIC && variant != RAFT_VARIANT_SMALL)) return RAFT_ERR_BAD_ARG;
+  if (!weights || !prepared) return RAFT_ERR_BAD_ARG;
+  RAFT_TRY(check_variant(variant));
   if (norm_type < 0 || norm_type > 2) return RAFT_ERR_BAD_ARG;
   if (out_dim < 32 || out_dim > 256 || out_dim % 32) return RAFT_ERR_BAD_SHAPE;
   return encoder_prepare(variant, norm_type, out_dim, weights, prepared, prepared_bytes, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int raft_b200_encoder_workspace_bytes(int variant, int N, int H, int W, size_t* bytes) {
-  if (!bytes || (variant != RAFT_VARIANT_BASIC && variant != RAFT_VARIANT_SMALL)) return RAFT_ERR_BAD_ARG;
+  if (!bytes) return RAFT_ERR_BAD_ARG;
+  RAFT_TRY(check_variant(variant));
   RAFT_TRY(check_dims(N, H, W));
   *bytes = enc_ws_layout(nullptr, variant, N, H, W).total;
   return RAFT_OK;
@@ -780,7 +712,7 @@ int raft_b200_encoder_forward(int variant, int norm_type, int out_dim, const voi
                               int N, int H, int W, int training, int image_norm, float* out, void* workspace,
                               size_t workspace_bytes, void* stream) {
   if (!prepared || !images || !out || !workspace) return RAFT_ERR_BAD_ARG;
-  if (variant != RAFT_VARIANT_BASIC && variant != RAFT_VARIANT_SMALL) return RAFT_ERR_BAD_ARG;
+  RAFT_TRY(check_variant(variant));
   if (norm_type < 0 || norm_type > 2) return RAFT_ERR_BAD_ARG;
   RAFT_TRY(check_dims(N, H, W));
   if (out_dim < 32 || out_dim > 256 || out_dim % 32 || H < 8 || W < 8) return RAFT_ERR_BAD_SHAPE;
@@ -792,10 +724,8 @@ int raft_b200_context_split(const float* cnet, int npix, int hidden, int context
                             void* stream) {
   if (!cnet || !net || !inp) return RAFT_ERR_BAD_ARG;
   if (npix < 1 || hidden < 1 || context < 1) return RAFT_ERR_BAD_SHAPE;
-  context_split_kernel<<<grid_for((size_t)npix * (hidden + context)), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      cnet, (size_t)npix, hidden, context, net, inp);
-  RAFT_COUNT_LAUNCH();
-  return raft_launch_status();
+  return launch(context_split_kernel, grid_for((size_t)npix * (hidden + context)), 256, 0, reinterpret_cast<cudaStream_t>(stream),
+                cnet, (size_t)npix, hidden, context, net, inp);
 }
 
 int raft_b200_conv2d(const float* x, const float* kernel, const float* bias, int B, int H, int W, int cin, int kh,
@@ -813,9 +743,7 @@ int raft_b200_conv2d(const float* x, const float* kernel, const float* bias, int
   p.out = out; p.out_stride = out_stride; p.out_c0 = out_c0;
   p.act = act; p.out_scale = 1.0f;
   dim3 grid((unsigned)ceil_div(B * H * W, 64), (unsigned)ceil_div(cout, 64));
-  conv_simt_kernel<<<grid, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
-  RAFT_COUNT_LAUNCH();
-  return raft_launch_status();
+  return launch(conv_simt_kernel, grid, 256, 0, reinterpret_cast<cudaStream_t>(stream), p);
 }
 
 int raft_b200_forward_loop(int variant, const void* prepared, const float* const pyr[], int levels, int radius,
@@ -831,8 +759,7 @@ int raft_b200_forward_loop(int variant, const void* prepared, const float* const
   const size_t npix = (size_t)B * h * w;
   const Workspace& W = c.W;
   RAFT_TRY(update_begin(c, net, inp));
-  flow_advance_kernel<<<grid_for(npix), 256, 0, c.stream>>>(coords1, nullptr, W.flow, B, h, w);   // model.py:97
-  RAFT_COUNT_LAUNCH();
+  RAFT_TRY(launch(flow_advance_kernel, grid_for(npix), 256, 0, c.stream, coords1, nullptr, W.flow, B, h, w));   // model.py:97
   const bool prof = g_prof.on && iters <= 64;
   if (prof && !g_prof.created) {
     for (int i = 0; i < 64; ++i)
@@ -854,8 +781,7 @@ int raft_b200_forward_loop(int variant, const void* prepared, const float* const
     } else {
       RAFT_TRY(lookup_launch(pyr, coords1, B, h, w, levels, radius, W.corr, d.corr_ch, nullptr, nullptr, 0, 0, c.stream));
       RAFT_TRY(update_core_fp32(c, net, W.delta, mask));
-      flow_advance_kernel<<<grid_for(npix), 256, 0, c.stream>>>(coords1, W.delta, W.flow, B, h, w);  // :102
-      RAFT_COUNT_LAUNCH();
+      RAFT_TRY(launch(flow_advance_kernel, grid_for(npix), 256, 0, c.stream, coords1, W.delta, W.flow, B, h, w));  // :102
     }
     if (flow_up[i]) {                                                                               // :105 / :223
       if (variant == RAFT_VARIANT_BASIC)

@@ -33,6 +33,19 @@ constexpr int kNumSMs = 132;         // H100 SXM; persistent kernels size their 
 
 __host__ __device__ constexpr int ceil_div(int a, int b) { return (a + b - 1) / b; }
 __host__ __device__ constexpr int round_up(int a, int b) { return ceil_div(a, b) * b; }
+inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
+
+// Kernels launched on this host thread (raft_b200_launch_count).
+extern thread_local long long g_launches;
+
+// Every kernel of the library except conv_tc_kernel (tc_launch, conv_tc.cuh) is launched here: launch, count, and return
+// the launch status.
+template <class... P, class... A>
+inline int launch(void (*kernel)(P...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, A&&... args) {
+  kernel<<<grid, block, smem, st>>>(static_cast<A&&>(args)...);
+  ++g_launches;
+  return raft_launch_status();
+}
 
 // ------------------------------------------------------------------------------------------
 // fp16 hi/lo split: v ~= float(hi) + float(lo), |error| <= 2^-23 |v| in the normal range.

@@ -23,6 +23,7 @@
 //   tile i+1 overlap the epilogue of tile i.
 #pragma once
 #include "common.cuh"
+#include "kernels.cuh"
 #include "tmap.cuh"
 
 namespace raft {
@@ -606,8 +607,92 @@ inline int tc_launch(TcConvParams& p, int n_tiles_n, cudaStream_t stream) {
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
+  ++g_launches;
   RAFT_CUDA_TRY(cudaLaunchKernelEx(&cfg, conv_tc_kernel, p));
   return raft_launch_status();
+}
+
+// ------------------------------------------------------------------------------------------------
+// Packed weights of one tensor-core convolution, the format conv_tc_kernel and update_mega_kernel read.  A slot in a
+// prepared-weights blob (update blocks and encoders alike) holds, each part 256-byte aligned and in this order:
+//   hi, lo   [tap][cout_pad][cin_pad] fp16 planes of w * 2^k (2^k puts max|w| in [2^12, 2^13), see weight_scale_kernel)
+//   bias     cout_pad + 64 floats (the epilogue reads whole 32-column chunks past the last column)
+//   scale    (2^k, 2^-k)
+//   absmax   the bits of max|w|, reduced while packing
+// ------------------------------------------------------------------------------------------------
+struct TcWeightSlot {
+  size_t hi, lo, bias, scale, absmax;    // byte offsets inside the blob
+  int kh, kw, cin_pad, cout_pad;
+};
+
+// Reserves a slot at byte offset `off` of a blob and advances `off` past it.
+inline TcWeightSlot tc_weight_slot(size_t& off, int kh, int kw, int cin_pad, int cout_pad) {
+  auto take = [&](size_t bytes) { const size_t o = off; off = align_up(off + bytes, 256); return o; };
+  TcWeightSlot s;
+  s.kh = kh; s.kw = kw; s.cin_pad = cin_pad; s.cout_pad = cout_pad;
+  const size_t plane = (size_t)kh * kw * cout_pad * cin_pad * sizeof(__half);
+  s.hi = take(plane);
+  s.lo = take(plane);
+  s.bias = take(sizeof(float) * (cout_pad + 64));
+  s.scale = take(2 * sizeof(float));
+  s.absmax = take(sizeof(unsigned int));
+  return s;
+}
+
+// Where the input channels of a packed convolution land: source channels [src0[r], src0[r] + n[r]) go to packed
+// channels [dst0[r], dst0[r] + n[r]), r < nrange.
+struct TcCinMap { int nrange, src0[2], n[2], dst0[2]; };
+
+// Writes slot `s` of the zeroed blob at `base` from nsrc (1 or 2) HWIO convolutions, concatenated along cout.
+// cin_map == null keeps the channels where they are.  flatten: each source runs as a 1x1 convolution over its
+// kh * kw * cin window channels (HWIO is already [tap * cin + c][cout]), for layers fed by im2col planes.  The scale is
+// shared by the sources: it comes from the absmax over all of them.
+inline int tc_pack_weights(uint8_t* base, const TcWeightSlot& s, const raft_conv* const src[], int nsrc,
+                           const TcCinMap* cin_map, bool flatten, cudaStream_t st) {
+  unsigned int* amax = reinterpret_cast<unsigned int*>(base + s.absmax);
+  float* scale = reinterpret_cast<float*>(base + s.scale);
+  for (int i = 0; i < nsrc; ++i) {
+    const size_t nw = (size_t)src[i]->kh * src[i]->kw * src[i]->cin * src[i]->cout;
+    RAFT_TRY(launch(absmax_kernel, grid_for(nw), 256, 0, st, src[i]->kernel, nw, amax));
+  }
+  RAFT_TRY(launch(weight_scale_kernel, 1, 1, 0, st, amax, scale));
+  int cout_off = 0;
+  for (int i = 0; i < nsrc; ++i) {
+    const raft_conv& cv = *src[i];
+    PackParams pp;
+    memset(&pp, 0, sizeof(pp));
+    pp.w = cv.kernel;
+    pp.kh = cv.kh; pp.kw = cv.kw; pp.cin = cv.cin; pp.cout = cv.cout;
+    if (flatten) { pp.cin = pp.kh * pp.kw * pp.cin; pp.kh = pp.kw = 1; }
+    pp.hi = reinterpret_cast<__half*>(base + s.hi);
+    pp.lo = reinterpret_cast<__half*>(base + s.lo);
+    pp.cout_pad = s.cout_pad; pp.cin_pad = s.cin_pad; pp.cout_off = cout_off;
+    const TcCinMap m = cin_map ? *cin_map : TcCinMap{1, {0, 0}, {pp.cin, 0}, {0, 0}};
+    pp.nrange = m.nrange;
+    for (int r = 0; r < m.nrange; ++r) {
+      pp.r_src0[r] = m.src0[r];
+      pp.r_n[r] = m.n[r];
+      pp.r_dst0[r] = m.dst0[r];
+    }
+    pp.scale = scale;
+    RAFT_TRY(launch(pack_weights_kernel, grid_for((size_t)cv.kh * cv.kw * cv.cin * cv.cout), 256, 0, st, pp));
+    RAFT_CUDA_TRY(cudaMemcpyAsync(base + s.bias + cout_off * sizeof(float), cv.bias, cv.cout * sizeof(float),
+                                  cudaMemcpyDeviceToDevice, st));
+    cout_off += cv.cout;
+  }
+  return RAFT_OK;
+}
+
+// Points `p` at the packed weights of slot `s` of the blob at `base`, read in column tiles of bn: weight tensor map,
+// taps, bias and 2^-k.
+inline int tc_use_weights(TcConvParams& p, const uint8_t* base, const TcWeightSlot& s, int bn) {
+  RAFT_TRY(make_tmap_wgt2(&p.b_map, reinterpret_cast<const __half*>(base + s.hi),
+                          reinterpret_cast<const __half*>(base + s.lo), s.kh * s.kw, s.cout_pad, s.cin_pad, bn));
+  p.kh = s.kh; p.kw = s.kw;
+  p.bn = bn;
+  p.bias = reinterpret_cast<const float*>(base + s.bias);
+  p.inv_scale = reinterpret_cast<const float*>(base + s.scale) + 1;
+  return RAFT_OK;
 }
 
 }  // namespace raft

@@ -23,15 +23,14 @@ inline EncSpec enc_spec(int variant) {
 }
 inline int pad64(int c) { return round_up(c, 64); }
 
-struct EncConvSlot { size_t hi, lo, bias, scale, absmax; int kh, kw, cin, cout, cin_pad, cout_pad; };
 struct EncNormSlot { size_t gamma, beta, fscale, fshift; int C; };
 struct EncLayout {
-  EncConvSlot conv1;                          // stem as a 1x1 conv over the 147 (->192) im2col channels
+  TcWeightSlot conv1;                         // stem as a 1x1 conv over the 147 (->192) im2col channels
   EncNormSlot norm1;
-  EncConvSlot bc1[6], bc2[6], bds[6];
+  TcWeightSlot bc1[6], bc2[6], bds[6];
   EncNormSlot bn1[6], bn2[6], bnd[6];
-  int has_ds[6], bcin[6], bc[6], bstride[6];
-  EncConvSlot conv2;
+  int has_ds[6], bc[6], bstride[6];
+  TcWeightSlot conv2;
   size_t total;
 };
 
@@ -41,16 +40,7 @@ inline EncLayout enc_layout(int variant, int out_dim) {
   const EncSpec S = enc_spec(variant);
   size_t off = 0;
   auto take = [&](size_t bytes) { size_t o = off; off = align_up(off + bytes, 256); return o; };
-  auto conv_slot = [&](int kh, int kw, int cin, int cout) {
-    EncConvSlot s;
-    s.kh = kh; s.kw = kw; s.cin = cin; s.cout = cout; s.cin_pad = pad64(cin); s.cout_pad = round_up(cout, 32);
-    const size_t plane = (size_t)kh * kw * s.cout_pad * s.cin_pad * sizeof(__half);
-    s.hi = take(plane); s.lo = take(plane);
-    s.bias = take(sizeof(float) * (s.cout_pad + 64));
-    s.scale = take(2 * sizeof(float));
-    s.absmax = take(sizeof(unsigned int));
-    return s;
-  };
+  auto conv_slot = [&](int kh, int kw, int cin, int cout) { return tc_weight_slot(off, kh, kw, pad64(cin), round_up(cout, 32)); };
   auto norm_slot = [&](int C) {
     EncNormSlot n;
     n.C = C;
@@ -63,7 +53,7 @@ inline EncLayout enc_layout(int variant, int out_dim) {
   int cin = S.c0;
   for (int k = 0; k < 6; ++k) {
     const int c = S.c[k / 2], st = (k % 2 == 0) ? S.s[k / 2] : 1;
-    L.bcin[k] = cin; L.bc[k] = c; L.bstride[k] = st;
+    L.bc[k] = c; L.bstride[k] = st;
     L.bc1[k] = conv_slot(3, 3, cin, c);
     L.bc2[k] = conv_slot(3, 3, c, c);
     L.bn1[k] = norm_slot(c);
@@ -116,25 +106,13 @@ inline EncWs enc_ws_layout(void* base, int variant, int N, int H, int W) {
 }
 
 // ---- prepare ----------------------------------------------------------------------------------
-inline int enc_pack_conv(const raft_conv& cv, const EncConvSlot& s, uint8_t* base, cudaStream_t st) {
+// Packs one convolution after checking that it has the shape (kh, kw, cin, cout); flatten: the 7x7 stem, as a 1x1 conv.
+inline int enc_pack_conv(const raft_conv& cv, int kh, int kw, int cin, int cout, const TcWeightSlot& s, bool flatten,
+                         uint8_t* base, cudaStream_t st) {
   if (!cv.kernel || !cv.bias) return RAFT_ERR_BAD_ARG;
-  if (cv.kh != s.kh || cv.kw != s.kw || cv.cin != s.cin || cv.cout != s.cout) return RAFT_ERR_BAD_SHAPE;
-  const size_t nw = (size_t)s.kh * s.kw * s.cin * s.cout;
-  unsigned int* amax = reinterpret_cast<unsigned int*>(base + s.absmax);
-  float* scale = reinterpret_cast<float*>(base + s.scale);
-  absmax_kernel<<<grid_for(nw), 256, 0, st>>>(cv.kernel, nw, amax);
-  weight_scale_kernel<<<1, 1, 0, st>>>(amax, scale);
-  PackParams pp;
-  memset(&pp, 0, sizeof(pp));
-  pp.w = cv.kernel; pp.kh = s.kh; pp.kw = s.kw; pp.cin = s.cin; pp.cout = s.cout;
-  pp.hi = reinterpret_cast<__half*>(base + s.hi); pp.lo = reinterpret_cast<__half*>(base + s.lo);
-  pp.cout_pad = s.cout_pad; pp.cin_pad = s.cin_pad; pp.cout_off = 0;
-  pp.nrange = 1; pp.r_src0[0] = 0; pp.r_n[0] = s.cin; pp.r_dst0[0] = 0;
-  pp.scale = scale;
-  pack_weights_kernel<<<grid_for(nw), 256, 0, st>>>(pp);
-  g_launches += 3;
-  RAFT_CUDA_TRY(cudaMemcpyAsync(base + s.bias, cv.bias, s.cout * sizeof(float), cudaMemcpyDeviceToDevice, st));
-  return raft_launch_status();
+  if (cv.kh != kh || cv.kw != kw || cv.cin != cin || cv.cout != cout) return RAFT_ERR_BAD_SHAPE;
+  const raft_conv* src[1] = {&cv};
+  return tc_pack_weights(base, s, src, 1, nullptr, flatten, st);
 }
 
 inline int enc_pack_norm(const raft_norm& nm, const EncNormSlot& s, int norm_type, uint8_t* base, cudaStream_t st) {
@@ -146,10 +124,8 @@ inline int enc_pack_norm(const raft_norm& nm, const EncNormSlot& s, int norm_typ
   RAFT_CUDA_TRY(cudaMemcpyAsync(b, nm.beta, s.C * sizeof(float), cudaMemcpyDeviceToDevice, st));
   if (norm_type == NORM_BATCH) {
     if (!nm.moving_mean || !nm.moving_variance) return RAFT_ERR_BAD_ARG;
-    bn_fold_kernel<<<ceil_div(s.C, 128), 128, 0, st>>>(nm.gamma, nm.beta, nm.moving_mean, nm.moving_variance, 1e-3f, s.C,
-                                                       reinterpret_cast<float*>(base + s.fscale),
-                                                       reinterpret_cast<float*>(base + s.fshift));
-    ++g_launches;
+    return launch(bn_fold_kernel, ceil_div(s.C, 128), 128, 0, st, nm.gamma, nm.beta, nm.moving_mean, nm.moving_variance,
+                  1e-3f, s.C, reinterpret_cast<float*>(base + s.fscale), reinterpret_cast<float*>(base + s.fshift));
   }
   return raft_launch_status();
 }
@@ -161,25 +137,22 @@ inline int encoder_prepare(int variant, int norm_type, int out_dim, const raft_e
   const EncSpec S = enc_spec(variant);
   uint8_t* base = reinterpret_cast<uint8_t*>(prepared);
   RAFT_CUDA_TRY(cudaMemsetAsync(base, 0, L.total, st));
-  if (!w->conv1.kernel || !w->conv1.bias) return RAFT_ERR_BAD_ARG;
-  if (w->conv1.kh != 7 || w->conv1.kw != 7 || w->conv1.cin != 3 || w->conv1.cout != S.c0) return RAFT_ERR_BAD_SHAPE;
-  {
-    raft_conv flat = w->conv1;            // HWIO (7,7,3,c0) is already [tap*3 + c][cout]: view it as 1x1 over 147
-    flat.kh = 1; flat.kw = 1; flat.cin = 147;
-    RAFT_TRY(enc_pack_conv(flat, L.conv1, base, st));
-  }
+  RAFT_TRY(enc_pack_conv(w->conv1, 7, 7, 3, S.c0, L.conv1, true, base, st));
   RAFT_TRY(enc_pack_norm(w->norm1, L.norm1, norm_type, base, st));
+  int cin = S.c0;
   for (int k = 0; k < 6; ++k) {
-    RAFT_TRY(enc_pack_conv(w->block[k].conv1, L.bc1[k], base, st));
-    RAFT_TRY(enc_pack_conv(w->block[k].conv2, L.bc2[k], base, st));
+    const int c = L.bc[k];
+    RAFT_TRY(enc_pack_conv(w->block[k].conv1, 3, 3, cin, c, L.bc1[k], false, base, st));
+    RAFT_TRY(enc_pack_conv(w->block[k].conv2, 3, 3, c, c, L.bc2[k], false, base, st));
     RAFT_TRY(enc_pack_norm(w->block[k].norm1, L.bn1[k], norm_type, base, st));
     RAFT_TRY(enc_pack_norm(w->block[k].norm2, L.bn2[k], norm_type, base, st));
     if (L.has_ds[k]) {
-      RAFT_TRY(enc_pack_conv(w->block[k].downsample, L.bds[k], base, st));
+      RAFT_TRY(enc_pack_conv(w->block[k].downsample, 1, 1, cin, c, L.bds[k], false, base, st));
       RAFT_TRY(enc_pack_norm(w->block[k].downsample_norm, L.bnd[k], norm_type, base, st));
     }
+    cin = c;
   }
-  RAFT_TRY(enc_pack_conv(w->conv2, L.conv2, base, st));
+  RAFT_TRY(enc_pack_conv(w->conv2, 1, 1, cin, out_dim, L.conv2, false, base, st));
   return raft_launch_status();
 }
 
@@ -200,19 +173,18 @@ inline int enc_norm_apply(const EncCtx& c, const EncNormSlot& ns, const float* y
   const float* beta = reinterpret_cast<const float*>(c.prep + ns.beta);
   // (Finalisation is a separate launch: inside norm_stats_kernel the merge of C channels by the last block of a group would
   //  be serial, where norm_final_kernel spreads it over G*C warps.)
-  norm_stats_kernel<<<dim3((unsigned)G, kNormSplit), 256, 0, c.st>>>(y, Pg, C, kNormSplit, c.W.part);
-  norm_final_kernel<<<ceil_div(G * C * 32, 256), 256, 0, c.st>>>(c.W.part, G, C, kNormSplit, gamma, 1e-3f, c.W.mean, c.W.mult);
-  norm_apply_kernel<<<grid_for(npix * (pad64(C) / 8)), 256, 0, c.st>>>(y, npix, P, C, c.per_image, c.W.mean, c.W.mult, beta, relu,
-                                                                 skip32, skip_hi, skip_lo, out32, hi, lo, pad64(C));
-  g_launches += 3;
-  return raft_launch_status();
+  RAFT_TRY(launch(norm_stats_kernel, dim3((unsigned)G, kNormSplit), 256, 0, c.st, y, Pg, C, kNormSplit, c.W.part));
+  RAFT_TRY(launch(norm_final_kernel, ceil_div(G * C * 32, 256), 256, 0, c.st, c.W.part, G, C, kNormSplit, gamma, 1e-3f,
+                  c.W.mean, c.W.mult));
+  return launch(norm_apply_kernel, grid_for(npix * (pad64(C) / 8)), 256, 0, c.st, y, npix, P, C, c.per_image, c.W.mean,
+                c.W.mult, beta, relu, skip32, skip_hi, skip_lo, out32, hi, lo, pad64(C));
 }
 
-// One tensor-core convolution of the encoder.  When the norm needs data statistics the raw output goes to
-// `raw32` (bias only); otherwise the folded affine, activation and skip are applied in the epilogue.
-inline int enc_conv_tc(const EncCtx& c, const EncConvSlot& cs, const EncNormSlot* ns, const __half* ahi, const __half* alo,
-                       int Hin, int Win, int Hout, int Wout, int stride, int relu, const float* skip, float* out32,
-                       __half* ohi, __half* olo) {
+// One tensor-core convolution of the encoder, cout output channels.  When the norm needs data statistics the raw output
+// goes to `raw32` (bias only); otherwise the folded affine, activation and skip are applied in the epilogue.
+inline int enc_conv_tc(const EncCtx& c, const TcWeightSlot& cs, int cout, const EncNormSlot* ns, const __half* ahi,
+                       const __half* alo, int Hin, int Win, int Hout, int Wout, int stride, int relu, const float* skip,
+                       float* out32, __half* ohi, __half* olo) {
   TcConvParams p;
   memset(&p, 0, sizeof(p));
   int tw, th;
@@ -221,11 +193,9 @@ inline int enc_conv_tc(const EncCtx& c, const EncConvSlot& cs, const EncNormSlot
   const int nsplit = tc_n_split(cs.cout_pad);          // layers wider than kMaxTileN run as more column tiles
   if (!nsplit) return RAFT_ERR_BAD_SHAPE;
   RAFT_TRY(make_tmap_act2(&p.a_map[0], ahi, alo, c.N, Hin, Win, cs.cin_pad, tw, th, stride));
-  RAFT_TRY(make_tmap_wgt2(&p.b_map, reinterpret_cast<const __half*>(c.prep + cs.hi),
-                          reinterpret_cast<const __half*>(c.prep + cs.lo), cs.kh * cs.kw, cs.cout_pad, cs.cin_pad,
-                          cs.cout_pad / nsplit));
+  RAFT_TRY(tc_use_weights(p, c.prep, cs, cs.cout_pad / nsplit));
   p.nseg = 1; p.seg_chunks[0] = cs.cin_pad / kChunkK; p.seg_c0[0] = 0;
-  p.kh = cs.kh; p.kw = cs.kw; p.stride = stride;
+  p.stride = stride;
   // Keras 'same': stride 1 -> (k-1)/2 before; stride 2 on even input -> total k-2, before = (k-2)/2 (0 for 3x3);
   // 1x1 convs are 'valid' (no padding).
   if (stride == 1) { p.ph = (cs.kh - 1) / 2; p.pw = (cs.kw - 1) / 2; }
@@ -234,12 +204,10 @@ inline int enc_conv_tc(const EncCtx& c, const EncConvSlot& cs, const EncNormSlot
     p.ph = (tot_h > 0 ? tot_h : 0) / 2; p.pw = (tot_w > 0 ? tot_w : 0) / 2;
   }
   p.B = c.N; p.H = Hout; p.W = Wout; p.TH = th; p.TW = tw;
-  p.bn = cs.cout_pad / nsplit; p.n_total = cs.cout;
+  p.n_total = cout;
   p.mode = EPI_LINEAR; p.out_scale = 1.0f;
-  p.bias = reinterpret_cast<const float*>(c.prep + cs.bias);
-  p.inv_scale = reinterpret_cast<const float*>(c.prep + cs.scale) + 1;
-  p.out_f32 = out32; p.f32_stride = cs.cout; p.f32_c0 = 0;
-  p.out_hi = ohi; p.out_lo = olo; p.h_stride = pad64(cs.cout); p.h_c0 = 0;
+  p.out_f32 = out32; p.f32_stride = cout; p.f32_c0 = 0;
+  p.out_hi = ohi; p.out_lo = olo; p.h_stride = pad64(cout); p.h_c0 = 0;
   if (ns && !c.stats && c.norm_type == NORM_BATCH) {
     p.post_scale = reinterpret_cast<const float*>(c.prep + ns->fscale);
     p.post_shift = reinterpret_cast<const float*>(c.prep + ns->fshift);
@@ -247,7 +215,7 @@ inline int enc_conv_tc(const EncCtx& c, const EncConvSlot& cs, const EncNormSlot
   const bool fused = !(ns && c.stats);
   if (fused) {
     p.act = relu ? ACT_RELU : ACT_NONE;
-    p.residual = skip; p.res_stride = cs.cout; p.res_c0 = 0;
+    p.residual = skip; p.res_stride = cout; p.res_c0 = 0;
   } else {
     p.act = ACT_NONE; p.out_hi = nullptr; p.out_lo = nullptr;
   }
@@ -255,7 +223,6 @@ inline int enc_conv_tc(const EncCtx& c, const EncConvSlot& cs, const EncNormSlot
   // accumulator may run for 5 chunks (60 MMA steps) between IEEE promotions instead of the update block's 2 (its
   // K = 1920 GRU contractions feed a 12-iteration recurrence).
   p.group_chunks = 5;
-  ++g_launches;
   return tc_launch(p, nsplit, c.st);
 }
 
@@ -283,28 +250,25 @@ inline int encoder_forward(int variant, int norm_type, int out_dim, const void* 
     const float* src = images;
     if (image_norm) {                                 // normalise once (O32 is free until the first ResBlock finishes)
       const size_t nimg = (size_t)N * H * W * 3;
-      image_norm_kernel<<<grid_for(nimg), 256, 0, st>>>(images, E.O32, nimg);
-      ++g_launches;
+      RAFT_TRY(launch(image_norm_kernel, grid_for(nimg), 256, 0, st, images, E.O32, nimg));
       src = E.O32;
     }
-    stem_im2col_kernel<<<grid_for(npix * 24), 256, 0, st>>>(src, N, H, W, h, w, (tot_h > 0 ? tot_h : 0) / 2,
-                                                            (tot_w > 0 ? tot_w : 0) / 2, 0, E.Ih, E.Il);
-    ++g_launches;
+    RAFT_TRY(launch(stem_im2col_kernel, grid_for(npix * 24), 256, 0, st, src, N, H, W, h, w, (tot_h > 0 ? tot_h : 0) / 2,
+                    (tot_w > 0 ? tot_w : 0) / 2, 0, E.Ih, E.Il));
     if (!c.stats && pad64(S.c0) != S.c0) {
       RAFT_CUDA_TRY(cudaMemsetAsync(E.Xh, 0, npix * pad64(S.c0) * 2, st));
       RAFT_CUDA_TRY(cudaMemsetAsync(E.Xl, 0, npix * pad64(S.c0) * 2, st));
     }
-    RAFT_TRY(enc_conv_tc(c, L.conv1, &L.norm1, E.Ih, E.Il, h, w, h, w, 1, 1, nullptr, c.stats ? E.Y32 : E.X32, E.Xh, E.Xl));
+    RAFT_TRY(enc_conv_tc(c, L.conv1, S.c0, &L.norm1, E.Ih, E.Il, h, w, h, w, 1, 1, nullptr, c.stats ? E.Y32 : E.X32, E.Xh, E.Xl));
     if (c.stats) RAFT_TRY(enc_norm_apply(c, L.norm1, E.Y32, npix, h * w, 1, nullptr, nullptr, nullptr, nullptr, E.Xh, E.Xl));
   }
 
   float *X32 = E.X32, *O32 = E.O32;
   __half *Xh = E.Xh, *Xl = E.Xl, *Oh = E.Oh, *Ol = E.Ol;
   for (int k = 0; k < 6; ++k) {
-    const int st2 = L.bstride[k], cin = L.bcin[k], cc = L.bc[k];
+    const int st2 = L.bstride[k], cc = L.bc[k];
     const int ho = (h + st2 - 1) / st2, wo = (w + st2 - 1) / st2;
     const size_t npo = (size_t)N * ho * wo;
-    (void)cin;
     const bool zero_pad_out = pad64(cc) != cc;     // fused epilogues write 32-column chunks: clear the 64-pad tail
     // conv1 + norm1 + relu -> F
     if (!c.stats && zero_pad_out) {
@@ -313,17 +277,17 @@ inline int encoder_forward(int variant, int norm_type, int out_dim, const void* 
       RAFT_CUDA_TRY(cudaMemsetAsync(Oh, 0, npo * pad64(cc) * 2, st));
       RAFT_CUDA_TRY(cudaMemsetAsync(Ol, 0, npo * pad64(cc) * 2, st));
     }
-    RAFT_TRY(enc_conv_tc(c, L.bc1[k], &L.bn1[k], Xh, Xl, h, w, ho, wo, st2, 1, nullptr, c.stats ? E.Y32 : nullptr, E.Fh, E.Fl));
+    RAFT_TRY(enc_conv_tc(c, L.bc1[k], cc, &L.bn1[k], Xh, Xl, h, w, ho, wo, st2, 1, nullptr, c.stats ? E.Y32 : nullptr, E.Fh, E.Fl));
     if (c.stats) RAFT_TRY(enc_norm_apply(c, L.bn1[k], E.Y32, npo, ho * wo, 1, nullptr, nullptr, nullptr, nullptr, E.Fh, E.Fl));
     // skip branch
     const float* skip = X32;
     if (L.has_ds[k]) {
-      RAFT_TRY(enc_conv_tc(c, L.bds[k], &L.bnd[k], Xh, Xl, h, w, ho, wo, st2, 0, nullptr, c.stats ? E.Y32 : E.D32, nullptr, nullptr));
+      RAFT_TRY(enc_conv_tc(c, L.bds[k], cc, &L.bnd[k], Xh, Xl, h, w, ho, wo, st2, 0, nullptr, c.stats ? E.Y32 : E.D32, nullptr, nullptr));
       if (c.stats) RAFT_TRY(enc_norm_apply(c, L.bnd[k], E.Y32, npo, ho * wo, 0, nullptr, nullptr, nullptr, E.D32, nullptr, nullptr));
       skip = E.D32;
     }
     // conv2 + norm2 + relu, then relu(skip + fx) -> O
-    RAFT_TRY(enc_conv_tc(c, L.bc2[k], &L.bn2[k], E.Fh, E.Fl, ho, wo, ho, wo, 1, 1, skip, c.stats ? E.Y32 : O32, Oh, Ol));
+    RAFT_TRY(enc_conv_tc(c, L.bc2[k], cc, &L.bn2[k], E.Fh, E.Fl, ho, wo, ho, wo, 1, 1, skip, c.stats ? E.Y32 : O32, Oh, Ol));
     if (c.stats) {   // skip = block input: from D32 after a downsample, else from the block's own fp16 operand planes
       if (L.has_ds[k]) RAFT_TRY(enc_norm_apply(c, L.bn2[k], E.Y32, npo, ho * wo, 1, E.D32, nullptr, nullptr, nullptr, Oh, Ol));
       else RAFT_TRY(enc_norm_apply(c, L.bn2[k], E.Y32, npo, ho * wo, 1, nullptr, Xh, Xl, nullptr, Oh, Ol));
@@ -335,7 +299,7 @@ inline int encoder_forward(int variant, int norm_type, int out_dim, const void* 
     h = ho; w = wo;
   }
   // conv2 1x1 -> (N, H/8, W/8, out_dim), bias only (extractor.py:125)
-  RAFT_TRY(enc_conv_tc(c, L.conv2, nullptr, Xh, Xl, h, w, h, w, 1, 0, nullptr, out, nullptr, nullptr));
+  RAFT_TRY(enc_conv_tc(c, L.conv2, out_dim, nullptr, Xh, Xl, h, w, h, w, 1, 0, nullptr, out, nullptr, nullptr));
   return raft_launch_status();
 }
 

@@ -192,28 +192,24 @@ __global__ void __launch_bounds__(256, 4) corr_lookup_win_kernel(const LookupPar
                       (size_t)gridDim.x * blockDim.x);
 }
 
-// Launch for (radius, levels) in {(4,4), (3,4)}; returns false when the configuration has no window instantiation.
-inline bool lookup_win_launch(const LookupParams& p, int levels, int radius, cudaStream_t st) {
+// The window kernel instantiation for (radius, levels) in {(4,4), (3,4)}; null when the configuration has none.
+using LookupKernel = void (*)(LookupParams);
+inline LookupKernel lookup_win_kernel(const LookupParams& p, int levels, int radius) {
   const size_t nwork = (size_t)p.nq * levels;
-  if (levels != 4 || (radius != 4 && radius != 3) || nwork >= (1u << 31)) return false;
+  if (levels != 4 || (radius != 4 && radius != 3) || nwork >= (1u << 31)) return nullptr;
   if ((size_t)p.nq * p.lh[0] * p.lw[0] >= (1u << 31) || (size_t)p.nq * (size_t)(p.out_hi ? p.h_stride : p.out_stride) >= (1u << 31))
-    return false;                                                    // 32-bit element offsets inside the kernel
+    return nullptr;                                                  // 32-bit element offsets inside the kernel
   bool vec = true;                                                  // 128-bit loads need 16-byte aligned rows on every level
   for (int l = 0; l < levels; ++l)
     vec = vec && (p.lw[l] % 4 == 0) && ((reinterpret_cast<uintptr_t>(p.pyr[l]) & 15) == 0);
-  const int grid = grid_for(nwork * 32, 256, kNumSMs * 4);           // 4 resident blocks per SM (64 registers): one wave
   const bool half = p.out_hi != nullptr;
-  if (half == (p.out != nullptr)) return false;                      // exactly one of the two output forms
-#define RAFT_LOOKUP_LAUNCH(RR, VV, HH) corr_lookup_win_kernel<RR, 4, VV, HH><<<grid, 256, 0, st>>>(p)
+  if (half == (p.out != nullptr)) return nullptr;                    // exactly one of the two output forms
   if (radius == 4) {
-    if (vec) { if (half) RAFT_LOOKUP_LAUNCH(4, true, true); else RAFT_LOOKUP_LAUNCH(4, true, false); }
-    else { if (half) RAFT_LOOKUP_LAUNCH(4, false, true); else RAFT_LOOKUP_LAUNCH(4, false, false); }
-  } else {
-    if (vec) { if (half) RAFT_LOOKUP_LAUNCH(3, true, true); else RAFT_LOOKUP_LAUNCH(3, true, false); }
-    else { if (half) RAFT_LOOKUP_LAUNCH(3, false, true); else RAFT_LOOKUP_LAUNCH(3, false, false); }
+    if (vec) return half ? corr_lookup_win_kernel<4, 4, true, true> : corr_lookup_win_kernel<4, 4, true, false>;
+    return half ? corr_lookup_win_kernel<4, 4, false, true> : corr_lookup_win_kernel<4, 4, false, false>;
   }
-#undef RAFT_LOOKUP_LAUNCH
-  return true;
+  if (vec) return half ? corr_lookup_win_kernel<3, 4, true, true> : corr_lookup_win_kernel<3, 4, true, false>;
+  return half ? corr_lookup_win_kernel<3, 4, false, true> : corr_lookup_win_kernel<3, 4, false, false>;
 }
 
 }  // namespace raft

@@ -240,8 +240,7 @@ inline int mega_launch(MegaPlan& M, unsigned int* flags, size_t flag_words, bool
   unsigned grid = 0;
   RAFT_TRY(persistent_grid<update_mega_kernel>(kSmemMax, M.P.nitems, &grid));
   if (zero_flags) RAFT_CUDA_TRY(cudaMemsetAsync(flags, 0, ((size_t)M.nflags + 1) * sizeof(unsigned int), stream));
-  update_mega_kernel<<<grid, kTcThreads, kSmemMax, stream>>>(M.P);
-  return raft_launch_status();
+  return launch(update_mega_kernel, grid, kTcThreads, kSmemMax, stream, M.P);
 }
 
 }  // namespace raft

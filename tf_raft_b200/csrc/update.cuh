@@ -9,9 +9,6 @@
 
 namespace raft {
 
-extern thread_local long long g_launches;
-#define RAFT_COUNT_LAUNCH() (++::raft::g_launches)
-
 // ------------------------------------------------------------------------------------------------
 // Reference convolutions, in raft_basic_weights / raft_small_weights member order.
 // ------------------------------------------------------------------------------------------------
@@ -42,34 +39,34 @@ struct TcLayerSpec {
   int nsrc, src[2];            // reference conv indices merged along cout
   int kh, kw;
   int cin_pad, cout_pad;       // packed dims
-  int nrange, r_src0[2], r_n[2], r_dst0[2];   // cin remap
+  TcCinMap cin_map;
   int bn, ntn;                 // N per column tile, column tiles (launch_tc_layer splits bn > kMaxTileN further)
   int flatten;                 // 1: (kh,kw,cin) flattened into the channel axis -- the layer runs as a 1x1 conv on im2col planes
 };
 
 static const TcLayerSpec kBasicTc[12] = {
-    /*T0 convc1 */ {1, {BC1, -1}, 1, 1, 384, 256, 1, {0, 0}, {324, 0}, {0, 0}, 256, 1},
-    /*T1 convc2 */ {1, {BC2, -1}, 3, 3, 256, 192, 1, {0, 0}, {256, 0}, {0, 0}, 192, 1},
-    /*T2 convf2 */ {1, {BF2, -1}, 3, 3, 128, 64, 1, {0, 0}, {128, 0}, {0, 0}, 64, 1},
-    /*T3 conv   */ {1, {BCV, -1}, 3, 3, 256, 128, 1, {0, 0}, {256, 0}, {0, 0}, 128, 1},
-    /*T4 zr1    */ {2, {BZ1, BR1}, 1, 5, 384, 256, 1, {0, 0}, {384, 0}, {0, 0}, 256, 1},
-    /*T5 q1     */ {1, {BQ1, -1}, 1, 5, 384, 128, 1, {0, 0}, {384, 0}, {0, 0}, 128, 1},
-    /*T6 zr2    */ {2, {BZ2, BR2}, 5, 1, 384, 256, 1, {0, 0}, {384, 0}, {0, 0}, 256, 1},
-    /*T7 q2     */ {1, {BQ2, -1}, 5, 1, 384, 128, 1, {0, 0}, {384, 0}, {0, 0}, 128, 1},
-    /*T8 fh1|m0 */ {2, {BFH1, BM0}, 3, 3, 128, 512, 1, {0, 0}, {128, 0}, {0, 0}, 256, 2},
-    /*T9 fh2    */ {1, {BFH2, -1}, 3, 3, 256, 16, 1, {0, 0}, {256, 0}, {0, 0}, 16, 1},
-    /*T10 mask2 */ {1, {BM2, -1}, 1, 1, 256, 576, 1, {0, 0}, {256, 0}, {0, 0}, 192, 3},
-    /*T11 convf1*/ {1, {BF1, -1}, 1, 1, 128, 128, 1, {0, 0}, {98, 0}, {0, 0}, 128, 1, 1}};
+    /*T0 convc1 */ {1, {BC1, -1}, 1, 1, 384, 256, {1, {0, 0}, {324, 0}, {0, 0}}, 256, 1},
+    /*T1 convc2 */ {1, {BC2, -1}, 3, 3, 256, 192, {1, {0, 0}, {256, 0}, {0, 0}}, 192, 1},
+    /*T2 convf2 */ {1, {BF2, -1}, 3, 3, 128, 64, {1, {0, 0}, {128, 0}, {0, 0}}, 64, 1},
+    /*T3 conv   */ {1, {BCV, -1}, 3, 3, 256, 128, {1, {0, 0}, {256, 0}, {0, 0}}, 128, 1},
+    /*T4 zr1    */ {2, {BZ1, BR1}, 1, 5, 384, 256, {1, {0, 0}, {384, 0}, {0, 0}}, 256, 1},
+    /*T5 q1     */ {1, {BQ1, -1}, 1, 5, 384, 128, {1, {0, 0}, {384, 0}, {0, 0}}, 128, 1},
+    /*T6 zr2    */ {2, {BZ2, BR2}, 5, 1, 384, 256, {1, {0, 0}, {384, 0}, {0, 0}}, 256, 1},
+    /*T7 q2     */ {1, {BQ2, -1}, 5, 1, 384, 128, {1, {0, 0}, {384, 0}, {0, 0}}, 128, 1},
+    /*T8 fh1|m0 */ {2, {BFH1, BM0}, 3, 3, 128, 512, {1, {0, 0}, {128, 0}, {0, 0}}, 256, 2},
+    /*T9 fh2    */ {1, {BFH2, -1}, 3, 3, 256, 16, {1, {0, 0}, {256, 0}, {0, 0}}, 16, 1},
+    /*T10 mask2 */ {1, {BM2, -1}, 1, 1, 256, 576, {1, {0, 0}, {256, 0}, {0, 0}}, 192, 3},
+    /*T11 convf1*/ {1, {BF1, -1}, 1, 1, 128, 128, {1, {0, 0}, {98, 0}, {0, 0}}, 128, 1, 1}};
 
 static const TcLayerSpec kSmallTc[8] = {
-    /*S0 convc1 */ {1, {SC1, -1}, 1, 1, 256, 96, 1, {0, 0}, {196, 0}, {0, 0}, 96, 1},
-    /*S1 convf2 */ {1, {SF2, -1}, 3, 3, 64, 32, 1, {0, 0}, {64, 0}, {0, 0}, 32, 1},
-    /*S2 conv   */ {1, {SCV, -1}, 3, 3, 128, 96, 1, {0, 0}, {128, 0}, {0, 0}, 96, 1},
-    /*S3 zr     */ {2, {SZ, SR}, 3, 3, 320, 192, 2, {0, 96}, {96, 146}, {0, 128}, 192, 1},
-    /*S4 q      */ {1, {SQ, -1}, 3, 3, 320, 96, 2, {0, 96}, {96, 146}, {0, 128}, 96, 1},
-    /*S5 fh1    */ {1, {SFH1, -1}, 3, 3, 128, 128, 1, {0, 0}, {96, 0}, {0, 0}, 128, 1},
-    /*S6 fh2    */ {1, {SFH2, -1}, 3, 3, 128, 16, 1, {0, 0}, {128, 0}, {0, 0}, 16, 1},
-    /*S7 convf1 */ {1, {SF1, -1}, 1, 1, 128, 64, 1, {0, 0}, {98, 0}, {0, 0}, 64, 1, 1}};
+    /*S0 convc1 */ {1, {SC1, -1}, 1, 1, 256, 96, {1, {0, 0}, {196, 0}, {0, 0}}, 96, 1},
+    /*S1 convf2 */ {1, {SF2, -1}, 3, 3, 64, 32, {1, {0, 0}, {64, 0}, {0, 0}}, 32, 1},
+    /*S2 conv   */ {1, {SCV, -1}, 3, 3, 128, 96, {1, {0, 0}, {128, 0}, {0, 0}}, 96, 1},
+    /*S3 zr     */ {2, {SZ, SR}, 3, 3, 320, 192, {2, {0, 96}, {96, 146}, {0, 128}}, 192, 1},
+    /*S4 q      */ {1, {SQ, -1}, 3, 3, 320, 96, {2, {0, 96}, {96, 146}, {0, 128}}, 96, 1},
+    /*S5 fh1    */ {1, {SFH1, -1}, 3, 3, 128, 128, {1, {0, 0}, {96, 0}, {0, 0}}, 128, 1},
+    /*S6 fh2    */ {1, {SFH2, -1}, 3, 3, 128, 16, {1, {0, 0}, {128, 0}, {0, 0}}, 16, 1},
+    /*S7 convf1 */ {1, {SF1, -1}, 1, 1, 128, 64, {1, {0, 0}, {98, 0}, {0, 0}}, 64, 1, 1}};
 
 inline int n_tc_layers(int variant) { return variant == RAFT_VARIANT_BASIC ? 12 : 8; }
 inline const TcLayerSpec* tc_layers(int variant) { return variant == RAFT_VARIANT_BASIC ? kBasicTc : kSmallTc; }
@@ -79,11 +76,9 @@ inline const TcLayerSpec* tc_layers(int variant) { return variant == RAFT_VARIAN
 // ------------------------------------------------------------------------------------------------
 struct PreparedLayout {
   size_t raw_w[15], raw_b[15];                 // fp32 copies of every reference conv (HWIO) + bias
-  size_t tc_hi[12], tc_lo[12], tc_bias[12], tc_scale[12], tc_absmax[12];
+  TcWeightSlot tc[12];                         // packed weights of every tensor-core layer (F16X2 only)
   size_t total;
 };
-
-inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
 inline PreparedLayout prepared_layout(int variant, int precision) {
   PreparedLayout L;
@@ -98,19 +93,8 @@ inline PreparedLayout prepared_layout(int variant, int precision) {
   }
   if (precision == RAFT_PREC_F16X2) {
     const TcLayerSpec* tl = tc_layers(variant);
-    for (int i = 0; i < n_tc_layers(variant); ++i) {
-      const size_t plane = (size_t)tl[i].kh * tl[i].kw * tl[i].cout_pad * tl[i].cin_pad * sizeof(__half);
-      L.tc_hi[i] = off;
-      off = align_up(off + plane, 256);
-      L.tc_lo[i] = off;
-      off = align_up(off + plane, 256);
-      L.tc_bias[i] = off;
-      off = align_up(off + sizeof(float) * (tl[i].cout_pad + 64), 256);
-      L.tc_scale[i] = off;
-      off = align_up(off + 2 * sizeof(float), 256);
-      L.tc_absmax[i] = off;
-      off = align_up(off + sizeof(unsigned int), 256);
-    }
+    for (int i = 0; i < n_tc_layers(variant); ++i)
+      L.tc[i] = tc_weight_slot(off, tl[i].kh, tl[i].kw, tl[i].cin_pad, tl[i].cout_pad);
   }
   L.total = off;
   return L;
@@ -123,16 +107,20 @@ struct VariantDims {
   int hid, ctx, corr_ch;
   int c_cor1, c_cf, c_flo1, c_x, c_fm;        // fp32-path plane widths
   int s_corr, s_cor1, s_cf, s_flo1, s_x, s_h, s_fm;   // fp16-plane channel strides (multiples of 64)
-  int x_motion_c0, motion_n;                  // where the motion-encoder output lands inside x
 };
 inline VariantDims variant_dims(int variant) {
-  if (variant == RAFT_VARIANT_BASIC) return {128, 128, 324, 256, 256, 128, 256, 512, 384, 256, 256, 128, 256, 128, 512, 128, 126};
-  return {96, 64, 196, 0, 128, 64, 148, 128, 256, 0, 128, 64, 192, 128, 128, 64, 80};
+  if (variant == RAFT_VARIANT_BASIC)
+    return {.hid = 128, .ctx = 128, .corr_ch = 324,
+            .c_cor1 = 256, .c_cf = 256, .c_flo1 = 128, .c_x = 256, .c_fm = 512,
+            .s_corr = 384, .s_cor1 = 256, .s_cf = 256, .s_flo1 = 128, .s_x = 256, .s_h = 128, .s_fm = 512};
+  return {.hid = 96, .ctx = 64, .corr_ch = 196,
+          .c_cor1 = 0, .c_cf = 128, .c_flo1 = 64, .c_x = 148, .c_fm = 128,
+          .s_corr = 256, .s_cor1 = 0, .s_cf = 128, .s_flo1 = 64, .s_x = 192, .s_h = 128, .s_fm = 128};
 }
 
 struct Workspace {
   // fp32 planes
-  float *corr, *cor1, *cf, *flo1, *x, *z, *r, *rh, *q, *fm, *flow, *delta, *mask, *net_tmp;
+  float *corr, *cor1, *cf, *flo1, *x, *z, *r, *rh, *q, *fm, *flow, *delta, *mask;
   // fp16 hi/lo planes (tensor-core path)
   __half *corr_hi, *corr_lo, *cor1_hi, *cor1_lo, *cf_hi, *cf_lo, *flo1_hi, *flo1_lo, *x_hi, *x_lo, *h_hi, *h_lo,
       *rh_hi, *rh_lo, *fm_hi, *fm_lo, *fim_hi, *fim_lo;
@@ -162,7 +150,6 @@ inline Workspace workspace_layout(void* base, int variant, int B, int h, int w, 
   W.delta = f32(2);
   W.mask = f32(576);
   W.z = f32(d.hid);
-  W.net_tmp = f32(d.hid);
   if (precision == RAFT_PREC_FP32) {
     W.corr = f32(d.corr_ch);
     if (d.c_cor1) W.cor1 = f32(d.c_cor1);
@@ -233,9 +220,7 @@ inline int launch_simt_conv(const UpdateCtx& c, int conv_idx, int nsrc, const fl
   p.act = act; p.out_scale = out_scale;
   const int npix = c.B * c.h * c.w;
   dim3 grid((unsigned)ceil_div(npix, 64), (unsigned)ceil_div(cd.cout, 64));
-  conv_simt_kernel<<<grid, 256, 0, c.stream>>>(p);
-  RAFT_COUNT_LAUNCH();
-  return raft_launch_status();
+  return launch(conv_simt_kernel, grid, 256, 0, c.stream, p);
 }
 
 inline int simt1(const UpdateCtx& c, int conv_idx, const float* src, int stride, int c0, int n, float* out, int out_stride,
@@ -269,24 +254,17 @@ inline int launch_tc_layer(const UpdateCtx& c, int layer, int nseg, const TcSeg*
     chunks += segs[i].chunks;
   }
   if (chunks * kChunkK != L.cin_pad) return RAFT_ERR_BAD_SHAPE;
-  const __half* whi = reinterpret_cast<const __half*>(c.prepared + c.PL.tc_hi[layer]);
-  const __half* wlo = reinterpret_cast<const __half*>(c.prepared + c.PL.tc_lo[layer]);
   const int nsplit = tc_n_split(L.bn);                // layers wider than kMaxTileN run as more column tiles
   if (!nsplit) return RAFT_ERR_BAD_SHAPE;
-  const int bn = L.bn / nsplit;
-  RAFT_TRY(make_tmap_wgt2(&p.b_map, whi, wlo, L.kh * L.kw, L.cout_pad, L.cin_pad, bn));
-  p.kh = L.kh; p.kw = L.kw; p.ph = (L.kh - 1) / 2; p.pw = (L.kw - 1) / 2;
+  RAFT_TRY(tc_use_weights(p, c.prepared, c.PL.tc[layer], L.bn / nsplit));
+  p.ph = (L.kh - 1) / 2; p.pw = (L.kw - 1) / 2;
   p.B = c.B; p.H = c.h; p.W = c.w; p.TH = th; p.TW = tw;
-  p.bn = bn;
-  p.bias = reinterpret_cast<const float*>(c.prepared + c.PL.tc_bias[layer]);
-  p.inv_scale = reinterpret_cast<const float*>(c.prepared + c.PL.tc_scale[layer]) + 1;
   if (p.out_scale == 0.0f) p.out_scale = 1.0f;
   // Promotion group of the update-block layers: 2 chunks (24-MMA chains).  Their K = 1920 GRU contractions feed a
   // 12-iteration recurrence (DESIGN.md section 4).
   p.group_chunks = 2;
   const int n_tiles_n = (ntn > 0 ? ntn : L.ntn) * nsplit;
   if (c.plan) return mega_add(*c.plan, layer, p, n_tiles_n, nsplit, deps);
-  RAFT_COUNT_LAUNCH();
   return tc_launch(p, n_tiles_n, c.stream);
 }
 
