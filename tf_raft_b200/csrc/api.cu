@@ -146,210 +146,6 @@ static int corr_build_tc(const float* f1, const float* f2, int B, int h, int w, 
   return launch(corr_tc_kernel, grid, kTcThreads, kCorrSmemBytes, st, p);
 }
 
-// ------------------------------------------------------------------------------------------------
-// Update block, fp32 FFMA path: the reference's op sequence, one launch per Conv2D.
-// ------------------------------------------------------------------------------------------------
-static int gru_fp32(const UpdateCtx& c, float* h, int iz, int ir, int iq, int hid, int xs, int xn) {
-  const Workspace& W = c.W;
-  const size_t n = (size_t)c.B * c.h * c.w * hid;
-  RAFT_TRY(simt2(c, iz, h, hid, hid, W.x, xs, xn, W.z, hid, SACT_SIGMOID));
-  RAFT_TRY(simt2(c, ir, h, hid, hid, W.x, xs, xn, W.r, hid, SACT_SIGMOID));
-  RAFT_TRY(launch(gru_rh_kernel, grid_for(n), 256, 0, c.stream, W.r, h, W.rh, n));
-  RAFT_TRY(simt2(c, iq, W.rh, hid, hid, W.x, xs, xn, W.q, hid, SACT_TANH));
-  return launch(gru_update_kernel, grid_for(n), 256, 0, c.stream, W.z, W.q, h, n);
-}
-
-static int update_core_fp32(const UpdateCtx& c, float* h, float* delta, float* mask) {
-  const Workspace& W = c.W;
-  const VariantDims d = variant_dims(c.variant);
-  const size_t npix = (size_t)c.B * c.h * c.w;
-  if (c.variant == RAFT_VARIANT_BASIC) {
-    RAFT_TRY(simt1(c, BC1, W.corr, 324, 0, 324, W.cor1, 256, 0, SACT_RELU));           // update.py:98
-    RAFT_TRY(simt1(c, BC2, W.cor1, 256, 0, 256, W.cf, 256, 0, SACT_RELU));              // :99
-    RAFT_TRY(simt1(c, BF1, W.flow, 2, 0, 2, W.flo1, 128, 0, SACT_RELU));                // :100
-    RAFT_TRY(simt1(c, BF2, W.flo1, 128, 0, 128, W.cf, 256, 192, SACT_RELU));            // :101,104
-    RAFT_TRY(simt1(c, BCV, W.cf, 256, 0, 256, W.x, 256, 128, SACT_RELU));               // :105
-    RAFT_TRY(launch(copy_channels_kernel, grid_for(npix * 2), 256, 0, c.stream, W.flow, 2, 0, W.x, 256, 254, 2, npix));  // :106
-    RAFT_TRY(gru_fp32(c, h, BZ1, BR1, BQ1, 128, 256, 256));                             // :53-58
-    RAFT_TRY(gru_fp32(c, h, BZ2, BR2, BQ2, 128, 256, 256));                             // :60-65
-    RAFT_TRY(simt1(c, BFH1, h, 128, 0, 128, W.fm, 512, 0, SACT_RELU));                  // :14
-    RAFT_TRY(simt1(c, BFH2, W.fm, 512, 0, 256, delta, 2, 0, SACT_NONE));
-    if (mask) {
-      RAFT_TRY(simt1(c, BM0, h, 128, 0, 128, W.fm, 512, 256, SACT_RELU));               // :137-141
-      RAFT_TRY(simt1(c, BM2, W.fm, 512, 256, 256, mask, 576, 0, SACT_NONE, 0.25f));     // :152
-    }
-  } else {
-    RAFT_TRY(simt1(c, SC1, W.corr, 196, 0, 196, W.cf, 128, 0, SACT_RELU));              // update.py:80
-    RAFT_TRY(simt1(c, SF1, W.flow, 2, 0, 2, W.flo1, 64, 0, SACT_RELU));                 // :81
-    RAFT_TRY(simt1(c, SF2, W.flo1, 64, 0, 64, W.cf, 128, 96, SACT_RELU));               // :82-83
-    RAFT_TRY(simt1(c, SCV, W.cf, 128, 0, 128, W.x, d.c_x, 64, SACT_RELU));              // :84
-    RAFT_TRY(launch(copy_channels_kernel, grid_for(npix * 2), 256, 0, c.stream, W.flow, 2, 0, W.x, d.c_x, 144, 2, npix));  // :85
-    RAFT_TRY(gru_fp32(c, h, SZ, SR, SQ, 96, d.c_x, 146));                               // :26-35
-    RAFT_TRY(simt1(c, SFH1, h, 96, 0, 96, W.fm, 128, 0, SACT_RELU));
-    RAFT_TRY(simt1(c, SFH2, W.fm, 128, 0, 128, delta, 2, 0, SACT_NONE));
-  }
-  return raft_launch_status();
-}
-
-// ------------------------------------------------------------------------------------------------
-// Update block, tensor-core path.  Operands travel between layers as fp16 hi/lo planes written by
-// the producing layer's epilogue; z||r and flow_head.conv1||mask[0] are single GEMMs.
-// ------------------------------------------------------------------------------------------------
-static void tc_params_init(TcConvParams& p, int mode, int act, int n_total) {
-  memset(&p, 0, sizeof(p));
-  p.mode = mode;
-  p.act = act;
-  p.n_total = n_total;
-  p.out_scale = 1.0f;
-}
-
-static TcDeps dep1(int layer, int ntile = -1) { return TcDeps{1, {layer, -1}, {ntile, -1}}; }
-static TcDeps dep2(int l0, int l1) { return TcDeps{2, {l0, l1}, {-1, -1}}; }
-
-static int gru_tc(const UpdateCtx& c, float* h, int lzr, int lq, int hid, int x_chunks, int src_layer) {
-  const Workspace& W = c.W;
-  const VariantDims d = variant_dims(c.variant);
-  TcConvParams p;
-  {
-    tc_params_init(p, EPI_GRU_ZR, ACT_NONE, 2 * hid);
-    p.z = W.z; p.h = h; p.hid = hid;
-    p.out_hi = W.rh_hi; p.out_lo = W.rh_lo; p.h_stride = d.s_h; p.h_c0 = 0;
-    TcSeg segs[2] = {{W.h_hi, W.h_lo, d.s_h, 0, d.s_h / kChunkK}, {W.x_hi, W.x_lo, d.s_x, 0, x_chunks}};
-    RAFT_TRY(launch_tc_layer(c, lzr, 2, segs, p, -1, dep1(src_layer)));
-  }
-  {
-    tc_params_init(p, EPI_GRU_Q, ACT_NONE, hid);
-    p.z = W.z; p.h = h; p.hid = hid;
-    p.out_hi = W.h_hi; p.out_lo = W.h_lo; p.h_stride = d.s_h; p.h_c0 = 0;
-    TcSeg segs[2] = {{W.rh_hi, W.rh_lo, d.s_h, 0, d.s_h / kChunkK}, {W.x_hi, W.x_lo, d.s_x, 0, x_chunks}};
-    RAFT_TRY(launch_tc_layer(c, lq, 2, segs, p, -1, dep1(lzr)));
-  }
-  return 0;
-}
-
-// Flow branch of BasicMotionEncoder (update.py:98-99): convf1 7x7 2->128 + relu, convf2 3x3 128->64 + relu ->
-// cor_flo[192:256).  Depends only on the current flow, so it may run beside the lookup and the correlation branch.
-// (two parts, so that the work list of update_mega_kernel can interleave them with the correlation branch: the list order is
-//  the order in which free CTAs claim items)
-static int flow_branch_basic_tc(const UpdateCtx& c, int part) {
-  const Workspace& W = c.W;
-  const VariantDims d = variant_dims(c.variant);
-  TcConvParams p;
-  if (part == 0) {  // convf1 7x7 2->128 + relu: K = 98 -> gather the window into 128-channel planes, run as a 1x1 GEMM
-    const size_t npix = (size_t)c.B * c.h * c.w;
-    if (!c.fim_ready) {              // (the iteration loop's lookup kernel has already produced the planes)
-      RAFT_TRY(launch(flow_im2col_kernel, grid_for(npix * 128), 256, 0, c.stream, W.flow, c.B, c.h, c.w, W.fim_hi, W.fim_lo));
-    }
-    tc_params_init(p, EPI_LINEAR, ACT_RELU, 128);
-    p.out_hi = W.flo1_hi; p.out_lo = W.flo1_lo; p.h_stride = d.s_flo1;
-    TcSeg s[1] = {{W.fim_hi, W.fim_lo, 128, 0, 2}};
-    RAFT_TRY(launch_tc_layer(c, 11, 1, s, p));
-  } else {  // convf2 3x3 128->64 + relu -> cor_flo[192:256)
-    tc_params_init(p, EPI_LINEAR, ACT_RELU, 64);
-    p.out_hi = W.cf_hi; p.out_lo = W.cf_lo; p.h_stride = d.s_cf; p.h_c0 = 192;
-    TcSeg s[1] = {{W.flo1_hi, W.flo1_lo, d.s_flo1, 0, 2}};
-    RAFT_TRY(launch_tc_layer(c, 2, 1, s, p, -1, dep1(11)));
-  }
-  return 0;
-}
-
-// adv_coords != null (iteration loop): the flow-head epilogue also applies coords1 += delta and flow = coords1 - grid.
-static int update_core_tc(const UpdateCtx& c, float* h, float* delta, float* mask, float* adv_coords = nullptr) {
-  const Workspace& W = c.W;
-  const VariantDims d = variant_dims(c.variant);
-  TcConvParams p;
-  if (c.variant == RAFT_VARIANT_BASIC) {
-    {  // convc1 1x1 324->256 + relu
-      tc_params_init(p, EPI_LINEAR, ACT_RELU, 256);
-      p.out_hi = W.cor1_hi; p.out_lo = W.cor1_lo; p.h_stride = d.s_cor1;
-      TcSeg s[1] = {{W.corr_hi, W.corr_lo, d.s_corr, 0, d.s_corr / kChunkK}};
-      RAFT_TRY(launch_tc_layer(c, 0, 1, s, p));
-    }
-    RAFT_TRY(flow_branch_basic_tc(c, 0));                   // convf1 (update.py:98)
-    {  // convc2 3x3 256->192 + relu -> cor_flo[0:192)
-      tc_params_init(p, EPI_LINEAR, ACT_RELU, 192);
-      p.out_hi = W.cf_hi; p.out_lo = W.cf_lo; p.h_stride = d.s_cf;
-      TcSeg s[1] = {{W.cor1_hi, W.cor1_lo, d.s_cor1, 0, 4}};
-      RAFT_TRY(launch_tc_layer(c, 1, 1, s, p, -1, dep1(0)));
-    }
-    RAFT_TRY(flow_branch_basic_tc(c, 1));                   // convf2 (update.py:99)
-    {  // conv 3x3 256->126 + relu, concat flow -> x[128:256)
-      tc_params_init(p, EPI_LINEAR, ACT_RELU, 126);
-      p.out_hi = W.x_hi; p.out_lo = W.x_lo; p.h_stride = d.s_x; p.h_c0 = 128;
-      p.concat_src = W.flow; p.concat_n = 2;
-      TcSeg s[1] = {{W.cf_hi, W.cf_lo, d.s_cf, 0, 4}};
-      RAFT_TRY(launch_tc_layer(c, 3, 1, s, p, -1, dep2(1, 2)));
-    }
-    RAFT_TRY(gru_tc(c, h, 4, 5, 128, 4, 3));
-    RAFT_TRY(gru_tc(c, h, 6, 7, 128, 4, 5));
-    {  // flow_head.conv1 || mask[0], 3x3 128->512 + relu
-      tc_params_init(p, EPI_LINEAR, ACT_RELU, mask ? 512 : 256);
-      p.out_hi = W.fm_hi; p.out_lo = W.fm_lo; p.h_stride = d.s_fm;
-      TcSeg s[1] = {{W.h_hi, W.h_lo, d.s_h, 0, 2}};
-      RAFT_TRY(launch_tc_layer(c, 8, 1, s, p, mask ? 2 : 1, dep1(7)));
-    }
-    {  // flow_head.conv2 3x3 256->2
-      tc_params_init(p, EPI_LINEAR, ACT_NONE, 2);
-      p.out_f32 = delta; p.f32_stride = 2;
-      p.adv_coords = adv_coords; p.adv_flow = adv_coords ? W.flow : nullptr;
-      TcSeg s[1] = {{W.fm_hi, W.fm_lo, d.s_fm, 0, 4}};
-      RAFT_TRY(launch_tc_layer(c, 9, 1, s, p, -1, dep1(8, 0)));
-    }
-    if (mask) {  // mask[2] 1x1 256->576, x0.25
-      tc_params_init(p, EPI_LINEAR, ACT_NONE, 576);
-      p.out_f32 = mask; p.f32_stride = 576; p.out_scale = 0.25f;
-      TcSeg s[1] = {{W.fm_hi, W.fm_lo, d.s_fm, 256, 4}};
-      RAFT_TRY(launch_tc_layer(c, 10, 1, s, p, -1, dep1(8, 1)));
-    }
-  } else {
-    {  // convc1 1x1 196->96 + relu -> cor_flo[0:96)
-      tc_params_init(p, EPI_LINEAR, ACT_RELU, 96);
-      p.out_hi = W.cf_hi; p.out_lo = W.cf_lo; p.h_stride = d.s_cf;
-      TcSeg s[1] = {{W.corr_hi, W.corr_lo, d.s_corr, 0, 4}};
-      RAFT_TRY(launch_tc_layer(c, 0, 1, s, p));
-    }
-    {  // convf1 7x7 2->64 + relu via im2col + 1x1 GEMM
-      const size_t npix = (size_t)c.B * c.h * c.w;
-      if (!c.fim_ready) {
-        RAFT_TRY(launch(flow_im2col_kernel, grid_for(npix * 128), 256, 0, c.stream, W.flow, c.B, c.h, c.w, W.fim_hi,
-                        W.fim_lo));
-      }
-      tc_params_init(p, EPI_LINEAR, ACT_RELU, 64);
-      p.out_hi = W.flo1_hi; p.out_lo = W.flo1_lo; p.h_stride = d.s_flo1;
-      TcSeg s[1] = {{W.fim_hi, W.fim_lo, 128, 0, 2}};
-      RAFT_TRY(launch_tc_layer(c, 7, 1, s, p));
-    }
-    {  // convf2 3x3 64->32 + relu -> cor_flo[96:128)
-      tc_params_init(p, EPI_LINEAR, ACT_RELU, 32);
-      p.out_hi = W.cf_hi; p.out_lo = W.cf_lo; p.h_stride = d.s_cf; p.h_c0 = 96;
-      TcSeg s[1] = {{W.flo1_hi, W.flo1_lo, d.s_flo1, 0, 1}};
-      RAFT_TRY(launch_tc_layer(c, 1, 1, s, p, -1, dep1(7)));
-    }
-    {  // conv 3x3 128->80 + relu, concat flow -> x[64:160)
-      tc_params_init(p, EPI_LINEAR, ACT_RELU, 80);
-      p.out_hi = W.x_hi; p.out_lo = W.x_lo; p.h_stride = d.s_x; p.h_c0 = 64;
-      p.concat_src = W.flow; p.concat_n = 2;
-      TcSeg s[1] = {{W.cf_hi, W.cf_lo, d.s_cf, 0, 2}};
-      RAFT_TRY(launch_tc_layer(c, 2, 1, s, p, -1, dep2(0, 1)));
-    }
-    RAFT_TRY(gru_tc(c, h, 3, 4, 96, 3, 2));
-    {  // flow_head.conv1 3x3 96->128 + relu
-      tc_params_init(p, EPI_LINEAR, ACT_RELU, 128);
-      p.out_hi = W.fm_hi; p.out_lo = W.fm_lo; p.h_stride = d.s_fm;
-      TcSeg s[1] = {{W.h_hi, W.h_lo, d.s_h, 0, 2}};
-      RAFT_TRY(launch_tc_layer(c, 5, 1, s, p, -1, dep1(4)));
-    }
-    {  // flow_head.conv2 3x3 128->2
-      tc_params_init(p, EPI_LINEAR, ACT_NONE, 2);
-      p.out_f32 = delta; p.f32_stride = 2;
-      p.adv_coords = adv_coords; p.adv_flow = adv_coords ? W.flow : nullptr;
-      TcSeg s[1] = {{W.fm_hi, W.fm_lo, d.s_fm, 0, 2}};
-      RAFT_TRY(launch_tc_layer(c, 6, 1, s, p, -1, dep1(5)));
-    }
-  }
-  return 0;
-}
-
 // Per-pair setup shared by the update_* entry points and the loop: zero the fp16 planes (their
 // padded channels must hold exact zeros), stage inp and the hidden state in operand format.
 static int update_begin(const UpdateCtx& c, const float* h, const float* inp) {
@@ -635,11 +431,11 @@ int raft_b200_update_prepare(int variant, const void* weights, void* prepared, s
     RAFT_CUDA_TRY(cudaMemcpyAsync(base + L.raw_b[i], convs[i].bias, cd[i].cout * sizeof(float), cudaMemcpyDeviceToDevice, st));
   }
   if (precision == RAFT_PREC_F16X2) {
-    const TcLayerSpec* tl = tc_layers(variant);
+    const TcLayer* tl = tc_layers(variant);
     for (int li = 0; li < n_tc_layers(variant); ++li) {
-      const TcLayerSpec& T = tl[li];
+      const TcLayer& T = tl[li];
       const raft_conv* src[2] = {&convs[T.src[0]], T.nsrc > 1 ? &convs[T.src[1]] : nullptr};
-      RAFT_TRY(tc_pack_weights(base, L.tc[li], src, T.nsrc, &T.cin_map, T.flatten != 0, st));
+      RAFT_TRY(tc_pack_weights(base, L.tc[li], src, T.nsrc, T.cin_map.nrange ? &T.cin_map : nullptr, T.flatten != 0, st));
     }
   }
   return raft_launch_status();

@@ -177,27 +177,24 @@ __global__ void __launch_bounds__(kTcThreads, 1) update_mega_kernel(const __grid
 // ------------------------------------------------------------------------------------------------
 // Host side: the plan of one update-block application.
 // ------------------------------------------------------------------------------------------------
-struct TcDeps { int n; int layer[2]; int ntile[2]; };            // by tensor-core layer id (update.cuh tables)
+// A layer reads output columns [col0, col1) of an earlier layer of the plan (col1 == 0: all of them).
+struct MegaDep { int layer, col0, col1; };
 
 struct MegaPlan {
   MegaParams P;
-  int pos_of_layer[32];          // tensor-core layer id -> position in P.layer (-1: not planned)
-  int nsplit[kMegaMaxLayers];    // column tiles per column tile of the layer's table entry (tc_n_split)
   int nflags;
   MegaPlan() {
     memset(&P, 0, sizeof(P));
-    for (int i = 0; i < 32; ++i) pos_of_layer[i] = -1;
     nflags = 0;
   }
 };
 
 inline int mega_flag_words(int B, int tiles) { return kMegaMaxLayers * 6 * B * tiles + 1; }   // upper bound used by the workspace layout
 
-// Appends a planned layer (p complete except for the launch fields).  Mirrors the checks of tc_launch().  nsplit: the
-// layer's column tiles are its table's column tiles split nsplit ways, so a dependency on table tile j reads tiles
-// [j * nsplit, (j + 1) * nsplit).
-inline int mega_add(MegaPlan& M, int layer_id, TcConvParams& p, int n_tiles_n, int nsplit, const TcDeps& deps) {
-  if (M.P.nlayers >= kMegaMaxLayers || layer_id < 0 || layer_id >= 32) return RAFT_ERR_UNSUPPORTED;
+// Appends a planned layer (p complete except for the launch fields).  Mirrors the checks of tc_launch().  A dependency
+// waits on the source's column tiles that hold the columns it reads.
+inline int mega_add(MegaPlan& M, TcConvParams& p, int n_tiles_n, int ndep, const MegaDep deps[]) {
+  if (M.P.nlayers >= kMegaMaxLayers || ndep < 0 || ndep > 2) return RAFT_ERR_UNSUPPORTED;
   RAFT_TRY(tc_check(p));
   if (p.stride < 1) p.stride = 1;
   tc_finalize(p);
@@ -209,21 +206,20 @@ inline int mega_add(MegaPlan& M, int layer_id, TcConvParams& p, int n_tiles_n, i
   const int mtiles = p.B * p.tiles_y * p.tiles_x;
   ML.item0 = M.P.nitems;
   ML.flag0 = M.nflags;
-  ML.ndep = deps.n;
-  for (int d = 0; d < deps.n; ++d) {
-    const int pos = M.pos_of_layer[deps.layer[d]];
-    if (pos < 0) return RAFT_ERR_BAD_ARG;            // a source layer must be planned before its consumer
-    ML.dep_layer[d] = pos;
-    const int f = M.nsplit[pos];
-    ML.dep_nlo[d] = deps.ntile[d] < 0 ? 0 : deps.ntile[d] * f;
-    ML.dep_nhi[d] = deps.ntile[d] < 0 ? M.P.layer[pos].c.n_tiles_n - 1 : deps.ntile[d] * f + f - 1;
+  ML.ndep = ndep;
+  for (int d = 0; d < ndep; ++d) {
+    const MegaDep& D = deps[d];
+    if (D.layer < 0 || D.layer >= M.P.nlayers) return RAFT_ERR_BAD_ARG;   // a source layer is planned before its consumer
+    const TcConvParams& s = M.P.layer[D.layer].c;
+    ML.dep_layer[d] = D.layer;
+    ML.dep_nlo[d] = D.col0 / s.bn;
+    ML.dep_nhi[d] = D.col1 > 0 ? (D.col1 - 1) / s.bn : s.n_tiles_n - 1;
+    if (ML.dep_nlo[d] > ML.dep_nhi[d] || ML.dep_nhi[d] >= s.n_tiles_n) return RAFT_ERR_BAD_ARG;
   }
   ML.dep_ry = ceil_div(p.ph > 0 ? p.ph : 1, p.TH);
   ML.dep_rx = ceil_div(p.pw > 0 ? p.pw : 1, p.TW);
   if (ML.dep_ry < 1) ML.dep_ry = 1;
   if (ML.dep_rx < 1) ML.dep_rx = 1;
-  M.pos_of_layer[layer_id] = M.P.nlayers;
-  M.nsplit[M.P.nlayers] = nsplit;
   M.P.nitems += mtiles * n_tiles_n;
   M.nflags += mtiles * n_tiles_n;
   ++M.P.nlayers;

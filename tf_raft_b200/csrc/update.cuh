@@ -32,44 +32,87 @@ inline int n_convs(int variant) { return variant == RAFT_VARIANT_BASIC ? 15 : 9;
 inline const ConvDim* conv_dims(int variant) { return variant == RAFT_VARIANT_BASIC ? kBasicConvs : kSmallConvs; }
 
 // ------------------------------------------------------------------------------------------------
-// Tensor-core layers: one or two reference convs merged along cout, cin remapped onto the
-// 64-channel-aligned operand planes.
+// Tensor-core layers (precision F16X2), one table per variant in work-list order: the order in which update_mega_kernel
+// hands out their tiles (list order is priority order), and the order of the per-layer launches.  A row is everything
+// about one layer: how its weights are packed, its tiling, the planes it reads, its epilogue and the rows it waits on.
 // ------------------------------------------------------------------------------------------------
-struct TcLayerSpec {
-  int nsrc, src[2];            // reference conv indices merged along cout
-  int kh, kw;
-  int cin_pad, cout_pad;       // packed dims
-  TcCinMap cin_map;
-  int bn, ntn;                 // N per column tile, column tiles (launch_tc_layer splits bn > kMaxTileN further)
-  int flatten;                 // 1: (kh,kw,cin) flattened into the channel axis -- the layer runs as a 1x1 conv on im2col planes
+// Operands: fp16 hi/lo planes of the workspace (channel stride from VariantDims; fim: 128), and the caller's fp32
+// outputs, which only an epilogue writes.
+enum TcPlane : int { PL_CORR, PL_COR1, PL_CF, PL_FLO1, PL_X, PL_H, PL_RH, PL_FM, PL_FIM, OUT_DELTA, OUT_MASK };
+
+struct TcSeg { int plane, c0, chunks; };   // K segment: `chunks` 64-channel chunks of a plane, from channel c0
+
+enum TcLayerFlags : int {
+  TC_CONCAT_FLOW = 1,   // the epilogue appends the 2 flow channels after column n_total (the motion encoder's output)
+  TC_ADVANCE = 2,       // inside the iteration loop the epilogue also applies coords1 += delta and flow = coords1 - grid
+  TC_MASK_ONLY = 4,     // runs only when the mask is wanted (only the last row may: a row's index is its plan position)
+  TC_MASK_TAIL = 8,     // the last table column tile (bn columns) feeds only the mask head: dropped without a mask
 };
 
-static const TcLayerSpec kBasicTc[12] = {
-    /*T0 convc1 */ {1, {BC1, -1}, 1, 1, 384, 256, {1, {0, 0}, {324, 0}, {0, 0}}, 256, 1},
-    /*T1 convc2 */ {1, {BC2, -1}, 3, 3, 256, 192, {1, {0, 0}, {256, 0}, {0, 0}}, 192, 1},
-    /*T2 convf2 */ {1, {BF2, -1}, 3, 3, 128, 64, {1, {0, 0}, {128, 0}, {0, 0}}, 64, 1},
-    /*T3 conv   */ {1, {BCV, -1}, 3, 3, 256, 128, {1, {0, 0}, {256, 0}, {0, 0}}, 128, 1},
-    /*T4 zr1    */ {2, {BZ1, BR1}, 1, 5, 384, 256, {1, {0, 0}, {384, 0}, {0, 0}}, 256, 1},
-    /*T5 q1     */ {1, {BQ1, -1}, 1, 5, 384, 128, {1, {0, 0}, {384, 0}, {0, 0}}, 128, 1},
-    /*T6 zr2    */ {2, {BZ2, BR2}, 5, 1, 384, 256, {1, {0, 0}, {384, 0}, {0, 0}}, 256, 1},
-    /*T7 q2     */ {1, {BQ2, -1}, 5, 1, 384, 128, {1, {0, 0}, {384, 0}, {0, 0}}, 128, 1},
-    /*T8 fh1|m0 */ {2, {BFH1, BM0}, 3, 3, 128, 512, {1, {0, 0}, {128, 0}, {0, 0}}, 256, 2},
-    /*T9 fh2    */ {1, {BFH2, -1}, 3, 3, 256, 16, {1, {0, 0}, {256, 0}, {0, 0}}, 16, 1},
-    /*T10 mask2 */ {1, {BM2, -1}, 1, 1, 256, 576, {1, {0, 0}, {256, 0}, {0, 0}}, 192, 3},
-    /*T11 convf1*/ {1, {BF1, -1}, 1, 1, 128, 128, {1, {0, 0}, {98, 0}, {0, 0}}, 128, 1, 1}};
+struct TcLayer {
+  int nsrc, src[2];               // packing: reference convs merged along cout,
+  int kh, kw, cin_pad, cout_pad;  //   packed dims,
+  int flatten;                    //   1: (kh,kw,cin) flattened into the channel axis, read as a 1x1 conv of im2col planes,
+  TcCinMap cin_map;               //   where the input channels land (nrange == 0: where they are)
+  int bn, ntn;                    // tiling: N per column tile, column tiles (split further when bn > kMaxTileN)
+  TcSeg seg[2];                   // inputs: one or two K segments (seg[1].chunks == 0: one)
+  int mode, act, n_total;         // epilogue (the GRU modes read z and update the caller's hidden state),
+  float out_scale;
+  int out, out_c0;                //   output plane and its first channel,
+  int flags;                      //   TcLayerFlags
+  int ndep;                       // rows read by this one, with the columns read: update_mega_kernel waits for their tiles
+  MegaDep dep[2];                 //   over the halo, which also covers the write-after-read hazards
+};
 
-static const TcLayerSpec kSmallTc[8] = {
-    /*S0 convc1 */ {1, {SC1, -1}, 1, 1, 256, 96, {1, {0, 0}, {196, 0}, {0, 0}}, 96, 1},
-    /*S1 convf2 */ {1, {SF2, -1}, 3, 3, 64, 32, {1, {0, 0}, {64, 0}, {0, 0}}, 32, 1},
-    /*S2 conv   */ {1, {SCV, -1}, 3, 3, 128, 96, {1, {0, 0}, {128, 0}, {0, 0}}, 96, 1},
-    /*S3 zr     */ {2, {SZ, SR}, 3, 3, 320, 192, {2, {0, 96}, {96, 146}, {0, 128}}, 192, 1},
-    /*S4 q      */ {1, {SQ, -1}, 3, 3, 320, 96, {2, {0, 96}, {96, 146}, {0, 128}}, 96, 1},
-    /*S5 fh1    */ {1, {SFH1, -1}, 3, 3, 128, 128, {1, {0, 0}, {96, 0}, {0, 0}}, 128, 1},
-    /*S6 fh2    */ {1, {SFH2, -1}, 3, 3, 128, 16, {1, {0, 0}, {128, 0}, {0, 0}}, 16, 1},
-    /*S7 convf1 */ {1, {SF1, -1}, 1, 1, 128, 64, {1, {0, 0}, {98, 0}, {0, 0}}, 64, 1, 1}};
+// Fields per row: nsrc, convs, kh, kw, cin_pad, cout_pad, flatten, cin map, bn, ntn, inputs,
+//                 mode, act, n_total, out_scale, out, out_c0, flags, ndep, deps.
+// The flow branch (convf1, convf2) needs only the current flow, so it is interleaved with the correlation branch.
+static const TcLayer kBasicTc[12] = {
+    /*  0 convc1 */ {1, {BC1}, 1, 1, 384, 256, 0, {}, 256, 1, {{PL_CORR, 0, 6}},
+                     EPI_LINEAR, ACT_RELU, 256, 1.0f, PL_COR1, 0, 0, 0, {}},
+    /*  1 convf1 */ {1, {BF1}, 1, 1, 128, 128, 1, {}, 128, 1, {{PL_FIM, 0, 2}},
+                     EPI_LINEAR, ACT_RELU, 128, 1.0f, PL_FLO1, 0, 0, 0, {}},
+    /*  2 convc2 */ {1, {BC2}, 3, 3, 256, 192, 0, {}, 192, 1, {{PL_COR1, 0, 4}},
+                     EPI_LINEAR, ACT_RELU, 192, 1.0f, PL_CF, 0, 0, 1, {{0}}},
+    /*  3 convf2 */ {1, {BF2}, 3, 3, 128, 64, 0, {}, 64, 1, {{PL_FLO1, 0, 2}},
+                     EPI_LINEAR, ACT_RELU, 64, 1.0f, PL_CF, 192, 0, 1, {{1}}},
+    /*  4 conv   */ {1, {BCV}, 3, 3, 256, 128, 0, {}, 128, 1, {{PL_CF, 0, 4}},
+                     EPI_LINEAR, ACT_RELU, 126, 1.0f, PL_X, 128, TC_CONCAT_FLOW, 2, {{2}, {3}}},
+    /*  5 z|r1   */ {2, {BZ1, BR1}, 1, 5, 384, 256, 0, {}, 256, 1, {{PL_H, 0, 2}, {PL_X, 0, 4}},
+                     EPI_GRU_ZR, ACT_NONE, 256, 1.0f, PL_RH, 0, 0, 1, {{4}}},
+    /*  6 q1     */ {1, {BQ1}, 1, 5, 384, 128, 0, {}, 128, 1, {{PL_RH, 0, 2}, {PL_X, 0, 4}},
+                     EPI_GRU_Q, ACT_NONE, 128, 1.0f, PL_H, 0, 0, 1, {{5}}},
+    /*  7 z|r2   */ {2, {BZ2, BR2}, 5, 1, 384, 256, 0, {}, 256, 1, {{PL_H, 0, 2}, {PL_X, 0, 4}},
+                     EPI_GRU_ZR, ACT_NONE, 256, 1.0f, PL_RH, 0, 0, 1, {{6}}},
+    /*  8 q2     */ {1, {BQ2}, 5, 1, 384, 128, 0, {}, 128, 1, {{PL_RH, 0, 2}, {PL_X, 0, 4}},
+                     EPI_GRU_Q, ACT_NONE, 128, 1.0f, PL_H, 0, 0, 1, {{7}}},
+    /*  9 fh1|m0 */ {2, {BFH1, BM0}, 3, 3, 128, 512, 0, {}, 256, 2, {{PL_H, 0, 2}},
+                     EPI_LINEAR, ACT_RELU, 512, 1.0f, PL_FM, 0, TC_MASK_TAIL, 1, {{8}}},
+    /* 10 fh2    */ {1, {BFH2}, 3, 3, 256, 16, 0, {}, 16, 1, {{PL_FM, 0, 4}},
+                     EPI_LINEAR, ACT_NONE, 2, 1.0f, OUT_DELTA, 0, TC_ADVANCE, 1, {{9, 0, 256}}},
+    /* 11 mask2  */ {1, {BM2}, 1, 1, 256, 576, 0, {}, 192, 3, {{PL_FM, 256, 4}},
+                     EPI_LINEAR, ACT_NONE, 576, 0.25f, OUT_MASK, 0, TC_MASK_ONLY, 1, {{9, 256, 512}}}};
+
+static const TcLayer kSmallTc[8] = {
+    /* 0 convc1 */ {1, {SC1}, 1, 1, 256, 96, 0, {}, 96, 1, {{PL_CORR, 0, 4}},
+                    EPI_LINEAR, ACT_RELU, 96, 1.0f, PL_CF, 0, 0, 0, {}},
+    /* 1 convf1 */ {1, {SF1}, 1, 1, 128, 64, 1, {}, 64, 1, {{PL_FIM, 0, 2}},
+                    EPI_LINEAR, ACT_RELU, 64, 1.0f, PL_FLO1, 0, 0, 0, {}},
+    /* 2 convf2 */ {1, {SF2}, 3, 3, 64, 32, 0, {}, 32, 1, {{PL_FLO1, 0, 1}},
+                    EPI_LINEAR, ACT_RELU, 32, 1.0f, PL_CF, 96, 0, 1, {{1}}},
+    /* 3 conv   */ {1, {SCV}, 3, 3, 128, 96, 0, {}, 96, 1, {{PL_CF, 0, 2}},
+                    EPI_LINEAR, ACT_RELU, 80, 1.0f, PL_X, 64, TC_CONCAT_FLOW, 2, {{0}, {2}}},
+    /* 4 z|r    */ {2, {SZ, SR}, 3, 3, 320, 192, 0, {2, {0, 96}, {96, 146}, {0, 128}}, 192, 1, {{PL_H, 0, 2}, {PL_X, 0, 3}},
+                    EPI_GRU_ZR, ACT_NONE, 192, 1.0f, PL_RH, 0, 0, 1, {{3}}},
+    /* 5 q      */ {1, {SQ}, 3, 3, 320, 96, 0, {2, {0, 96}, {96, 146}, {0, 128}}, 96, 1, {{PL_RH, 0, 2}, {PL_X, 0, 3}},
+                    EPI_GRU_Q, ACT_NONE, 96, 1.0f, PL_H, 0, 0, 1, {{4}}},
+    /* 6 fh1    */ {1, {SFH1}, 3, 3, 128, 128, 0, {}, 128, 1, {{PL_H, 0, 2}},
+                    EPI_LINEAR, ACT_RELU, 128, 1.0f, PL_FM, 0, 0, 1, {{5}}},
+    /* 7 fh2    */ {1, {SFH2}, 3, 3, 128, 16, 0, {}, 16, 1, {{PL_FM, 0, 2}},
+                    EPI_LINEAR, ACT_NONE, 2, 1.0f, OUT_DELTA, 0, TC_ADVANCE, 1, {{6}}}};
 
 inline int n_tc_layers(int variant) { return variant == RAFT_VARIANT_BASIC ? 12 : 8; }
-inline const TcLayerSpec* tc_layers(int variant) { return variant == RAFT_VARIANT_BASIC ? kBasicTc : kSmallTc; }
+inline const TcLayer* tc_layers(int variant) { return variant == RAFT_VARIANT_BASIC ? kBasicTc : kSmallTc; }
 
 // ------------------------------------------------------------------------------------------------
 // Prepared-weights blob (device).  Offsets are a pure function of (variant, precision).
@@ -92,7 +135,7 @@ inline PreparedLayout prepared_layout(int variant, int precision) {
     off = align_up(off + sizeof(float) * cd[i].cout, 256);
   }
   if (precision == RAFT_PREC_F16X2) {
-    const TcLayerSpec* tl = tc_layers(variant);
+    const TcLayer* tl = tc_layers(variant);
     for (int i = 0; i < n_tc_layers(variant); ++i)
       L.tc[i] = tc_weight_slot(off, tl[i].kh, tl[i].kw, tl[i].cin_pad, tl[i].cout_pad);
   }
@@ -236,36 +279,107 @@ inline int simt2(const UpdateCtx& c, int conv_idx, const float* s0, int st0, int
   return launch_simt_conv(c, conv_idx, 2, s, st, o, nn, out, out_stride, 0, act, 1.0f);
 }
 
-// One tensor-core layer.  Operand planes: up to two K segments (hi/lo plane pair, channel stride,
-// first channel, number of 64-channel chunks).
-struct TcSeg { const __half* hi; const __half* lo; int stride, c0, chunks; };
+// ------------------------------------------------------------------------------------------------
+// Update block, fp32 FFMA path: the reference's op sequence, one launch per Conv2D.
+// ------------------------------------------------------------------------------------------------
+inline int gru_fp32(const UpdateCtx& c, float* h, int iz, int ir, int iq, int hid, int xs, int xn) {
+  const Workspace& W = c.W;
+  const size_t n = (size_t)c.B * c.h * c.w * hid;
+  RAFT_TRY(simt2(c, iz, h, hid, hid, W.x, xs, xn, W.z, hid, SACT_SIGMOID));
+  RAFT_TRY(simt2(c, ir, h, hid, hid, W.x, xs, xn, W.r, hid, SACT_SIGMOID));
+  RAFT_TRY(launch(gru_rh_kernel, grid_for(n), 256, 0, c.stream, W.r, h, W.rh, n));
+  RAFT_TRY(simt2(c, iq, W.rh, hid, hid, W.x, xs, xn, W.q, hid, SACT_TANH));
+  return launch(gru_update_kernel, grid_for(n), 256, 0, c.stream, W.z, W.q, h, n);
+}
 
-inline int launch_tc_layer(const UpdateCtx& c, int layer, int nseg, const TcSeg* segs, TcConvParams& p, int ntn = -1,
-                           const TcDeps& deps = TcDeps{0, {-1, -1}, {-1, -1}}) {
-  const TcLayerSpec& L = tc_layers(c.variant)[layer];
+inline int update_core_fp32(const UpdateCtx& c, float* h, float* delta, float* mask) {
+  const Workspace& W = c.W;
+  const VariantDims d = variant_dims(c.variant);
+  const size_t npix = (size_t)c.B * c.h * c.w;
+  if (c.variant == RAFT_VARIANT_BASIC) {
+    RAFT_TRY(simt1(c, BC1, W.corr, 324, 0, 324, W.cor1, 256, 0, SACT_RELU));           // update.py:98
+    RAFT_TRY(simt1(c, BC2, W.cor1, 256, 0, 256, W.cf, 256, 0, SACT_RELU));              // :99
+    RAFT_TRY(simt1(c, BF1, W.flow, 2, 0, 2, W.flo1, 128, 0, SACT_RELU));                // :100
+    RAFT_TRY(simt1(c, BF2, W.flo1, 128, 0, 128, W.cf, 256, 192, SACT_RELU));            // :101,104
+    RAFT_TRY(simt1(c, BCV, W.cf, 256, 0, 256, W.x, 256, 128, SACT_RELU));               // :105
+    RAFT_TRY(launch(copy_channels_kernel, grid_for(npix * 2), 256, 0, c.stream, W.flow, 2, 0, W.x, 256, 254, 2, npix));  // :106
+    RAFT_TRY(gru_fp32(c, h, BZ1, BR1, BQ1, 128, 256, 256));                             // :53-58
+    RAFT_TRY(gru_fp32(c, h, BZ2, BR2, BQ2, 128, 256, 256));                             // :60-65
+    RAFT_TRY(simt1(c, BFH1, h, 128, 0, 128, W.fm, 512, 0, SACT_RELU));                  // :14
+    RAFT_TRY(simt1(c, BFH2, W.fm, 512, 0, 256, delta, 2, 0, SACT_NONE));
+    if (mask) {
+      RAFT_TRY(simt1(c, BM0, h, 128, 0, 128, W.fm, 512, 256, SACT_RELU));               // :137-141
+      RAFT_TRY(simt1(c, BM2, W.fm, 512, 256, 256, mask, 576, 0, SACT_NONE, 0.25f));     // :152
+    }
+  } else {
+    RAFT_TRY(simt1(c, SC1, W.corr, 196, 0, 196, W.cf, 128, 0, SACT_RELU));              // update.py:80
+    RAFT_TRY(simt1(c, SF1, W.flow, 2, 0, 2, W.flo1, 64, 0, SACT_RELU));                 // :81
+    RAFT_TRY(simt1(c, SF2, W.flo1, 64, 0, 64, W.cf, 128, 96, SACT_RELU));               // :82-83
+    RAFT_TRY(simt1(c, SCV, W.cf, 128, 0, 128, W.x, d.c_x, 64, SACT_RELU));              // :84
+    RAFT_TRY(launch(copy_channels_kernel, grid_for(npix * 2), 256, 0, c.stream, W.flow, 2, 0, W.x, d.c_x, 144, 2, npix));  // :85
+    RAFT_TRY(gru_fp32(c, h, SZ, SR, SQ, 96, d.c_x, 146));                               // :26-35
+    RAFT_TRY(simt1(c, SFH1, h, 96, 0, 96, W.fm, 128, 0, SACT_RELU));
+    RAFT_TRY(simt1(c, SFH2, W.fm, 128, 0, 128, delta, 2, 0, SACT_NONE));
+  }
+  return raft_launch_status();
+}
+
+// ------------------------------------------------------------------------------------------------
+// Update block, tensor-core path: the rows of tc_layers(variant), in order.  Operands travel between layers as fp16
+// hi/lo planes written by the producing layer's epilogue.  h: the caller's hidden state, updated in place; mask == null:
+// no mask head; adv_coords != null (iteration loop): the flow head's epilogue also advances coords1 and the flow.
+// With c.plan the layers are appended to the plan (one update_mega_kernel launch), else launched one by one.
+// ------------------------------------------------------------------------------------------------
+inline int update_core_tc(const UpdateCtx& c, float* h, float* delta, float* mask, float* adv_coords) {
+  const Workspace& W = c.W;
+  const VariantDims d = variant_dims(c.variant);
+  struct Plane { __half *hi, *lo; int stride; };
+  const Plane planes[] = {{W.corr_hi, W.corr_lo, d.s_corr}, {W.cor1_hi, W.cor1_lo, d.s_cor1}, {W.cf_hi, W.cf_lo, d.s_cf},
+                          {W.flo1_hi, W.flo1_lo, d.s_flo1}, {W.x_hi, W.x_lo, d.s_x},          {W.h_hi, W.h_lo, d.s_h},
+                          {W.rh_hi, W.rh_lo, d.s_h},        {W.fm_hi, W.fm_lo, d.s_fm},       {W.fim_hi, W.fim_lo, 128}};
   int tw, th;
   tc_pick_tile(c.w, c.h, &tw, &th);
-  p.nseg = nseg;
-  int chunks = 0;
-  for (int i = 0; i < nseg; ++i) {
-    RAFT_TRY(make_tmap_act2(&p.a_map[i], segs[i].hi, segs[i].lo, c.B, c.h, c.w, segs[i].stride, tw, th));
-    p.seg_chunks[i] = segs[i].chunks;
-    p.seg_c0[i] = segs[i].c0;
-    chunks += segs[i].chunks;
+  const TcLayer* rows = tc_layers(c.variant);
+  for (int i = 0; i < n_tc_layers(c.variant); ++i) {
+    const TcLayer& L = rows[i];
+    if ((L.flags & TC_MASK_ONLY) && !mask) continue;
+    const bool no_tail = (L.flags & TC_MASK_TAIL) && !mask;
+    if (L.flatten && !c.fim_ready)           // (in the iteration loop the lookup kernel has already produced the planes)
+      RAFT_TRY(launch(flow_im2col_kernel, grid_for((size_t)c.B * c.h * c.w * 128), 256, 0, c.stream, W.flow, c.B, c.h, c.w,
+                      W.fim_hi, W.fim_lo));
+    TcConvParams p;
+    memset(&p, 0, sizeof(p));
+    int chunks = 0;
+    for (int s = 0; s < 2 && L.seg[s].chunks; ++s) {
+      const Plane& a = planes[L.seg[s].plane];
+      RAFT_TRY(make_tmap_act2(&p.a_map[s], a.hi, a.lo, c.B, c.h, c.w, a.stride, tw, th));
+      p.seg_chunks[s] = L.seg[s].chunks;
+      p.seg_c0[s] = L.seg[s].c0;
+      chunks += L.seg[s].chunks;
+      p.nseg = s + 1;
+    }
+    if (chunks * kChunkK != L.cin_pad) return RAFT_ERR_BAD_SHAPE;
+    const int nsplit = tc_n_split(L.bn);                // layers wider than kMaxTileN run as more column tiles
+    if (!nsplit) return RAFT_ERR_BAD_SHAPE;
+    RAFT_TRY(tc_use_weights(p, c.prepared, c.PL.tc[i], L.bn / nsplit));
+    p.ph = (L.kh - 1) / 2; p.pw = (L.kw - 1) / 2;
+    p.B = c.B; p.H = c.h; p.W = c.w; p.TH = th; p.TW = tw;
+    // Promotion group of the update-block layers: 2 chunks (24-MMA chains).  Their K = 1920 GRU contractions feed a
+    // 12-iteration recurrence (DESIGN.md section 4).
+    p.group_chunks = 2;
+    p.mode = L.mode; p.act = L.act; p.out_scale = L.out_scale;
+    p.n_total = no_tail ? L.n_total - L.bn : L.n_total;
+    if (L.out == OUT_DELTA) { p.out_f32 = delta; p.f32_stride = 2; }
+    else if (L.out == OUT_MASK) { p.out_f32 = mask; p.f32_stride = 576; }
+    else { p.out_hi = planes[L.out].hi; p.out_lo = planes[L.out].lo; p.h_stride = planes[L.out].stride; p.h_c0 = L.out_c0; }
+    if (L.flags & TC_CONCAT_FLOW) { p.concat_src = W.flow; p.concat_n = 2; }
+    if (L.mode != EPI_LINEAR) { p.z = W.z; p.h = h; p.hid = d.hid; }
+    if ((L.flags & TC_ADVANCE) && adv_coords) { p.adv_coords = adv_coords; p.adv_flow = W.flow; }
+    const int n_tiles_n = (no_tail ? L.ntn - 1 : L.ntn) * nsplit;
+    if (c.plan && c.plan->P.nlayers != i) return RAFT_ERR_UNSUPPORTED;   // a dependency names its source by row index
+    RAFT_TRY(c.plan ? mega_add(*c.plan, p, n_tiles_n, L.ndep, L.dep) : tc_launch(p, n_tiles_n, c.stream));
   }
-  if (chunks * kChunkK != L.cin_pad) return RAFT_ERR_BAD_SHAPE;
-  const int nsplit = tc_n_split(L.bn);                // layers wider than kMaxTileN run as more column tiles
-  if (!nsplit) return RAFT_ERR_BAD_SHAPE;
-  RAFT_TRY(tc_use_weights(p, c.prepared, c.PL.tc[layer], L.bn / nsplit));
-  p.ph = (L.kh - 1) / 2; p.pw = (L.kw - 1) / 2;
-  p.B = c.B; p.H = c.h; p.W = c.w; p.TH = th; p.TW = tw;
-  if (p.out_scale == 0.0f) p.out_scale = 1.0f;
-  // Promotion group of the update-block layers: 2 chunks (24-MMA chains).  Their K = 1920 GRU contractions feed a
-  // 12-iteration recurrence (DESIGN.md section 4).
-  p.group_chunks = 2;
-  const int n_tiles_n = (ntn > 0 ? ntn : L.ntn) * nsplit;
-  if (c.plan) return mega_add(*c.plan, layer, p, n_tiles_n, nsplit, deps);
-  return tc_launch(p, n_tiles_n, c.stream);
+  return 0;
 }
 
 }  // namespace raft
