@@ -102,9 +102,14 @@ def param_shapes(variant):
 
 def init_params(variant, seed=1234, bias_scale=0.0, norm_jitter=0.0):
     """name -> float32 ndarray, drawn in tree order from default_rng(seed)."""
+    return draw_params(param_shapes(variant), seed, bias_scale, norm_jitter)
+
+
+def draw_params(shapes, seed=1234, bias_scale=0.0, norm_jitter=0.0):
+    """{name: shape} (in order) -> name -> float32 ndarray, with the distributions of the module docstring."""
     rng = np.random.default_rng(seed)
     out = OrderedDict()
-    for name, shape in param_shapes(variant).items():
+    for name, shape in OrderedDict(shapes).items():
         leaf = name.rsplit('.', 1)[1]
         if leaf == 'kernel':
             kh, kw, cin, cout = shape

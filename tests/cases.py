@@ -57,3 +57,66 @@ def update_inputs(variant, b, h, w, seed=20):
     corr = (rng.standard_normal((b, h, w, cch)) * 3).astype(F32)
     flow = (rng.standard_normal((b, h, w, 2)) * 4).astype(F32)
     return net, inp, corr, flow
+
+
+# ---------------------------------------------------------------------------------------------- geometry sweep
+def tc_tile(h, w):
+    """(TW, TH) pixel tile of every tensor-core convolution on an h x w grid: a Python mirror of tc_pick_tile
+    (tf_raft_b200/csrc/conv_tc.cuh).  TW * TH = 128 with TW a power of two from 128 down to 8; the least padded area
+    wins, and on a tie the wider tile (the first one tried)."""
+    best = None
+    tw = 128
+    while tw >= 8:
+        th = 128 // tw
+        area = -(-w // tw) * tw * (-(-h // th) * th)
+        if best is None or area < best[0]:
+            best = (area, tw, th)
+        tw //= 2
+    return best[1], best[2]
+
+
+# (B, h, w) update-block grids: one per tile shape, then one whose work list is many times the 132 SMs of an H100.  The
+# 128 x 1 grid has 9 rows (not fewer) so that a 4-level pyramid, and with it the whole model loop, also runs on it.
+TILE_GRIDS = (
+    (2, 9, 128),       # 128 x 1 (the tile of the Sintel grid 56 x 128; TH = 1 gives the 5 x 1 GRU convolutions a 2-row halo)
+    (2, 5, 40),        # 64 x 2
+    (2, 9, 25),        # 32 x 4
+    (3, 13, 11),       # 16 x 8
+    (2, 9, 7),         # 8 x 16 (W <= 8, H >= 9)
+    (4, 24, 40),       # 16 x 8, 36 pixel tiles per layer
+)
+
+# (B, h, w) lookup grids per pyramid depth.  Each has a deepest level of width or height 1; the second 4-level grid has
+# every level width a multiple of 4 (the window kernel's 128-bit loads), the first has none.
+LOOKUP_GRIDS = {
+    1: ((2, 5, 7), (2, 1, 9)),
+    2: ((2, 7, 3),),
+    4: ((2, 9, 13), (1, 8, 32)),
+    5: ((1, 17, 19),),
+    6: ((1, 33, 37),),
+}
+
+# (B, h, w, C, levels) correlation pyramids: 1 to 6 levels (levels > 4 take the per-level pooling path of the tensor-core
+# build), C from 64 to 256 (sqrt(C) a power of two or not), odd h and w, N = h*w never a multiple of 128.
+PYRAMID_CASES = (
+    (3, 9, 13, 64, 1),
+    (3, 11, 7, 128, 2),
+    (3, 15, 15, 192, 4),
+    (3, 19, 23, 256, 4),
+    (2, 31, 31, 256, 5),
+    (1, 31, 95, 192, 5),
+    (1, 63, 63, 64, 6),
+    (1, 63, 63, 128, 6),
+)
+
+
+def level_sizes(h, w, levels):
+    """(h, w) of every pyramid level: 2x2 VALID average pooling floors odd sizes (corr.py:113)."""
+    return [(h >> l, w >> l) for l in range(levels)]
+
+
+def encoder_params(variant, norm_type, out_dim, seed=99, bias_scale=0.05, norm_jitter=0.2):
+    """Parameters of a BasicEncoder ('raft') / SmallEncoder ('small') with any norm type, under the prefix 'enc.'."""
+    from oracle import weights
+    c0, stages = (64, ((64, 1), (96, 2), (128, 2))) if variant == 'raft' else (32, ((32, 1), (64, 2), (96, 2)))
+    return weights.draw_params(weights.encoder_shapes('enc', norm_type, c0, stages, out_dim), seed, bias_scale, norm_jitter)

@@ -1,0 +1,109 @@
+"""CPU checks of the geometry sweep's case lists and fp64 references (tests/test_gpu_geometry.py): the grids reach the
+code paths they are meant to reach, and the references used as truth are right."""
+import numpy as np
+import torch
+
+import cases
+from oracle import corr_np, raft_torch as rt, weights
+
+ALL_TILES = {(128, 1), (64, 2), (32, 4), (16, 8), (8, 16)}
+
+
+def test_tile_mirror_known_answers():
+    assert cases.tc_tile(56, 128) == (128, 1)      # Sintel (436 x 1024 padded to 448 x 1024)
+    assert cases.tc_tile(56, 64) == (64, 2)        # FlyingChairs-size benchmark grid (448 x 512)
+    assert cases.tc_tile(8, 8) == (16, 8)
+    assert cases.tc_tile(8, 12) == (16, 8)
+    for h in range(1, 70):
+        for w in range(1, 140):
+            tw, th = cases.tc_tile(h, w)
+            assert tw * th == 128 and (tw, th) in ALL_TILES
+            area = -(-w // tw) * tw * (-(-h // th) * th)
+            for t in (128, 64, 32, 16, 8):                       # least padded area, the wider tile on a tie
+                other = -(-w // t) * t * (-(-h // (128 // t)) * (128 // t))
+                assert area < other or (area == other and tw >= t)
+
+
+def test_tile_grids_reach_every_tile_shape():
+    tiles = [cases.tc_tile(h, w) for _, h, w in cases.TILE_GRIDS]
+    assert set(tiles) == ALL_TILES, tiles
+    b, h, w = cases.TILE_GRIDS[-1]
+    tw, th = cases.tc_tile(h, w)
+    assert b * -(-h // th) * -(-w // tw) == 36          # pixel tiles per layer: with ~15 layers, several times 132 work items
+    # the loop test needs a 4-level pyramid on the 128 x 1 grid
+    assert min(cases.TILE_GRIDS[0][1:]) >> 3 >= 1
+
+
+def test_lookup_grids_reach_every_kernel_form():
+    for levels, grids in cases.LOOKUP_GRIDS.items():
+        deepest = [cases.level_sizes(h, w, levels)[-1] for _, h, w in grids]
+        assert all(min(s) >= 1 for s in deepest)
+        assert any(1 in s for s in deepest), (levels, deepest)                 # a deepest level 1 wide or 1 high
+    vec = [all(lw % 4 == 0 for _, lw in cases.level_sizes(h, w, 4)) for _, h, w in cases.LOOKUP_GRIDS[4]]
+    assert sorted(vec) == [False, True]                                     # 128-bit and scalar window loads
+    assert not any(w % 4 == 0 for _, _, w in cases.LOOKUP_GRIDS[4][:1])
+
+
+def test_pyramid_cases_cover_levels_channels_and_odd_sizes():
+    levels = {c[4] for c in cases.PYRAMID_CASES}
+    assert {1, 2, 4, 5, 6} <= levels
+    assert {64, 128, 192, 256} <= {c[3] for c in cases.PYRAMID_CASES}
+    pow2 = {float(np.sqrt(c)).is_integer() and (int(np.sqrt(c)) & (int(np.sqrt(c)) - 1)) == 0 for c in (64, 128, 192, 256)}
+    assert pow2 == {True, False}                                                # corr_mul and corr_div scalings
+    for b, h, w, c, lv in cases.PYRAMID_CASES:
+        assert (h * w) % 128 != 0 and c % 64 == 0
+        assert min(min(s) for s in cases.level_sizes(h, w, lv)) >= 1
+    assert any(all(lh % 2 and lw % 2 for lh, lw in cases.level_sizes(h, w, lv)) and lv > 4
+               for b, h, w, c, lv in cases.PYRAMID_CASES)                    # odd at every level, generic path
+    assert any(b == 3 for b, *_ in cases.PYRAMID_CASES)
+
+
+def test_fp64_pyramid_matches_the_literal_numpy_restatement():
+    """The fp64 truth of the pyramid test (raft_torch.CorrBlock on double features) is the reference's volume, pooled the
+    reference's way: it agrees with the op-by-op NumPy restatement to fp32 rounding, on odd sizes through 5 levels."""
+    b, h, w, c, levels = 1, 31, 33, 64, 5
+    f1, f2 = cases.fmaps(b, h, w, c, seed=3)
+    truth = rt.CorrBlock(torch.from_numpy(f1).double(), torch.from_numpy(f2).double(), levels, 4).corr_pyramid
+    lit = corr_np.CorrBlock(f1, f2, levels, 4).corr_pyramid
+    for l, (lh, lw) in enumerate(cases.level_sizes(h, w, levels)):
+        assert truth[l].shape == lit[l].shape == (b * h * w, lh, lw, 1)
+        np.testing.assert_allclose(truth[l].numpy(), lit[l], atol=5e-6, rtol=1e-5)
+
+
+def test_fp64_lookup_gradient_matches_finite_differences():
+    """The backward truth (torch.autograd through raft_torch's sampler in fp64) is the derivative of the sampler, checked
+    by central differences at non-integer coordinates, out-of-range ones (clamped: zero gradient) included."""
+    b, h, w, levels, r = 1, 5, 7, 3, 2
+    f1, f2 = cases.fmaps(b, h, w, 64, seed=4)
+    pyr = [p.clone().requires_grad_(True)
+           for p in rt.CorrBlock(torch.from_numpy(f1).double(), torch.from_numpy(f2).double(), levels, r).corr_pyramid]
+    coords = torch.from_numpy(cases.lookup_coords(b, h, w, 'jitter', seed=8)).double().requires_grad_(True)
+
+    def f(c, *p):
+        cb = rt.CorrBlock.__new__(rt.CorrBlock)
+        cb.corr_pyramid, cb.num_levels, cb.radius = list(p), levels, r
+        return cb.retrieve(c)
+    assert torch.autograd.gradcheck(f, (coords, *pyr), eps=1e-7, atol=1e-6)
+
+
+def test_encoder_params_fit_both_encoders_and_every_norm():
+    from tf_raft_b200.layers.extractor import BasicEncoder, SmallEncoder
+    for variant, cls, out_dim in (('raft', BasicEncoder, 256), ('small', SmallEncoder, 128)):
+        for norm in ('instance', 'batch', None):
+            p = cases.encoder_params(variant, norm, out_dim)
+            enc = cls(output_dim=out_dim, norm_type=norm, device='cpu')
+            assert set(enc.params) == {k[len('enc.'):] for k in p}
+            enc.load_params(p, 'enc.')
+    # the refactored parameter generator draws the same values as before
+    p = weights.init_params('small', 1234, bias_scale=0.05, norm_jitter=0.1)
+    q = weights.draw_params(weights.param_shapes('small'), 1234, 0.05, 0.1)
+    assert list(p) == list(q) and all(np.array_equal(p[k], q[k]) for k in p)
+
+
+def test_fp64_encoder_output_shape_on_odd_sizes():
+    """rt.encoder pads the stride-2 stages the TensorFlow way: the output is ceil(H / 8) x ceil(W / 8)."""
+    p = cases.encoder_params('small', 'instance', 128)
+    for H, W in ((70, 98), (36, 52)):
+        x = torch.zeros(1, 3, H, W, dtype=torch.float64)
+        out = rt.encoder(rt.Ops(p, torch.float64), x, 'enc', 'instance', False)
+        assert tuple(out.shape) == (1, 128, -(-H // 8), -(-W // 8))

@@ -386,26 +386,28 @@ import torch
 import cases
 from oracle import weights
 import tf_raft_b200 as T
-for variant, compute_mask in (('raft', True), ('raft', False), ('small', False)):
-    blk = (T.BasicUpdateBlock if variant == 'raft' else T.SmallUpdateBlock)(precision='f16x2')
-    blk.load_params(weights.init_params(variant, 1234), 'update_block.')
-    net, inp, corr, flow = [torch.from_numpy(a).cuda() for a in cases.update_inputs(variant, 4, 56, 64)]
-    out = blk([net, inp, corr, flow], compute_mask=compute_mask) if variant == 'raft' else blk([net, inp, corr, flow])
-    torch.cuda.synchronize()
-    assert (out[1] is not None) == compute_mask
-    h = hashlib.sha256()
-    for t in out:
-        if t is not None:
-            h.update(t.cpu().numpy().tobytes())
-    print('HASH', variant, 'mask' if compute_mask else 'no-mask', h.hexdigest())
+for b, hh, ww in ((4, 56, 64),) + cases.TILE_GRIDS:
+    for variant, compute_mask in (('raft', True), ('raft', False), ('small', False)):
+        blk = (T.BasicUpdateBlock if variant == 'raft' else T.SmallUpdateBlock)(precision='f16x2')
+        blk.load_params(weights.init_params(variant, 1234), 'update_block.')
+        net, inp, corr, flow = [torch.from_numpy(a).cuda() for a in cases.update_inputs(variant, b, hh, ww)]
+        out = blk([net, inp, corr, flow], compute_mask=compute_mask) if variant == 'raft' else blk([net, inp, corr, flow])
+        torch.cuda.synchronize()
+        assert (out[1] is not None) == compute_mask
+        h = hashlib.sha256()
+        for t in out:
+            if t is not None:
+                h.update(t.cpu().numpy().tobytes())
+        print('HASH', f'{b}x{hh}x{ww}', variant, 'mask' if compute_mask else 'no-mask', h.hexdigest())
 '''
 
 
 def test_update_block_forms_are_bit_identical(T):
     """update_mega_kernel (the default) and one launch per layer (RAFT_B200_MEGA=0) run the same accumulation chains in the
-    same order: their outputs (net, mask if any, delta_flow) at batch 4, 56x64 must be identical byte for byte, for
-    BasicUpdateBlock with and without its mask head and for SmallUpdateBlock.  (The switch is read once per process, hence
-    the subprocesses.)"""
+    same order: their outputs (net, mask if any, delta_flow) must be identical byte for byte, for BasicUpdateBlock with and
+    without its mask head and for SmallUpdateBlock, at batch 4, 56x64 and on every grid of cases.TILE_GRIDS (every pixel
+    tile, so every dependency halo, the 2-row one of the 5x1 convolutions at TH = 1 included).  (The switch is read once
+    per process, hence the subprocesses.)"""
     import os
     import subprocess
     import sys
@@ -416,5 +418,5 @@ def test_update_block_forms_are_bit_identical(T):
                              timeout=300)
         assert res.returncode == 0, f'{name}: {res.stderr[-2000:]}'
         hashes[name] = [l for l in res.stdout.splitlines() if l.startswith('HASH')]
-        assert len(hashes[name]) == 3, f'{name}: {res.stdout[-2000:]}'
+        assert len(hashes[name]) == 3 * (1 + len(cases.TILE_GRIDS)), f'{name}: {res.stdout[-2000:]}'
     assert hashes['mega'] == hashes['per_layer'], hashes
