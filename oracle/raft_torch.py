@@ -33,10 +33,13 @@ def _same_pads(n_in, k, s):
 class Ops:
     """Conv / norm primitives on NCHW tensors bound to a parameter dict."""
 
-    def __init__(self, params, dtype=torch.float32, quant=None, split=None):
+    def __init__(self, params, dtype=torch.float32, quant=None, split=None, bn_record=None):
         self.dtype = dtype
         self.quant = quant
         self.split = split          # None | (xh_q, xl_q, wh_q, wl_q): emulate split-precision tensor-core passes
+        # None | dict: every training-mode BatchNorm layer stores (batch mean, biased batch variance, count) under its
+        # name, detached -- what oracle.train_ref.bn_moving_update advances the moving statistics with
+        self.bn_record = bn_record
         self.p = {k: _t(v, dtype) for k, v in params.items()}
         self._wcache = {}
 
@@ -81,6 +84,9 @@ class Ops:
             if training:
                 mean = x.mean(dim=(0, 2, 3), keepdim=True)
                 var = x.var(dim=(0, 2, 3), unbiased=False, keepdim=True)
+                if self.bn_record is not None:
+                    self.bn_record[name] = (mean.detach().flatten(), var.detach().flatten(),
+                                            x.shape[0] * x.shape[2] * x.shape[3])
             else:
                 mean = self.p[name + '.moving_mean'].view(1, -1, 1, 1)
                 var = self.p[name + '.moving_variance'].view(1, -1, 1, 1)
@@ -265,15 +271,16 @@ VARIANTS = {
 
 
 def forward(params, image1, image2, variant='raft', iters=12, training=False,
-            dtype=torch.float32, quant=None, split=None, return_intermediates=False):
+            dtype=torch.float32, quant=None, split=None, return_intermediates=False, bn_record=None):
     """RAFT.call (model.py:68-109) / SmallRAFT.call (model.py:190-226).
 
     image1/2: (B, H, W, 3) in 0..255.  Returns the list of `iters` NHWC flow predictions
     (torch tensors); with return_intermediates also a dict of the tensors at the kernel
-    boundaries (fmaps, net/inp, per-iteration corr/net/mask/delta/coords).
+    boundaries (fmaps, net/inp, per-iteration corr/net/mask/delta/coords).  `bn_record` (a dict)
+    receives the batch statistics of every training-mode BatchNorm layer (see Ops).
     """
     cfg = VARIANTS[variant]
-    ops = Ops(params, dtype, quant, split)
+    ops = Ops(params, dtype, quant, split, bn_record)
     x1 = _t(image1, dtype)
     x2 = _t(image2, dtype)
     bs, H, W, _ = x1.shape

@@ -99,9 +99,9 @@ class _Params:
             if training:
                 mean = x.mean(dim=(0, 2, 3), keepdim=True)
                 var = x.var(dim=(0, 2, 3), unbiased=False, keepdim=True)
-                mom = 0.99
+                mom, n = 0.99, x.shape[0] * x.shape[2] * x.shape[3]      # keras fused update: n / (n - 1) (DESIGN.md §9)
                 self.params[name + '.moving_mean'].mul_(mom).add_((1 - mom) * mean.flatten())
-                self.params[name + '.moving_variance'].mul_(mom).add_((1 - mom) * var.flatten())
+                self.params[name + '.moving_variance'].mul_(mom).add_((1 - mom) * n / max(n - 1, 1) * var.flatten())
             else:
                 mean = self.params[name + '.moving_mean'].view(1, -1, 1, 1)
                 var = self.params[name + '.moving_variance'].view(1, -1, 1, 1)

@@ -244,10 +244,10 @@ class TrainGraph:
             n = n_local * (dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1)
             mean = (stats[0] / n).view(1, -1, 1, 1)
             var = (stats[1] / n).view(1, -1, 1, 1) - mean * mean
-            with torch.no_grad():                       # keras moving statistics, momentum 0.99 (biased variance)
+            with torch.no_grad():                       # keras moving statistics, momentum 0.99 (DESIGN.md §9)
                 mom = 0.99
                 self.moving[name + '.moving_mean'].mul_(mom).add_((1 - mom) * mean.flatten())
-                self.moving[name + '.moving_variance'].mul_(mom).add_((1 - mom) * var.flatten())
+                self.moving[name + '.moving_variance'].mul_(mom).add_((1 - mom) * n / max(n - 1, 1) * var.flatten())
         return (x - mean) * torch.rsqrt(var + eps) * g + b
 
     def res_block(self, x, p, nt, stride):
