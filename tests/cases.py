@@ -115,6 +115,73 @@ def level_sizes(h, w, levels):
     return [(h >> l, w >> l) for l in range(levels)]
 
 
+def lookup_path(B, h, w, levels, radius, out_stride, vec_ok=True):
+    """The lookup kernel CorrBlock.retrieve and the loop launch for a B x h x w grid: a Python mirror of
+    lookup_win_kernel (tf_raft_b200/csrc/lookup.cuh).  'window-vec' / 'window' = corr_lookup_win_kernel with 128-bit /
+    scalar footprint loads, 'generic' = corr_lookup_kernel.  The window kernel exists for (radius, levels) = (4, 4) and
+    (3, 4) and addresses the pyramid with 32-bit offsets, so it declines once level 0 (B*h*w planes of h*w elements) or
+    the output (B*h*w rows of out_stride) holds 2^31 elements or more.  vec_ok: every level starts 16-byte aligned."""
+    nq = B * h * w
+    if levels != 4 or radius not in (3, 4) or nq * levels >= 2 ** 31:
+        return 'generic'
+    if nq * h * w >= 2 ** 31 or nq * out_stride >= 2 ** 31:
+        return 'generic'
+    vec = vec_ok and all(lw % 4 == 0 for _, lw in level_sizes(h, w, levels))
+    return 'window-vec' if vec else 'window'
+
+
+# (B, h, w) grids on both sides of the window kernel's 2^31-element limit on pyramid level 0, and one past 2^32: the
+# pyramid (4 levels, fp32) takes 11.2 to 23.0 GB of device memory.
+LARGE_CASES = (
+    (1, 215, 215),     # images 1720 x 1720: B*N^2 = 2 136 750 625 < 2^31, window kernel, scalar loads
+    (1, 216, 216),     # images 1728 x 1728: 2 176 782 336 >= 2^31, generic kernel
+    (41, 56, 128),     # Sintel grid, batch 41: 2 106 589 184 < 2^31, window kernel, 128-bit loads
+    (42, 56, 128),     # batch 42: 2 157 969 408 >= 2^31, generic kernel
+    (1, 257, 256),     # 4 328 587 264 > 2^32, generic kernel
+)
+
+
+def boundary_queries(B, h, w):
+    """Queries whose level-0 plane (elements [q*N, (q+1)*N) of the volume, N = h*w) holds element 2^31 or 2^32."""
+    n = h * w
+    return [e // n for e in (2 ** 31, 2 ** 32) if e < B * n * n]
+
+
+def large_sample(B, h, w, n_random=32, seed=7):
+    """Sorted query indices to check on a large grid: the first and last 4 queries of every image, each boundary query
+    (boundary_queries) with its neighbours, and n_random seeded random queries."""
+    n = h * w
+    qs = set()
+    for b in range(B):
+        qs.update(range(b * n, b * n + 4))
+        qs.update(range((b + 1) * n - 4, (b + 1) * n))
+    for q in boundary_queries(B, h, w):
+        qs.update(range(q - 1, q + 2))
+    qs.update(np.random.default_rng(seed).integers(0, B * n, n_random).tolist())
+    return np.array(sorted(q for q in qs if 0 <= q < B * n), dtype=np.int64)
+
+
+def corr_rows(f1, f2, qs, levels):
+    """float64 pyramid planes of the queries qs only: level 0 = f1[q] . f2[b]^T / sqrt(C) as an h x w plane, deeper
+    levels pooled 2 x 2 VALID from it, the way oracle.raft_torch.CorrBlock pools.  f1, f2: (B, h, w, C) NumPy arrays.
+    Returns levels tensors (len(qs), h_l, w_l, 1)."""
+    import torch
+    import torch.nn.functional as F
+    B, h, w, c = f1.shape
+    n = h * w
+    qs = np.asarray(qs, dtype=np.int64)
+    rows = torch.empty((len(qs), 1, h, w), dtype=torch.float64)
+    for b in np.unique(qs // n):
+        sel = np.nonzero(qs // n == b)[0]
+        a = torch.from_numpy(f1[b].reshape(n, c)[qs[sel] - b * n]).double()
+        t = torch.from_numpy(f2[b].reshape(n, c)).double()
+        rows[torch.from_numpy(sel)] = ((a @ t.T) / np.sqrt(c)).reshape(len(sel), 1, h, w)
+    out = [rows]
+    for _ in range(levels - 1):
+        out.append(F.avg_pool2d(out[-1], 2, 2))
+    return [p.permute(0, 2, 3, 1) for p in out]
+
+
 def encoder_params(variant, norm_type, out_dim, seed=99, bias_scale=0.05, norm_jitter=0.2):
     """Parameters of a BasicEncoder ('raft') / SmallEncoder ('small') with any norm type, under the prefix 'enc.'."""
     from oracle import weights

@@ -107,3 +107,64 @@ def test_fp64_encoder_output_shape_on_odd_sizes():
         x = torch.zeros(1, 3, H, W, dtype=torch.float64)
         out = rt.encoder(rt.Ops(p, torch.float64), x, 'enc', 'instance', False)
         assert tuple(out.shape) == (1, 128, -(-H // 8), -(-W // 8))
+
+
+# ------------------------------------------------------------------------------------ large grids (test_gpu_large.py)
+def test_lookup_path_mirror_known_answers():
+    assert cases.lookup_path(1, 8, 32, 4, 4, 324) == 'window-vec'       # every level width a multiple of 4
+    assert cases.lookup_path(2, 9, 13, 4, 3, 196) == 'window'
+    assert cases.lookup_path(1, 8, 32, 4, 2, 100) == 'generic'          # no window kernel for radius 2
+    assert cases.lookup_path(1, 17, 19, 5, 4, 405) == 'generic'         # ... nor for 5 levels
+    assert cases.lookup_path(4, 56, 64, 4, 4, 384) == 'window-vec'      # the benchmark grid, the loop's operand planes
+    assert cases.lookup_path(1, 180, 320, 4, 4, 324) == 'generic'       # 1440p: 3.3e9 level-0 elements
+    assert cases.lookup_path(3, 136, 240, 4, 4, 324) == 'generic'       # 1080p padded to 1088, batch 3: 3.2e9
+
+
+def test_large_cases_straddle_the_lookup_limits():
+    """Each large case sits on the side of the 2^31 (and 2^32) element limits its comment gives, for RAFT (radius 4) and
+    SmallRAFT (radius 3), with fp32 output rows (retrieve) and fp16 operand rows (the loop)."""
+    expect = {(1, 215, 215): (2136750625, 'window'), (1, 216, 216): (2176782336, 'generic'),
+              (41, 56, 128): (2106589184, 'window-vec'), (42, 56, 128): (2157969408, 'generic'),
+              (1, 257, 256): (4328587264, 'generic')}
+    assert cases.LARGE_CASES == tuple(expect)
+    for (B, h, w), (elements, path) in expect.items():
+        assert B * (h * w) ** 2 == elements
+        assert (elements >= 2 ** 31) == (path == 'generic')
+        for radius, strides in ((4, (324, 384)), (3, (196, 256))):
+            for stride in strides:
+                assert cases.lookup_path(B, h, w, 4, radius, stride) == path, (B, h, w, radius, stride)
+    assert [B * (h * w) ** 2 > 2 ** 32 for B, h, w in cases.LARGE_CASES] == [False] * 4 + [True]
+
+
+def test_large_samples_hold_the_boundary_queries():
+    """The sampled queries of every large case: the first and last 4 of every image, and the queries whose level-0
+    planes hold elements 2^31 and 2^32, with their neighbours."""
+    want = {(1, 216, 216): [46028], (42, 56, 128): [299593], (1, 257, 256): [32640, 65280]}
+    assert divmod(299593, 56 * 128) == (41, 44 * 128 + 73)              # image 41, pixel y = 44, x = 73
+    for B, h, w in cases.LARGE_CASES:
+        n = h * w
+        bq = cases.boundary_queries(B, h, w)
+        assert bq == want.get((B, h, w), [])
+        qs = cases.large_sample(B, h, w)
+        assert qs.dtype == np.int64 and np.all(np.diff(qs) > 0) and qs[0] == 0 and qs[-1] == B * n - 1
+        s = set(qs.tolist())
+        for q, e in zip(bq, (2 ** 31, 2 ** 32)):
+            assert q * n <= e < (q + 1) * n
+            assert {q - 1, q, q + 1} <= s
+        for b in range(B):
+            assert set(range(b * n, b * n + 4)) | set(range((b + 1) * n - 4, (b + 1) * n)) <= s
+        assert len(s) >= 8 * B + 3 * len(bq) + 24                          # ~32 random queries besides
+    np.testing.assert_array_equal(cases.large_sample(1, 216, 216), cases.large_sample(1, 216, 216))
+
+
+def test_corr_rows_equal_the_oracle_pyramid_rows():
+    """The subset reference of test_gpu_large.py equals the rows of oracle.raft_torch.CorrBlock in float64."""
+    B, h, w, c = 3, 11, 13, 64
+    f1, f2 = cases.fmaps(B, h, w, c, seed=3)
+    full = rt.CorrBlock(torch.from_numpy(f1).double(), torch.from_numpy(f2).double(), 4, 4).corr_pyramid
+    qs = np.array([0, 5, 142, 143, 300, 428])
+    rows = cases.corr_rows(f1, f2, qs, 4)
+    assert len(rows) == 4
+    for l in range(4):
+        assert rows[l].dtype == torch.float64 and rows[l].shape == full[l][qs].shape
+        np.testing.assert_allclose(rows[l].numpy(), full[l][qs].numpy(), rtol=1e-13, atol=1e-13)
