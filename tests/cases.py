@@ -187,3 +187,80 @@ def encoder_params(variant, norm_type, out_dim, seed=99, bias_scale=0.05, norm_j
     from oracle import weights
     c0, stages = (64, ((64, 1), (96, 2), (128, 2))) if variant == 'raft' else (32, ((32, 1), (64, 2), (96, 2)))
     return weights.draw_params(weights.encoder_shapes('enc', norm_type, c0, stages, out_dim), seed, bias_scale, norm_jitter)
+
+
+# ---------------------------------------------------------------------------------------------- value sweep
+def split_f16(v):
+    """NumPy emulation of the fp16 hi/lo operand split (split_f16, tf_raft_b200/csrc/common.cuh): values beyond fp16's
+    range, +-inf included, saturate to +-65504, hi = fp16(v), lo = fp16(v - hi) with the difference taken in fp32.
+    astype(np.float16) rounds to nearest even like __float2half_rn, subnormals included.  NaN stays NaN.  Returns
+    (hi, lo) as float16 arrays."""
+    v = np.asarray(v, dtype=F32)
+    with np.errstate(invalid='ignore'):
+        s = np.clip(v, F32(-65504), F32(65504)).astype(F32)
+        hi = s.astype(np.float16)
+        lo = (s - hi.astype(F32)).astype(np.float16)
+    return hi, lo
+
+
+def split_product(a, b):
+    """float64 value of the three-pass product of a (M, K) and b (N, K) on split operands: hi.hi' + hi.lo' + lo.hi'
+    (what the tensor-core kernels compute, up to their fp32 accumulation), and sum |a||b| over K, the scale of that
+    accumulation's error.  Both (M, N)."""
+    ah, al = (x.astype(np.float64) for x in split_f16(a))
+    bh, bl = (x.astype(np.float64) for x in split_f16(b))
+    return ah @ bh.T + ah @ bl.T + al @ bh.T, np.abs(a).astype(np.float64) @ np.abs(b).astype(np.float64).T
+
+
+def dilate(mask, kh, kw, stride=1, padding='same'):
+    """Receptive-field propagation through one convolution: mask (B, H, W) bool of the input pixels that hold a NaN ->
+    the output pixels whose kh x kw window (Keras 'same' / 'valid' padding, stride 1 or 2, asymmetric 'same' padding
+    for stride 2 as TF pads) reaches one.  Images never mix."""
+    B, H, W = mask.shape
+    if padding == 'same':
+        ho, wo = -(-H // stride), -(-W // stride)
+        pt = max((ho - 1) * stride + kh - H, 0) // 2
+        pl = max((wo - 1) * stride + kw - W, 0) // 2
+    else:
+        ho, wo = (H - kh) // stride + 1, (W - kw) // stride + 1
+        pt = pl = 0
+    pad = np.zeros((B, pt + stride * ho + kh, pl + stride * wo + kw), dtype=bool)
+    pad[:, pt:pt + H, pl:pl + W] = mask
+    out = np.zeros((B, ho, wo), dtype=bool)
+    for dy in range(kh):
+        for dx in range(kw):
+            out |= pad[:, dy:dy + stride * ho:stride, dx:dx + stride * wo:stride]
+    return out
+
+
+def encoder_field(mask):
+    """dilate() through BasicEncoder / SmallEncoder without normalisation (extractor.py:113-130): the stem 7x7 s2, three
+    stages of two residual blocks (3x3 convolutions, the first block of stages 2 and 3 with stride 2 and a 1x1 s2 VALID
+    downsample on the skip path), then the 1x1 output convolution, which does not dilate."""
+    m = dilate(mask, 7, 7, 2)
+    for s in (1, 2, 2):
+        for stride in (s, 1):
+            fx = dilate(dilate(m, 3, 3, stride), 3, 3, 1)
+            skip = dilate(m, 1, 1, stride, 'valid') if stride != 1 else m
+            m = fx | skip
+    return m
+
+
+def update_field(variant, net, inp, corr, flow):
+    """dilate() through the update block (update.py:70-153): per-pixel masks of the inputs -> masks of the new hidden
+    state, of delta (the flow head's two 3x3 convolutions) and of the mask head (3x3, then 1x1).  1x1 convolutions
+    (convc1 of both variants, mask.2) do not dilate."""
+    if variant == 'raft':
+        cor = dilate(dilate(corr, 1, 1, 1, 'valid'), 3, 3)
+        flo = dilate(dilate(flow, 7, 7), 3, 3)
+    else:
+        cor = dilate(corr, 1, 1)
+        flo = dilate(dilate(flow, 7, 7), 3, 3)
+    x = dilate(cor | flo, 3, 3) | flow | inp
+    passes = ((1, 5), (5, 1)) if variant == 'raft' else ((3, 3),)
+    h = net
+    for kh, kw in passes:
+        zr = dilate(h | x, kh, kw)
+        q = dilate(zr | h | x, kh, kw)
+        h = h | zr | q
+    return h, dilate(dilate(h, 3, 3), 3, 3), dilate(h, 3, 3)

@@ -35,21 +35,18 @@ writes cover its output columns over the whole grid.  Also checked: every operan
 plane or buffer that the row names, with the stride the kernel assumes.
 """
 import functools
-import hashlib
 import json
 import os
-import shutil
 import subprocess
-import tempfile
 
 import numpy as np
 import pytest
 
 import cases
+import probe_build
 
 ROOT = os.path.abspath(os.path.join(os.path.dirname(__file__), '..'))
 PROBE_SRC = os.path.join(ROOT, 'tests', 'mega_plan_probe.cu')
-CSRC = os.path.join(ROOT, 'tf_raft_b200', 'csrc')
 
 EPI_LINEAR, EPI_GRU_ZR, EPI_GRU_Q = 0, 1, 2
 TC_CONCAT_FLOW, TC_ADVANCE, TC_MASK_ONLY, TC_MASK_TAIL = 1, 2, 4, 8
@@ -67,42 +64,11 @@ CASES = [(v, b, h, w, m, a) for (b, h, w) in GRIDS for (v, m) in FORMS for a in 
 
 
 # ---------------------------------------------------------------------------------------------------------------- probe
-def _nvcc_and_flags():
-    from tf_raft_b200 import build as tb
-    try:
-        nvcc = tb._nvcc()
-    except RuntimeError:
-        return None, None
-    # the library's flags, for an executable linked against the shared cudart (its cudaGetDriverEntryPoint interposes)
-    flags = [f for f in tb.NVCC_FLAGS if f != '-shared' and not f.startswith('--use_fast_math')]
-    lib = os.path.join(os.path.dirname(os.path.dirname(os.path.realpath(nvcc))), 'lib64')
-    return nvcc, flags + ['-cudart', 'shared', '-Xlinker', '-rpath=' + lib]
-
-
 @pytest.fixture(scope='module')
 def probe():
-    nvcc, flags = _nvcc_and_flags()
-    if nvcc is None:
+    exe = probe_build.build(PROBE_SRC, 'raft_mega_plan_probe')
+    if exe is None:
         pytest.skip('nvcc not found: the plan probe cannot be built')
-    h = hashlib.sha256(' '.join([nvcc] + flags).encode())
-    srcs = [PROBE_SRC, os.path.join(ROOT, 'include', 'raft_b200.h')] + \
-        sorted(os.path.join(CSRC, f) for f in os.listdir(CSRC))
-    for s in srcs:
-        with open(s, 'rb') as f:
-            h.update(os.path.relpath(s, ROOT).encode() + b'\0' + f.read())
-    cache = os.path.join(tempfile.gettempdir(), 'raft_mega_plan_probe_%d' % os.getuid())
-    os.makedirs(cache, exist_ok=True)
-    exe = os.path.join(cache, 'probe_' + h.hexdigest()[:24])
-    if not os.path.exists(exe):
-        tmp = tempfile.mkdtemp(dir=cache)
-        try:
-            out = os.path.join(tmp, 'probe')
-            cmd = [nvcc] + flags + [PROBE_SRC, '-o', out]
-            res = subprocess.run(cmd, capture_output=True, text=True)
-            assert res.returncode == 0, 'nvcc failed:\n' + ' '.join(cmd) + '\n' + res.stdout + res.stderr
-            os.replace(out, exe)
-        finally:
-            shutil.rmtree(tmp, ignore_errors=True)
     return exe
 
 

@@ -47,12 +47,28 @@ inline int launch(void (*kernel)(P...), dim3 grid, dim3 block, size_t smem, cuda
   return raft_launch_status();
 }
 
+// ReLU that keeps NaN: max.NaN returns NaN when an operand is NaN; for every other input it is fmaxf(v, 0) (-0 -> +0).
+// fmaxf returns the non-NaN operand, so fmaxf(NaN, 0) = 0 would hide a NaN that torch and TF propagate.
+__device__ __forceinline__ float relu_nan(float v) {
+  float r;
+  asm("max.NaN.f32 %0, %1, 0f00000000;" : "=f"(r) : "f"(v));
+  return r;
+}
+
 // ------------------------------------------------------------------------------------------
 // fp16 hi/lo split: v ~= float(hi) + float(lo), |error| <= 2^-23 |v| in the normal range.
 // The tensor-core path computes x*w as xh*wh + xl*wh + xh*wl with fp32 accumulation.
+// Values beyond fp16's range, +-inf included, saturate to +-65504 (instead of an inf hi and a NaN lo downstream).  NaN
+// stays NaN: max.NaN / min.NaN cost what fmaxf / fminf cost and give their bits for every other input.
 // ------------------------------------------------------------------------------------------
+__device__ __forceinline__ float f16_saturate(float v) {
+  float r;
+  asm("max.NaN.f32 %0, %1, 0fC77FE000;\n\tmin.NaN.f32 %0, %0, 0f477FE000;" : "=f"(r) : "f"(v));   // +-65504
+  return r;
+}
+
 __device__ __forceinline__ void split_f16(float v, __half& hi, __half& lo) {
-  v = fminf(fmaxf(v, -65504.f), 65504.f);            // saturate instead of inf -> NaN downstream
+  v = f16_saturate(v);
   hi = __float2half_rn(v);
   lo = __float2half_rn(v - __half2float(hi));
 }
@@ -60,8 +76,8 @@ __device__ __forceinline__ void split_f16(float v, __half& hi, __half& lo) {
 // Two values at once: the packed conversion (cvt.rn.f16x2.f32 -> F2FP.F16.F32.PACK_AB, ALU pipe) instead of two scalar F2F
 // (conversion pipe, a quarter of the rate).  Same roundings as split_f16; lane order as pack_h2 (a in the low half).
 __device__ __forceinline__ void split_f16x2(float a, float b, uint32_t& hi2, uint32_t& lo2) {
-  a = fminf(fmaxf(a, -65504.f), 65504.f);
-  b = fminf(fmaxf(b, -65504.f), 65504.f);
+  a = f16_saturate(a);
+  b = f16_saturate(b);
   const __half2 h = __floats2half2_rn(a, b);
   const float2 hf = __half22float2(h);
   const __half2 l = __floats2half2_rn(a - hf.x, b - hf.y);

@@ -145,7 +145,7 @@ __device__ __forceinline__ void tc_epilogue_regs(const TcConvParams& p, float (&
     const bool full = col + 32 <= p.n_total;
 #pragma unroll
     for (int j = 0; j < 32; ++j) {
-      if (p.act == ACT_RELU) v[j] = fmaxf(v[j], 0.0f);
+      if (p.act == ACT_RELU) v[j] = relu_nan(v[j]);
       v[j] *= p.out_scale;
     }
     if (full) {
@@ -157,18 +157,18 @@ __device__ __forceinline__ void tc_epilogue_regs(const TcConvParams& p, float (&
             float r8[8];
             ldnc8(rp + 8 * q, r8);
 #pragma unroll
-            for (int e = 0; e < 8; ++e) v[8 * q + e] = fmaxf(v[8 * q + e] + r8[e], 0.f);
+            for (int e = 0; e < 8; ++e) v[8 * q + e] = relu_nan(v[8 * q + e] + r8[e]);
           }
         } else if (((p.res_stride | p.res_c0) & 3) == 0) {
 #pragma unroll
           for (int q = 0; q < 8; ++q) {
             const float4 r4 = ldg4(rp + 4 * q);
-            v[4 * q] = fmaxf(v[4 * q] + r4.x, 0.f); v[4 * q + 1] = fmaxf(v[4 * q + 1] + r4.y, 0.f);
-            v[4 * q + 2] = fmaxf(v[4 * q + 2] + r4.z, 0.f); v[4 * q + 3] = fmaxf(v[4 * q + 3] + r4.w, 0.f);
+            v[4 * q] = relu_nan(v[4 * q] + r4.x); v[4 * q + 1] = relu_nan(v[4 * q + 1] + r4.y);
+            v[4 * q + 2] = relu_nan(v[4 * q + 2] + r4.z); v[4 * q + 3] = relu_nan(v[4 * q + 3] + r4.w);
           }
         } else {
 #pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j] + __ldg(rp + j), 0.f);
+          for (int j = 0; j < 32; ++j) v[j] = relu_nan(v[j] + __ldg(rp + j));
         }
       }
     } else {                                           // ragged tail: concat columns / zeros / residual per column
@@ -176,7 +176,7 @@ __device__ __forceinline__ void tc_epilogue_regs(const TcConvParams& p, float (&
       for (int j = 0; j < 32; ++j) {
         const int cj = col + j - p.n_total;
         if (cj >= 0) v[j] = (p.concat_src && cj < p.concat_n) ? __ldg(p.concat_src + pix * p.concat_n + cj) : 0.0f;
-        else if (p.residual) v[j] = fmaxf(v[j] + __ldg(p.residual + pix * (size_t)p.res_stride + p.res_c0 + col + j), 0.0f);
+        else if (p.residual) v[j] = relu_nan(v[j] + __ldg(p.residual + pix * (size_t)p.res_stride + p.res_c0 + col + j));
       }
     }
     if (p.out_f32) {

@@ -344,7 +344,7 @@ __global__ void __launch_bounds__(256) conv_simt_kernel(const SimtConvParams p) 
       if (n >= p.cout) continue;
       float v = acc[i][j] + (p.bias ? __ldg(p.bias + n) : 0.f);
       if (p.post_scale) v = v * __ldg(p.post_scale + n) + __ldg(p.post_shift + n);
-      if (p.act == SACT_RELU) v = fmaxf(v, 0.f);
+      if (p.act == SACT_RELU) v = relu_nan(v);
       else if (p.act == SACT_SIGMOID) v = sigmoidf_acc(v);
       else if (p.act == SACT_TANH) v = tanhf(v);
       v *= p.out_scale;
@@ -557,7 +557,7 @@ __global__ void __launch_bounds__(256) norm_stats_kernel(const float* __restrict
       n += 1.f;
     }
     mean = K + s1 / n;
-    m2 = fmaxf(s2 - s1 * s1 / n, 0.f);
+    m2 = relu_nan(s2 - s1 * s1 / n);                   // a NaN sample keeps the variance NaN, not 0
   }
   red[0][threadIdx.x] = n; red[1][threadIdx.x] = mean; red[2][threadIdx.x] = m2;
   __syncthreads();
@@ -622,13 +622,13 @@ __global__ void norm_apply_kernel(const float* __restrict__ y, size_t npix, int 
 #pragma unroll
       for (int e = 0; e < 8; ++e) {
         v[e] = (yy[e] - __ldg(mp + e)) * __ldg(ap + e) + __ldg(bp + e);
-        if (relu) v[e] = fmaxf(v[e], 0.f);
+        if (relu) v[e] = relu_nan(v[e]);
       }
       if (skip32) {
         const float4 s0 = *reinterpret_cast<const float4*>(skip32 + px * C + c), s1 = *reinterpret_cast<const float4*>(skip32 + px * C + c + 4);
         const float ss[8] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
 #pragma unroll
-        for (int e = 0; e < 8; ++e) v[e] = fmaxf(ss[e] + v[e], 0.f);
+        for (int e = 0; e < 8; ++e) v[e] = relu_nan(ss[e] + v[e]);
       } else if (skip_hi) {
         const uint4 h4 = *reinterpret_cast<const uint4*>(skip_hi + px * c_pad + c), l4 = *reinterpret_cast<const uint4*>(skip_lo + px * c_pad + c);
         const uint32_t hw[4] = {h4.x, h4.y, h4.z, h4.w}, lw[4] = {l4.x, l4.y, l4.z, l4.w};
@@ -636,8 +636,8 @@ __global__ void norm_apply_kernel(const float* __restrict__ y, size_t npix, int 
         for (int e = 0; e < 4; ++e) {
           const float2 hf = __half22float2(*reinterpret_cast<const __half2*>(&hw[e]));
           const float2 lf = __half22float2(*reinterpret_cast<const __half2*>(&lw[e]));
-          v[2 * e] = fmaxf(hf.x + lf.x + v[2 * e], 0.f);
-          v[2 * e + 1] = fmaxf(hf.y + lf.y + v[2 * e + 1], 0.f);
+          v[2 * e] = relu_nan(hf.x + lf.x + v[2 * e]);
+          v[2 * e + 1] = relu_nan(hf.y + lf.y + v[2 * e + 1]);
         }
       }
       if (out32) {
@@ -767,7 +767,7 @@ __global__ void context_split_kernel(const float* __restrict__ cnet, size_t npix
     const int c = (int)(i - px * C);
     const float v = cnet[i];
     if (c < hid) net[px * hid + c] = tanhf(v);
-    else inp[px * ctx + (c - hid)] = fmaxf(v, 0.f);
+    else inp[px * ctx + (c - hid)] = relu_nan(v);
   }
 }
 
