@@ -114,6 +114,18 @@ int raft_b200_bilinear_sampler(const float* image, const float* coords, int M, i
 /* coords_grid(B, h, w): corr.py:72-90 -> (B, h, w, 2), out[b,y,x] = (x, y).                    */
 int raft_b200_coords_grid(int B, int h, int w, float* out, void* stream);
 
+/* RAFT's warm start: forward interpolation of a (B,h,w,2) low-resolution flow (an addition beyond the reference, whose
+ * loop always starts from zero flow).  Per image, source pixel (x, y) lands at (x1, y1) = (x + fx, y + fy) in fp64 and is
+ * valid iff 0 < x1 < w and 0 < y1 < h (NaN / inf never are); target (X, Y) receives a copy of the flow of the valid
+ * source minimising (x1 - X)^2 + (y1 - Y)^2 (fp64, each operation rounded, no FMA), ties to the lowest source index;
+ * an image without a valid source gets zero flow.  out (B,h,w,2) must not alias flow.  O((h*w)^2) per image;
+ * h*w must stay below 2^31 - 512 (RAFT_ERR_BAD_SHAPE otherwise).                                                    */
+int raft_b200_forward_interpolate(const float* flow, int B, int h, int w, float* out, void* stream);
+
+/* coords1 = coords_grid(B,h,w) + flow_init (fp32, one rounding per component): the loop's warm-start entry state.
+ * coords1 may alias flow_init.                                                                                      */
+int raft_b200_coords_init(const float* flow_init, int B, int h, int w, float* coords1, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Update blocks  (tf_raft/layers/update.py)
  * ------------------------------------------------------------------------------------------- */
@@ -240,7 +252,9 @@ int raft_b200_upflow8(const float* flow, int B, int h, int w, float* out, void* 
  *   pyr          : the CorrBlock pyramid (levels entries)
  *   net          : (B,h,w,hidden) in/out -- the tanh() half of cnet's output on entry
  *   inp          : (B,h,w,context)       -- the relu() half
- *   coords1      : (B,h,w,2) in/out; must hold coords_grid(B,h,w) on entry (model.py:89)
+ *   coords1      : (B,h,w,2) in/out; holds coords_grid(B,h,w) plus an initial flow on entry: zero flow in the
+ *                  reference (model.py:89), raft_b200_coords_init for a warm start; the loop's first
+ *                  flow is coords1 - coords_grid
  *   flow_up      : iters pointers to (B,8h,8w,2) outputs; entries may be NULL to skip that
  *                  iteration's upsampling (predict_step keeps only the last, model.py:166);
  *                  for BASIC a skipped iteration also skips the mask head.                        */

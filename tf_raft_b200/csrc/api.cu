@@ -1,6 +1,7 @@
 // extern "C" entry points of libraft_b200.so (see include/raft_b200.h for the contract and the
 // reference file:line each one replaces).  Host code only decides shapes and launches kernels;
 // there is no CPU compute path.
+#include <limits.h>
 #include <stdlib.h>
 
 #include <algorithm>
@@ -8,6 +9,7 @@
 #include "corr_tc.cuh"
 #include "encoder.cuh"
 #include "train.cuh"
+#include "video.cuh"
 
 namespace raft {
 thread_local long long g_launches = 0;
@@ -397,6 +399,21 @@ int raft_b200_coords_grid(int B, int h, int w, float* out, void* stream) {
   if (!out) return RAFT_ERR_BAD_ARG;
   RAFT_TRY(check_dims(B, h, w));
   return launch(coords_grid_kernel, grid_for((size_t)B * h * w), 256, 0, reinterpret_cast<cudaStream_t>(stream), out, B, h, w);
+}
+
+int raft_b200_forward_interpolate(const float* flow, int B, int h, int w, float* out, void* stream) {
+  if (!flow || !out) return RAFT_ERR_BAD_ARG;
+  RAFT_TRY(check_dims(B, h, w));
+  if ((size_t)h * w > (size_t)INT_MAX - kFiChunk) return RAFT_ERR_BAD_SHAPE;     // pixel indices are int
+  dim3 grid((unsigned)ceil_div(h * w, kFiThreads), (unsigned)std::min(B, 65535));
+  return launch(forward_interpolate_kernel, grid, kFiThreads, 0, reinterpret_cast<cudaStream_t>(stream), flow, out, B, h, w);
+}
+
+int raft_b200_coords_init(const float* flow_init, int B, int h, int w, float* coords1, void* stream) {
+  if (!flow_init || !coords1) return RAFT_ERR_BAD_ARG;
+  RAFT_TRY(check_dims(B, h, w));
+  return launch(coords_init_kernel, grid_for((size_t)B * h * w), 256, 0, reinterpret_cast<cudaStream_t>(stream), flow_init,
+                coords1, B, h, w);
 }
 
 int raft_b200_update_prepared_bytes(int variant, int corr_channels, int precision, size_t* bytes) {

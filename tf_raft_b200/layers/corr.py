@@ -51,6 +51,41 @@ def coords_grid(batch_size, height, width, device=None):
     return out
 
 
+def _flow_field(flow, what):
+    flow = _lib.f32c(flow)
+    if flow.dim() != 4 or flow.shape[-1] != 2:
+        raise ValueError(f'{what}: expected a (B, h, w, 2) flow, got {tuple(flow.shape)}')
+    return flow
+
+
+def forward_interpolate(flow):
+    """RAFT's warm start for the next pair of a video (an addition: tf-raft has none).  (B, h, w, 2) -> (B, h, w, 2).
+
+    Per image, source pixel (x, y) lands at (x + fx, y + fy) (fp64) and counts only strictly inside the frame,
+    0 < x1 < w and 0 < y1 < h (NaN / inf flow never does).  Target pixel (X, Y) takes the flow of the landed source
+    nearest to it (squared fp64 distance), ties to the lowest source index: scipy's
+    `griddata((x1, y1), f, (X, Y), method='nearest')` with a deterministic tie rule.  Where griddata raises (no source
+    lands inside the frame) the image gets zero flow.  Brute force on the GPU: O((h*w)^2) per image."""
+    flow = _flow_field(flow, 'forward_interpolate')
+    b, h, w, _ = flow.shape
+    out = torch.empty_like(flow)
+    with torch.cuda.device(flow.device):
+        _lib.check(_lib.lib().raft_b200_forward_interpolate(_lib.ptr(flow), b, h, w, _lib.ptr(out), _lib.stream()),
+                   'forward_interpolate')
+    return out
+
+
+def coords_init(flow_init):
+    """coords_grid(B, h, w) + flow_init in fp32: the iteration loop's entry state for a warm start (B, h, w, 2)."""
+    flow_init = _flow_field(flow_init, 'coords_init')
+    b, h, w, _ = flow_init.shape
+    out = torch.empty_like(flow_init)
+    with torch.cuda.device(flow_init.device):
+        _lib.check(_lib.lib().raft_b200_coords_init(_lib.ptr(flow_init), b, h, w, _lib.ptr(out), _lib.stream()),
+                   'coords_init')
+    return out
+
+
 def upflow8(flow, mode='bilinear'):
     """Reference corr.py:93-96: 8 * tf.image.resize(flow, (8h, 8w), 'bilinear') (half-pixel centres)."""
     if mode != 'bilinear':

@@ -11,7 +11,7 @@ from collections import OrderedDict
 import torch
 
 from . import _lib
-from .layers.corr import CorrBlock, coords_grid, upflow8
+from .layers.corr import CorrBlock, coords_grid, coords_init, forward_interpolate, upflow8
 from .layers.extractor import BasicEncoder, SmallEncoder
 from .layers.update import BasicUpdateBlock, SmallUpdateBlock
 from .losses import end_point_error, sequence_loss
@@ -93,6 +93,10 @@ class RAFT:
     def _encode(self, image1, image2, training):
         # model.py:70-71 (2*(x/255)-1) happens inside the encoders' first load (raw_image=True)
         fmap1, fmap2 = self.fnet([image1, image2], training=training, raw_image=True)     # :74
+        net, inp = self._context(image1, training)
+        return fmap1, fmap2, net, inp
+
+    def _context(self, image1, training):
         cnet = self.cnet(image1, training=training, raw_image=True)                       # :82
         b, h, w, _ = cnet.shape
         net = torch.empty((b, h, w, self.hidden_dim), dtype=torch.float32, device=cnet.device)
@@ -101,7 +105,7 @@ class RAFT:
             _lib.check(_lib.lib().raft_b200_context_split(_lib.ptr(cnet), b * h * w, self.hidden_dim,
                                                           self.context_dim, _lib.ptr(net), _lib.ptr(inp),
                                                           _lib.stream()), 'context_split')
-        return fmap1, fmap2, net, inp
+        return net, inp
 
     def _loop(self, corr_block, net, inp, coords1, flow_ups, b, h, w):
         ub = self.update_block
@@ -112,64 +116,144 @@ class RAFT:
                 self.corr_radius, _lib.ptr(net), _lib.ptr(inp), _lib.ptr(coords1), _lib.ptr_array(flow_ups),
                 len(flow_ups), b, h, w, _lib.ptr(ws), ws.numel(), self.precision, _lib.stream()), 'forward_loop')
 
-    def __call__(self, inputs, training, *, last_only=False):
+    def __call__(self, inputs, training, *, last_only=False, flow_init=None):
         """inputs = [image1, image2], each (B, H, W, 3) float in 0..255 on the GPU.
 
         `training` is required, as in the reference (model.py:68).  `last_only=True` (keyword-only
         extra) computes just the final prediction -- what predict_step returns (model.py:166).
+        `flow_init` (keyword-only extra; tf-raft has no warm start): a (B, H/8, W/8, 2) float32 tensor on the images'
+        device.  The loop then starts from coords1 = coords0 + flow_init (raft_b200_coords_init) instead of zero flow:
+        RAFT's warm start, usually `forward_interpolate` of the previous pair's low-resolution flow (predict_video).
         With `use_graph=True` the whole forward of a given input shape is captured once into a CUDA graph
-        and replayed; the returned tensors are then static buffers that the next call overwrites."""
+        and replayed; the returned tensors are then static buffers that the next call overwrites.  `flow_init` is then
+        one more static input, copied in before each replay; warm and cold calls never share a graph."""
         image1, image2 = inputs
         image1, image2 = _lib.f32c(image1), _lib.f32c(image2)
+        if flow_init is not None:
+            flow_init = self._check_flow_init(flow_init, image1)
         self._sync_trained_params()
         if self.use_graph and not training:
-            return self._graph_call(image1, image2, last_only)
-        return self._forward(image1, image2, training, last_only)
+            return self._graph_call(image1, image2, last_only, flow_init)
+        return self._forward(image1, image2, training, last_only, flow_init)
 
-    def _graph_call(self, image1, image2, last_only):
-        key = (tuple(image1.shape), bool(last_only))
+    @staticmethod
+    def _check_flow_init(flow_init, image):
+        if not isinstance(flow_init, torch.Tensor):
+            raise TypeError(f'flow_init must be a torch tensor, got {type(flow_init).__name__}')
+        if flow_init.dtype != torch.float32:
+            raise TypeError(f'flow_init must be float32, got {flow_init.dtype}')
+        if flow_init.device != image.device:
+            raise ValueError(f'flow_init is on {flow_init.device}, the images on {image.device}')
+        bs, H, W, _ = image.shape
+        want = (bs, H // 8, W // 8, 2)
+        if tuple(flow_init.shape) != want:
+            raise ValueError(f'flow_init: expected {want} for {H}x{W} images, got {tuple(flow_init.shape)}')
+        return flow_init.contiguous()
+
+    def _graph_call(self, image1, image2, last_only, flow_init=None):
+        warm = flow_init is not None
+        key = (tuple(image1.shape), bool(last_only), warm)
         entry = self._graphs.get(key)
         if entry is None:
             s1, s2 = image1.clone(), image2.clone()
+            s3 = flow_init.clone() if warm else None
             side = torch.cuda.Stream(device=self.device)
             side.wait_stream(torch.cuda.current_stream(self.device))
             with torch.cuda.stream(side):                      # warm-up: allocations, attributes, weight packing
                 for _ in range(2):
-                    self._forward(s1, s2, False, last_only)
+                    self._forward(s1, s2, False, last_only, s3)
             torch.cuda.current_stream(self.device).wait_stream(side)
             torch.cuda.synchronize(self.device)
             graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(graph):
-                outs = self._forward(s1, s2, False, last_only)
+                outs = self._forward(s1, s2, False, last_only, s3)
             # The captured kernels hold raw addresses of the encoder / update-block workspaces; those caches keep one
             # shape at a time, so the graph entry owns references to the buffers it was captured with.
             keep = [list(m._ws.values()) for m in (self.fnet, self.cnet, self.update_block)]
-            entry = (graph, s1, s2, outs, self._last, keep)
+            entry = (graph, s1, s2, s3, outs, self._last, keep)
             self._graphs[key] = entry
-        graph, s1, s2, outs, last, _keep = entry
+        graph, s1, s2, s3, outs, last, _keep = entry
         s1.copy_(image1, non_blocking=True)
         s2.copy_(image2, non_blocking=True)
+        if warm:
+            s3.copy_(flow_init, non_blocking=True)
         graph.replay()
         self._last = last
         return outs
 
-    def _forward(self, image1, image2, training, last_only):
-        bs, H, W, _ = image1.shape
+    @staticmethod
+    def _check_size(H, W):
         if H % 8 or W % 8:
             raise ValueError(f'image height and width must be multiples of 8 (got {H}x{W}); the reference fails in '
                              'update.py:146 for other sizes -- crop-or-pad first (datasets/dataset.py:323-334)')
+
+    def _forward(self, image1, image2, training, last_only, flow_init=None):
+        bs, H, W, _ = image1.shape
+        self._check_size(H, W)
+        fmap1, fmap2, net, inp = self._encode(image1, image2, training)
+        return self._iterate(fmap1, fmap2, net, inp, bs, H, W, training, last_only, flow_init)
+
+    def _iterate(self, fmap1, fmap2, net, inp, bs, H, W, training, last_only, flow_init):
+        """Everything after the encoders: pyramid, entry state, iteration loop (model.py:77-106)."""
         h, w = H // 8, W // 8
         iters = self.iters if training else self.iters_pred                  # model.py:92
-        fmap1, fmap2, net, inp = self._encode(image1, image2, training)
         corr_block = CorrBlock(fmap1, fmap2, num_levels=self.corr_levels, radius=self.corr_radius,
                                precision=self.precision)                      # :77-79
-        coords1 = coords_grid(bs, h, w, self.device)                          # :89
+        if flow_init is None:
+            coords1 = coords_grid(bs, h, w, self.device)                      # :89
+        else:
+            coords1 = coords_init(flow_init)                                  # :89 plus the warm start's initial flow
         preds = [torch.empty((bs, H, W, 2), dtype=torch.float32, device=self.device)
                  if (not last_only or i == iters - 1) else None for i in range(iters)]
         if iters:
             self._loop(corr_block, net, inp, coords1, preds, bs, h, w)        # :93-106
         self._last = dict(net=net, coords1=coords1, corr_block=corr_block)
         return [p for p in preds if p is not None] if last_only else preds
+
+    def predict_video(self, frames, *, warm_start=True):
+        """Flow along B video clips at once (an addition: tf-raft evaluates pairs only).
+
+        `frames` is an iterable of (B, H, W, 3) CUDA tensors in 0..255, frame t of B independent clips.  A generator:
+        for t = 1 .. T-1 it yields the finest (B, H, W, 2) flow from frame t-1 to frame t after `iters_pred`
+        iterations, what `predict_step` returns for that pair.  Each frame is encoded by `fnet` once: its feature map
+        serves as fmap2 of one pair and fmap1 of the next.  The feature encoder's instance norm works per image, so on
+        the native encoders (the f16x2 default) the result does not depend on the batch the image was encoded in and
+        every pair equals `__call__` bit for bit; the cuDNN encoders of the fp32 configuration may pick another
+        algorithm for the smaller batch and differ in the last bits.  A step costs two image encodes (fnet on frame t,
+        cnet on frame t-1) instead of the three of a `__call__` per pair.
+
+        `warm_start=True`: from the second pair on, the loop starts from `forward_interpolate` of the previous pair's
+        final low-resolution flow (coords1 - coords0), as RAFT does on Sintel and KITTI sequences; the first pair
+        starts from zero flow.  `warm_start=False`: every pair starts from zero flow.
+
+        A frame whose shape differs from the first raises ValueError; fewer than two frames yield nothing.  Eager
+        only: the video step is never captured into a CUDA graph, whatever `use_graph` says, and every yielded tensor
+        is a new one."""
+        self._sync_trained_params()
+        if self.iters_pred < 1:
+            raise ValueError('predict_video needs iters_pred >= 1')
+        shape = coords0 = frame_prev = fmap_prev = flow_init = None
+        for t, frame in enumerate(frames):
+            frame = _lib.f32c(frame)
+            if shape is None:
+                shape = tuple(frame.shape)
+                if len(shape) != 4 or shape[-1] != 3:
+                    raise ValueError(f'frames must be (B, H, W, 3); got {shape}')
+                bs, H, W, _ = shape
+                self._check_size(H, W)
+            elif tuple(frame.shape) != shape:
+                raise ValueError(f'frame {t}: shape {tuple(frame.shape)} differs from the first frame {shape}')
+            fmap = self.fnet(frame, training=False, raw_image=True)                    # model.py:74, frame t only
+            if frame_prev is not None:
+                net, inp = self._context(frame_prev, False)                                # :82-86
+                flow = self._iterate(fmap_prev, fmap, net, inp, bs, H, W, False, True, flow_init)[-1]
+                if warm_start:
+                    if coords0 is None:
+                        coords0 = coords_grid(bs, H // 8, W // 8, self.device)
+                    # flow_low = coords1 - coords0 with flow_advance_kernel's fp32 subtraction
+                    flow_init = forward_interpolate(self._last['coords1'] - coords0)
+                yield flow
+            frame_prev, fmap_prev = frame, fmap
 
     call = __call__
 
