@@ -126,6 +126,19 @@ int raft_b200_forward_interpolate(const float* flow, int B, int h, int w, float*
  * coords1 may alias flow_init.                                                                                      */
 int raft_b200_coords_init(const float* flow_init, int B, int h, int w, float* coords1, void* stream);
 
+/* Forward-backward consistency (an addition beyond the reference).  flow_fw, flow_bw: (B, H, W, 2) float32, the flow
+ * a->b and b->a of B image pairs, 8-byte aligned.  occ_fw[b,y,x] = 1 where pixel (x,y) of image a has no consistent
+ * correspondence in b, occ_bw likewise for image b; else 0.  One launch covers both directions.  For direction fw,
+ * with F = flow_fw[b], G = flow_bw[b] (bw swaps them), every operation a rounded fp32 one in this order, no FMA:
+ *   p = (x + Fx, y + Fy); occluded unless 0 <= px <= W-1 and 0 <= py <= H-1 (NaN never is inside);
+ *   g = bilinear sample of G at p (x0 = floor(px), x1 = min(x0+1, W-1), ax = px - x0, bx = 1 - ax, y likewise;
+ *       g = by*(bx*G[y0,x0] + ax*G[y0,x1]) + ay*(bx*G[y1,x0] + ax*G[y1,x1]));
+ *   consistent iff |F + g|^2 <= alpha1*(|F|^2 + |g|^2) + alpha2; anything else (NaN included) is occluded.
+ * A non-finite texel makes g non-finite even at weight 0.  alpha1, alpha2 finite and >= 0 (RAFT_ERR_BAD_ARG otherwise);
+ * Sundaram et al. use 0.01 and 0.5 (DESIGN.md section 3.5).                                                         */
+int raft_b200_fb_occlusion(const float* flow_fw, const float* flow_bw, int B, int H, int W, float alpha1, float alpha2,
+                           uint8_t* occ_fw, uint8_t* occ_bw, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Update blocks  (tf_raft/layers/update.py)
  * ------------------------------------------------------------------------------------------- */

@@ -1,4 +1,5 @@
-"""Video inference throughput at the Sintel geometry: per-pair calls against predict_video (cold and warm start).
+"""Video inference throughput at the Sintel geometry: per-pair calls against predict_video (cold and warm start), one
+direction and both directions with occlusion masks.
 
     python scripts/bench_video.py --out DIR [--clips 4 --frames 13 --height 448 --width 1024 --iters 24 12 --repeats 3]
 
@@ -6,12 +7,18 @@ B seeded synthetic clips of T frames, RAFT with the seeded weights of the tests,
 `iters_pred` it times, over the whole sequence (B * (T - 1) flows):
   * per_pair:   model([f_{t-1}, f_t], training=False, last_only=True) for t = 1 .. T-1 (three image encodes per pair);
   * video_cold: model.predict_video(frames, warm_start=False) (two image encodes per pair);
-  * video_warm: model.predict_video(frames, warm_start=True) (two encodes plus the forward interpolation).
-Rates are flows per second (B * (T - 1) / window) from CUDA events around device-synchronised windows, after one
-untimed pass of every mode; median and best of `--repeats` windows.  Also timed: one fnet and one cnet call on B frames,
-and the forward_interpolate kernel on (4, 56, 128) and (1, 216, 216) flows.  The GPU's name, power limit and maximum SM
-clock are read (nvidia-smi, query only) in the same run and written beside the numbers: one JSON line on stdout and in
-DIR/bench_video.json.
+  * video_warm: model.predict_video(frames, warm_start=True) (two encodes plus the forward interpolation);
+and both directions of every pair with their forward-backward occlusion masks:
+  * per_pair_both:    model([f_{t-1}, f_t]) and model([f_t, f_{t-1}]) plus fb_occlusion (six image encodes per pair);
+  * video_bidir_cold: model.predict_video(frames, warm_start=False, bidirectional=True) (two encodes per pair, one
+                      batch-2B loop);
+  * video_bidir_warm: the same with warm_start=True (one forward interpolation of both halves per pair).
+Rates are flows per second (B * (T - 1) / window) for the one-direction modes and bidirectional pairs per second
+(B * (T - 1) / window, each pair two flows and two masks) for the others, from CUDA events around device-synchronised
+windows, after one untimed pass of every mode; median and best of `--repeats` windows.  Also timed: one fnet and one cnet
+call on B frames, the forward_interpolate kernel on (B, H/8, W/8) and (1, 216, 216) flows, and fb_occlusion on
+(B, H, W) flows.  The GPU's name, power limit and maximum SM clock are read (nvidia-smi, query only) in the same run and
+written beside the numbers: one JSON line on stdout and in DIR/bench_video.json.
 """
 import argparse
 import json
@@ -79,9 +86,15 @@ def main():
         for t in range(1, n):
             model([frames[t - 1], frames[t]], training=False, last_only=True)
 
-    def video(warm):
+    def per_pair_both():
+        for t in range(1, n):
+            fw = model([frames[t - 1], frames[t]], training=False, last_only=True)[-1]
+            bw = model([frames[t], frames[t - 1]], training=False, last_only=True)[-1]
+            T.fb_occlusion(fw, bw)
+
+    def video(warm, bidirectional=False):
         def run():
-            for _ in model.predict_video(frames, warm_start=warm):
+            for _ in model.predict_video(frames, warm_start=warm, bidirectional=bidirectional):
                 pass
         return run
 
@@ -89,17 +102,27 @@ def main():
                   clips=B, frames=n, height=H, width=W, precision='f16x2', repeats=args.repeats, modes={})
     for iters in args.iters:
         model.iters_pred = iters
-        modes = {'per_pair': per_pair, 'video_cold': video(False), 'video_warm': video(True)}
+        modes = {'per_pair': per_pair, 'video_cold': video(False), 'video_warm': video(True),
+                 'per_pair_both': per_pair_both, 'video_bidir_cold': video(False, True),
+                 'video_bidir_warm': video(True, True)}
         for fn in modes.values():                                  # warm-up: every shape and mode once
             fn()
         # the same sequence's last flow from the two cold paths, as a cross-check (bit-identical on the native encoders)
         last_pair = model([frames[-2], frames[-1]], training=False, last_only=True)[-1].clone()
         last_video = list(model.predict_video(frames[-2:], warm_start=False))[-1]
         row = {'cold_video_equals_per_pair': bool(torch.equal(last_pair, last_video))}
+        # and both directions: the cold bidirectional video against predict_bidirectional and the two per-pair flows
+        both = [x.clone() for x in model.predict_bidirectional([frames[-2], frames[-1]])]
+        last_bidir = list(model.predict_video(frames[-2:], warm_start=False, bidirectional=True))[-1]
+        last_bw = model([frames[-1], frames[-2]], training=False, last_only=True)[-1]
+        row['cold_bidir_video_equals_per_pair'] = bool(
+            all(torch.equal(a, b) for a, b in zip(both, last_bidir)) and torch.equal(both[0], last_pair)
+            and torch.equal(both[1], last_bw))
         for name, fn in modes.items():
             ms = timed(fn, args.repeats)
-            row[name] = {'flows_per_s_median': round(flows / (statistics.median(ms) / 1e3), 2),
-                         'flows_per_s_best': round(flows / (min(ms) / 1e3), 2),
+            unit = 'bidir_pairs' if name in ('per_pair_both', 'video_bidir_cold', 'video_bidir_warm') else 'flows'
+            row[name] = {f'{unit}_per_s_median': round(flows / (statistics.median(ms) / 1e3), 2),
+                         f'{unit}_per_s_best': round(flows / (min(ms) / 1e3), 2),
                          'window_ms': [round(m, 2) for m in ms]}
         result['modes'][f'iters_pred={iters}'] = row
 
@@ -120,6 +143,17 @@ def main():
         ms = timed(lambda: [T.forward_interpolate(flow) for _ in range(reps)], args.repeats)
         fi[f'{b}x{h}x{w}_ms'] = round(statistics.median(ms) / reps, 4)
     result['forward_interpolate'] = fi
+
+    fw, bw = (torch.from_numpy(rng.uniform(-3, 3, (B, H, W, 2)).astype(np.float32)).cuda() for _ in range(2))
+    for _ in range(3):
+        T.fb_occlusion(fw, bw)
+    ms = timed(lambda: [T.fb_occlusion(fw, bw) for _ in range(50)], args.repeats)
+    # the kernel alone: raw entry-point launches into preallocated masks, queued faster than they run
+    occ = [torch.empty((B, H, W), dtype=torch.bool, device='cuda') for _ in range(2)]
+    args_c = [_lib.ptr(fw), _lib.ptr(bw), B, H, W, 0.01, 0.5, _lib.ptr(occ[0]), _lib.ptr(occ[1]), _lib.stream()]
+    ms_k = timed(lambda: [_lib.lib().raft_b200_fb_occlusion(*args_c) for _ in range(200)], args.repeats)
+    result['fb_occlusion'] = {f'{B}x{H}x{W}_ms_per_call': round(statistics.median(ms) / 50, 4),
+                              f'{B}x{H}x{W}_ms_kernel': round(statistics.median(ms_k) / 200, 4)}
 
     line = json.dumps(result)
     print(line)

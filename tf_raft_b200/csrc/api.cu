@@ -1,6 +1,7 @@
 // extern "C" entry points of libraft_b200.so (see include/raft_b200.h for the contract and the
 // reference file:line each one replaces).  Host code only decides shapes and launches kernels;
 // there is no CPU compute path.
+#include <float.h>
 #include <limits.h>
 #include <stdlib.h>
 
@@ -414,6 +415,17 @@ int raft_b200_coords_init(const float* flow_init, int B, int h, int w, float* co
   RAFT_TRY(check_dims(B, h, w));
   return launch(coords_init_kernel, grid_for((size_t)B * h * w), 256, 0, reinterpret_cast<cudaStream_t>(stream), flow_init,
                 coords1, B, h, w);
+}
+
+int raft_b200_fb_occlusion(const float* flow_fw, const float* flow_bw, int B, int H, int W, float alpha1, float alpha2,
+                           uint8_t* occ_fw, uint8_t* occ_bw, void* stream) {
+  if (!flow_fw || !flow_bw || !occ_fw || !occ_bw) return RAFT_ERR_BAD_ARG;
+  if (!(alpha1 >= 0.0f && alpha1 <= FLT_MAX) || !(alpha2 >= 0.0f && alpha2 <= FLT_MAX)) return RAFT_ERR_BAD_ARG;
+  if ((reinterpret_cast<uintptr_t>(flow_fw) | reinterpret_cast<uintptr_t>(flow_bw)) % sizeof(float2)) return RAFT_ERR_BAD_ARG;
+  RAFT_TRY(check_dims(B, H, W));
+  return launch(fb_occlusion_kernel, grid_for(2 * (size_t)B * H * W), 256, 0, reinterpret_cast<cudaStream_t>(stream),
+                reinterpret_cast<const float2*>(flow_fw), reinterpret_cast<const float2*>(flow_bw), B, H, W, alpha1, alpha2,
+                occ_fw, occ_bw);
 }
 
 int raft_b200_update_prepared_bytes(int variant, int corr_channels, int precision, size_t* bytes) {

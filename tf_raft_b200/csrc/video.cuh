@@ -1,6 +1,6 @@
 // Warm start for video inference: RAFT's forward interpolation of the previous pair's low-resolution flow onto the new
 // frame, and the loop's entry state coords1 = coords_grid + flow_init.  Both are additions beyond tf-raft, whose
-// model.py:89 always starts from zero flow.
+// model.py:89 always starts from zero flow.  Also the forward-backward occlusion check of bidirectional flow.
 #pragma once
 #include <math_constants.h>
 
@@ -78,6 +78,54 @@ __global__ void coords_init_kernel(const float* flow_init, float* coords1, int B
     const float fx = flow_init[2 * i], fy = flow_init[2 * i + 1];
     coords1[2 * i] = __fadd_rn(gx, fx);
     coords1[2 * i + 1] = __fadd_rn(gy, fy);
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
+// fb_occlusion: the forward-backward consistency check (Sundaram, Brox and Keutzer, ECCV 2010; UnFlow's boundary), an
+// addition beyond tf-raft.  Thread i < n = B*H*W handles pixel i of direction fw (F = flow_fw, G = flow_bw), thread
+// n + i pixel i of direction bw (the roles swapped).  Pixel (x, y) of image b:
+//   p = (x + fx, y + fy); occluded unless 0 <= px <= W-1 and 0 <= py <= H-1 (closed; NaN never passes);
+//   g = bilinear sample of G[b] at p: x0 = floor(px), x1 = min(x0 + 1, W-1), ax = px - x0, bx = 1 - ax (y likewise),
+//       g = by*(bx*G[y0,x0] + ax*G[y0,x1]) + ay*(bx*G[y1,x0] + ax*G[y1,x1]);
+//   consistent iff |f + g|^2 <= alpha1*(|f|^2 + |g|^2) + alpha2, every other outcome (NaN included) occluded.
+// Every operation is an explicitly rounded fp32 intrinsic in the order written, so no FMA is contracted and NumPy float32
+// reproduces each bit (oracle/occlusion_np.py).  A non-finite texel reaches g even at weight 0 (0 * inf = NaN).
+// ------------------------------------------------------------------------------------------------
+__global__ void fb_occlusion_kernel(const float2* __restrict__ flow_fw, const float2* __restrict__ flow_bw, int B, int H,
+                                    int W, float alpha1, float alpha2, uint8_t* __restrict__ occ_fw,
+                                    uint8_t* __restrict__ occ_bw) {
+  const size_t hw = (size_t)H * W, n = (size_t)B * hw;
+  const float xmax = (float)(W - 1), ymax = (float)(H - 1);
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < 2 * n; i += (size_t)gridDim.x * blockDim.x) {
+    const bool bw = i >= n;
+    const size_t p = bw ? i - n : i;
+    const float2* F = bw ? flow_bw : flow_fw;
+    const float2* G = (bw ? flow_fw : flow_bw) + (p / hw) * hw;
+    const size_t q = p % hw;
+    const float2 f = F[p];
+    const float px = __fadd_rn((float)(q % W), f.x), py = __fadd_rn((float)(q / W), f.y);
+    bool occ = true;
+    if (px >= 0.0f && px <= xmax && py >= 0.0f && py <= ymax) {
+      const float fx0 = floorf(px), fy0 = floorf(py);
+      const int x0 = (int)fx0, y0 = (int)fy0;
+      const size_t x1 = (size_t)min(x0 + 1, W - 1), y1 = (size_t)min(y0 + 1, H - 1);
+      const float ax = __fsub_rn(px, fx0), bx = __fsub_rn(1.0f, ax);
+      const float ay = __fsub_rn(py, fy0), by = __fsub_rn(1.0f, ay);
+      const float2 g00 = G[(size_t)y0 * W + x0], g01 = G[(size_t)y0 * W + x1];
+      const float2 g10 = G[y1 * W + x0], g11 = G[y1 * W + x1];
+      const float gx = __fadd_rn(__fmul_rn(by, __fadd_rn(__fmul_rn(bx, g00.x), __fmul_rn(ax, g01.x))),
+                                 __fmul_rn(ay, __fadd_rn(__fmul_rn(bx, g10.x), __fmul_rn(ax, g11.x))));
+      const float gy = __fadd_rn(__fmul_rn(by, __fadd_rn(__fmul_rn(bx, g00.y), __fmul_rn(ax, g01.y))),
+                                 __fmul_rn(ay, __fadd_rn(__fmul_rn(bx, g10.y), __fmul_rn(ax, g11.y))));
+      const float sx = __fadd_rn(f.x, gx), sy = __fadd_rn(f.y, gy);
+      const float lhs = __fadd_rn(__fmul_rn(sx, sx), __fmul_rn(sy, sy));
+      const float mag = __fadd_rn(__fadd_rn(__fmul_rn(f.x, f.x), __fmul_rn(f.y, f.y)),
+                                  __fadd_rn(__fmul_rn(gx, gx), __fmul_rn(gy, gy)));
+      const float rhs = __fadd_rn(__fmul_rn(alpha1, mag), alpha2);
+      occ = !(lhs <= rhs);
+    }
+    (bw ? occ_bw : occ_fw)[p] = occ ? 1 : 0;
   }
 }
 

@@ -75,6 +75,39 @@ def forward_interpolate(flow):
     return out
 
 
+def fb_occlusion(flow_fw, flow_bw, alpha1=0.01, alpha2=0.5):
+    """Forward-backward occlusion masks of bidirectional flow (an addition: tf-raft has none).
+
+    flow_fw, flow_bw: (B, H, W, 2) flows a->b and b->a of B image pairs on one CUDA device -> (occ_fw, occ_bw), torch.bool
+    (B, H, W).  occ_fw is True where pixel (x, y) of image a has no consistent correspondence in image b: its landing
+    p = (x, y) + f leaves the closed frame [0, W-1] x [0, H-1], or, with g the bilinear sample of flow_bw at p,
+    |f + g|^2 > alpha1 * (|f|^2 + |g|^2) + alpha2 (Sundaram, Brox and Keutzer, ECCV 2010, as used by UnFlow; the
+    defaults are theirs).  occ_bw likewise with the roles swapped.  NaN anywhere in that computation counts as
+    occluded.  Every operation is one fp32 rounding with no FMA (raft_b200_fb_occlusion, DESIGN.md section 3.5)."""
+    for f in (flow_fw, flow_bw):
+        if not isinstance(f, torch.Tensor) or not f.is_floating_point():
+            raise TypeError(f'fb_occlusion: flows must be floating-point torch tensors, got '
+                            f'{getattr(f, "dtype", type(f).__name__)}')
+    flow_fw = _flow_field(flow_fw, 'fb_occlusion')
+    flow_bw = _flow_field(flow_bw, 'fb_occlusion')
+    if flow_fw.shape != flow_bw.shape:
+        raise ValueError(f'fb_occlusion: flow_fw {tuple(flow_fw.shape)} and flow_bw {tuple(flow_bw.shape)} differ')
+    if flow_fw.device != flow_bw.device:
+        raise ValueError(f'fb_occlusion: flow_fw is on {flow_fw.device}, flow_bw on {flow_bw.device}')
+    a1, a2 = ctypes.c_float(alpha1).value, ctypes.c_float(alpha2).value          # the kernel's fp32 thresholds
+    if not (0.0 <= a1 < float('inf') and 0.0 <= a2 < float('inf')):
+        raise ValueError(f'fb_occlusion: alpha1 and alpha2 must be finite and >= 0 in fp32, got {alpha1}, {alpha2}')
+    # the kernel loads float2: a view starting at an odd float is copied to an aligned buffer
+    flow_fw, flow_bw = (f if f.data_ptr() % 8 == 0 else f.clone() for f in (flow_fw, flow_bw))
+    b, h, w, _ = flow_fw.shape
+    occ_fw = torch.empty((b, h, w), dtype=torch.bool, device=flow_fw.device)
+    occ_bw = torch.empty_like(occ_fw)
+    with torch.cuda.device(flow_fw.device):
+        _lib.check(_lib.lib().raft_b200_fb_occlusion(_lib.ptr(flow_fw), _lib.ptr(flow_bw), b, h, w, a1, a2,
+                                                     _lib.ptr(occ_fw), _lib.ptr(occ_bw), _lib.stream()), 'fb_occlusion')
+    return occ_fw, occ_bw
+
+
 def coords_init(flow_init):
     """coords_grid(B, h, w) + flow_init in fp32: the iteration loop's entry state for a warm start (B, h, w, 2)."""
     flow_init = _flow_field(flow_init, 'coords_init')

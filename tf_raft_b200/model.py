@@ -11,7 +11,7 @@ from collections import OrderedDict
 import torch
 
 from . import _lib
-from .layers.corr import CorrBlock, coords_grid, coords_init, forward_interpolate, upflow8
+from .layers.corr import CorrBlock, coords_grid, coords_init, fb_occlusion, forward_interpolate, upflow8
 from .layers.extractor import BasicEncoder, SmallEncoder
 from .layers.update import BasicUpdateBlock, SmallUpdateBlock
 from .losses import end_point_error, sequence_loss
@@ -133,7 +133,9 @@ class RAFT:
             flow_init = self._check_flow_init(flow_init, image1)
         self._sync_trained_params()
         if self.use_graph and not training:
-            return self._graph_call(image1, image2, last_only, flow_init)
+            key = (tuple(image1.shape), bool(last_only), flow_init is not None)
+            return self._graph_run(key, lambda a, b, f: self._forward(a, b, False, last_only, f),
+                                   (image1, image2, flow_init))
         return self._forward(image1, image2, training, last_only, flow_init)
 
     @staticmethod
@@ -150,33 +152,31 @@ class RAFT:
             raise ValueError(f'flow_init: expected {want} for {H}x{W} images, got {tuple(flow_init.shape)}')
         return flow_init.contiguous()
 
-    def _graph_call(self, image1, image2, last_only, flow_init=None):
-        warm = flow_init is not None
-        key = (tuple(image1.shape), bool(last_only), warm)
+    def _graph_run(self, key, fn, inputs):
+        """fn(*inputs) captured once per `key` into a CUDA graph over static copies of `inputs` (None entries stay
+        None), then replayed: each call copies its inputs into the static ones and returns the captured outputs."""
         entry = self._graphs.get(key)
         if entry is None:
-            s1, s2 = image1.clone(), image2.clone()
-            s3 = flow_init.clone() if warm else None
+            statics = [None if t is None else t.clone() for t in inputs]
             side = torch.cuda.Stream(device=self.device)
             side.wait_stream(torch.cuda.current_stream(self.device))
             with torch.cuda.stream(side):                      # warm-up: allocations, attributes, weight packing
                 for _ in range(2):
-                    self._forward(s1, s2, False, last_only, s3)
+                    fn(*statics)
             torch.cuda.current_stream(self.device).wait_stream(side)
             torch.cuda.synchronize(self.device)
             graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(graph):
-                outs = self._forward(s1, s2, False, last_only, s3)
+                outs = fn(*statics)
             # The captured kernels hold raw addresses of the encoder / update-block workspaces; those caches keep one
             # shape at a time, so the graph entry owns references to the buffers it was captured with.
             keep = [list(m._ws.values()) for m in (self.fnet, self.cnet, self.update_block)]
-            entry = (graph, s1, s2, s3, outs, self._last, keep)
+            entry = (graph, statics, outs, self._last, keep)
             self._graphs[key] = entry
-        graph, s1, s2, s3, outs, last, _keep = entry
-        s1.copy_(image1, non_blocking=True)
-        s2.copy_(image2, non_blocking=True)
-        if warm:
-            s3.copy_(flow_init, non_blocking=True)
+        graph, statics, outs, last, _keep = entry
+        for s, t in zip(statics, inputs):
+            if t is not None:
+                s.copy_(t, non_blocking=True)
         graph.replay()
         self._last = last
         return outs
@@ -210,7 +210,47 @@ class RAFT:
         self._last = dict(net=net, coords1=coords1, corr_block=corr_block)
         return [p for p in preds if p is not None] if last_only else preds
 
-    def predict_video(self, frames, *, warm_start=True):
+    def predict_bidirectional(self, inputs):
+        """Flow in both directions of B image pairs, with forward-backward occlusion masks (an addition: tf-raft
+        evaluates one direction).  inputs = [image1, image2], each (B, H, W, 3) float in 0..255 on the GPU.
+
+        Returns (flow_fw, flow_bw, occ_fw, occ_bw): the finest (B, H, W, 2) flows image1 -> image2 and image2 -> image1
+        after `iters_pred` iterations, what `predict_step` returns for [image1, image2] and for [image2, image1], and the
+        torch.bool (B, H, W) masks of `fb_occlusion(flow_fw, flow_bw)` at its default thresholds.  Each image is encoded
+        once by `fnet` and once by `cnet` (four image encodes where two calls make six), and both directions run as one
+        loop at batch 2B with fmap1 = [f1; f2], fmap2 = [f2; f1].  Every image's result is independent of the batch it
+        runs in, so on the native encoders (the f16x2 default) the flows equal the two single-direction calls bit for
+        bit; the cuDNN encoders of the fp32 configuration may pick another algorithm for the other batch and differ in
+        the last bits.  With `use_graph=True` the whole call, the occlusion check included, is captured once per input
+        shape (apart from `__call__`'s graphs) and replayed; the returned tensors are then static buffers that the next
+        call overwrites."""
+        image1, image2 = inputs
+        image1, image2 = _lib.f32c(image1), _lib.f32c(image2)
+        if image1.shape != image2.shape:
+            raise ValueError(f'image1 {tuple(image1.shape)} and image2 {tuple(image2.shape)} differ in shape')
+        if self.iters_pred < 1:
+            raise ValueError('predict_bidirectional needs iters_pred >= 1')
+        self._sync_trained_params()
+        if self.use_graph:
+            return self._graph_run(('bidirectional', tuple(image1.shape)), self._bidirectional, (image1, image2))
+        return self._bidirectional(image1, image2)
+
+    def _bidirectional(self, image1, image2):
+        bs, H, W, _ = image1.shape
+        self._check_size(H, W)
+        images = torch.cat([image1, image2])
+        fmap = self.fnet(images, training=False, raw_image=True)                    # [f1; f2]
+        net, inp = self._context(images, False)
+        return self._iterate_bidirectional(fmap, torch.cat([fmap[bs:], fmap[:bs]]), net, inp, bs, H, W, None)
+
+    def _iterate_bidirectional(self, fmap1, fmap2, net, inp, bs, H, W, flow_init):
+        """Both directions of B pairs as one loop at batch 2B (first half a -> b, second half b -> a), then the occlusion
+        check on the two halves of the finest prediction: (flow_fw, flow_bw, occ_fw, occ_bw)."""
+        flow = self._iterate(fmap1, fmap2, net, inp, 2 * bs, H, W, False, True, flow_init)[-1]
+        flow_fw, flow_bw = flow[:bs], flow[bs:]
+        return (flow_fw, flow_bw) + fb_occlusion(flow_fw, flow_bw)
+
+    def predict_video(self, frames, *, warm_start=True, bidirectional=False):
         """Flow along B video clips at once (an addition: tf-raft evaluates pairs only).
 
         `frames` is an iterable of (B, H, W, 3) CUDA tensors in 0..255, frame t of B independent clips.  A generator:
@@ -226,13 +266,24 @@ class RAFT:
         final low-resolution flow (coords1 - coords0), as RAFT does on Sintel and KITTI sequences; the first pair
         starts from zero flow.  `warm_start=False`: every pair starts from zero flow.
 
+        `bidirectional=True`: it yields (flow_fw, flow_bw, occ_fw, occ_bw) for the pair (t-1, t), what
+        `predict_bidirectional` returns for it.  `cnet` then runs once per frame too, and frame t's cached context
+        serves the backward direction of pair (t-1, t) and the forward direction of pair (t, t+1), copied into the
+        batch-2B loop (which writes it).  A step still costs two image encodes, fnet and cnet on frame t, and runs both
+        directions as one loop at batch 2B.  The warm start extends RAFT's, which covers the forward direction only:
+        the forward half starts from `forward_interpolate(F_low)` exactly as above, so the forward flows equal those of
+        `bidirectional=False` bit for bit; the backward half starts from `-forward_interpolate(-B_low)`, B_low being
+        the previous pair's backward low-resolution flow B_{t-1->t-2}.  Under constant velocity a point at x in frame
+        t-1 with backward flow b was at x + b in frame t-2 and will be at x - b in frame t, so B_{t->t-1}(x - b) = b:
+        splatting -b forward and negating the result gives it.  Both negations are exact.
+
         A frame whose shape differs from the first raises ValueError; fewer than two frames yield nothing.  Eager
         only: the video step is never captured into a CUDA graph, whatever `use_graph` says, and every yielded tensor
         is a new one."""
         self._sync_trained_params()
         if self.iters_pred < 1:
             raise ValueError('predict_video needs iters_pred >= 1')
-        shape = coords0 = frame_prev = fmap_prev = flow_init = None
+        shape = coords0 = frame_prev = fmap_prev = flow_init = ctx_prev = None
         for t, frame in enumerate(frames):
             frame = _lib.f32c(frame)
             if shape is None:
@@ -244,16 +295,31 @@ class RAFT:
             elif tuple(frame.shape) != shape:
                 raise ValueError(f'frame {t}: shape {tuple(frame.shape)} differs from the first frame {shape}')
             fmap = self.fnet(frame, training=False, raw_image=True)                    # model.py:74, frame t only
+            if bidirectional:
+                ctx = self._context(frame, False)                                      # :82-86, frame t only
             if frame_prev is not None:
-                net, inp = self._context(frame_prev, False)                                # :82-86
-                flow = self._iterate(fmap_prev, fmap, net, inp, bs, H, W, False, True, flow_init)[-1]
+                if bidirectional:
+                    net, inp = (torch.cat([p, c]) for p, c in zip(ctx_prev, ctx))     # copies: the loop writes net
+                    out = self._iterate_bidirectional(torch.cat([fmap_prev, fmap]), torch.cat([fmap, fmap_prev]), net,
+                                                      inp, bs, H, W, flow_init)
+                else:
+                    net, inp = self._context(frame_prev, False)                            # :82-86
+                    out = self._iterate(fmap_prev, fmap, net, inp, bs, H, W, False, True, flow_init)[-1]
                 if warm_start:
                     if coords0 is None:
-                        coords0 = coords_grid(bs, H // 8, W // 8, self.device)
+                        coords0 = coords_grid(2 * bs if bidirectional else bs, H // 8, W // 8, self.device)
                     # flow_low = coords1 - coords0 with flow_advance_kernel's fp32 subtraction
-                    flow_init = forward_interpolate(self._last['coords1'] - coords0)
-                yield flow
+                    if bidirectional:                           # [F_low; B_low] -> [fi(F_low); -fi(-B_low)], one launch
+                        flow_low = self._last['coords1'] - coords0
+                        flow_low[bs:].neg_()
+                        flow_init = forward_interpolate(flow_low)
+                        flow_init[bs:].neg_()
+                    else:
+                        flow_init = forward_interpolate(self._last['coords1'] - coords0)
+                yield out
             frame_prev, fmap_prev = frame, fmap
+            if bidirectional:
+                ctx_prev = ctx
 
     call = __call__
 
