@@ -140,6 +140,56 @@ int raft_b200_fb_occlusion(const float* flow_fw, const float* flow_bw, int B, in
                            uint8_t* occ_fw, uint8_t* occ_bw, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Training augmentation  (tf_raft/datasets/augmentor.py FlowAugmentor :9-129, SparseFlowAugmentor :132-267, given
+ * their random draws; dataset.py:102's dense valid)
+ * ------------------------------------------------------------------------------------------- */
+
+/* One sample.  Every pointer is device memory; sources and outputs are HWC and contiguous.  Per image k (0 = img1):
+ * lut[k][0] is albumentations' brightness/contrast LUT (identity when that transform is skipped); when hsv[k] is set
+ * the image then goes RGB->HSV (cv2, uint8), through lut[k][1..3] (hue, sat, val) and back (augmentor.py:42-59).
+ * rect[0..n_rects) = (x0, y0, dx, dy) eraser rectangles of img2 at source resolution, filled with the truncated mean of
+ * the colour-transformed img2 (:61-74).  spatial: cv2.resize by (scale_x, scale_y), INTER_LINEAR, to
+ * (rint(H*scale_y), rint(W*scale_x)), the flow then scaled in fp64 (:93-98); otherwise a copy.  Then h/v flips and the
+ * (crop_h, crop_w) window at (y0, x0) of the flipped image (:100-116).  ws_offset is filled by
+ * raft_b200_augment_workspace_bytes.                                                                                */
+typedef struct raft_augment_sample {
+  const uint8_t* img1;
+  const uint8_t* img2;          /* (H, W, 3)                                                                       */
+  const float* flow;            /* (H, W, 2)                                                                       */
+  const float* valid;           /* (H, W), sparse samples only (a source counts where valid >= 1)                 */
+  uint8_t* out_img1;
+  uint8_t* out_img2;            /* (crop_h, crop_w, 3)                                                             */
+  float* out_flow;              /* (crop_h, crop_w, 2)                                                             */
+  float* out_valid;             /* (crop_h, crop_w)                                                                */
+  double scale_x, scale_y;
+  size_t ws_offset;
+  int H, W, crop_h, crop_w, y0, x0;
+  int spatial, hflip, vflip;
+  int hsv[2];
+  int n_rects;
+  int rect[2][4];
+  uint8_t lut[2][4][256];
+} raft_augment_sample;
+
+/* Workspace of one raft_b200_augment_dense / _sparse call over samples[0..B) (host array); fills each sample's
+ * ws_offset.  RAFT_ERR_BAD_SHAPE if a crop does not fit the (resized) image or a size is out of range.               */
+int raft_b200_augment_workspace_bytes(raft_augment_sample* samples, int B, int sparse, size_t* bytes);
+
+/* FlowAugmentor.__call__ + dataset.py:102 for B samples of any source sizes in one launch set (3 kernels): out_flow is
+ * float32 of the fp64 flow, out_valid = |fx| < 1000 && |fy| < 1000 evaluated on the fp64 flow.  samples_host and
+ * samples_dev hold the same array (host copy for checks and grid sizes, device copy read by the kernels).
+ * Asynchronous on `stream`, no allocation: graph-capturable.                                                         */
+int raft_b200_augment_dense(const raft_augment_sample* samples_host, const raft_augment_sample* samples_dev, int B,
+                            void* workspace, size_t workspace_bytes, void* stream);
+
+/* SparseFlowAugmentor.__call__ likewise (4 kernels).  A spatial sample's flow goes through resize_sparse_flow_map
+ * (:183-215): source (x, y) with valid >= 1 lands at (rint(x*fx), rint(y*fy)) in fp64, half to even, kept iff
+ * 0 < xx < rw and 0 < yy < rh; the last source in index order wins a target; flow = float32(fp64 flow * scale), valid 1.
+ * A non-spatial sample copies flow and valid.                                                                        */
+int raft_b200_augment_sparse(const raft_augment_sample* samples_host, const raft_augment_sample* samples_dev, int B,
+                             void* workspace, size_t workspace_bytes, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Update blocks  (tf_raft/layers/update.py)
  * ------------------------------------------------------------------------------------------- */
 

@@ -7,6 +7,7 @@
 
 #include <algorithm>
 
+#include "augment.cuh"
 #include "corr_tc.cuh"
 #include "encoder.cuh"
 #include "train.cuh"
@@ -426,6 +427,74 @@ int raft_b200_fb_occlusion(const float* flow_fw, const float* flow_bw, int B, in
   return launch(fb_occlusion_kernel, grid_for(2 * (size_t)B * H * W), 256, 0, reinterpret_cast<cudaStream_t>(stream),
                 reinterpret_cast<const float2*>(flow_fw), reinterpret_cast<const float2*>(flow_bw), B, H, W, alpha1, alpha2,
                 occ_fw, occ_bw);
+}
+
+// Checks every sample of an augmentation call and lays out its workspace: fills (fill) or verifies each ws_offset.
+static int augment_layout(raft_augment_sample* samples, const raft_augment_sample* check, int B, int sparse,
+                          size_t* bytes, int* max_src, int* max_map, int* max_out) {
+  if ((!samples && !check) || !bytes || (sparse != 0 && sparse != 1)) return RAFT_ERR_BAD_ARG;
+  if (B < 1 || B > 65535) return RAFT_ERR_BAD_SHAPE;
+  size_t off = 0;
+  *max_src = *max_map = *max_out = 1;
+  for (int b = 0; b < B; ++b) {
+    const raft_augment_sample& s = check ? check[b] : samples[b];
+    if (!s.img1 || !s.img2 || !s.flow || !s.out_img1 || !s.out_img2 || !s.out_flow || !s.out_valid) return RAFT_ERR_BAD_ARG;
+    if ((sparse && !s.valid) || (sparse && s.vflip) || s.n_rects < 0 || s.n_rects > 2) return RAFT_ERR_BAD_ARG;
+    for (int r = 0; r < s.n_rects; ++r)
+      for (int k = 0; k < 4; ++k)
+        if (s.rect[r][k] < 0) return RAFT_ERR_BAD_ARG;
+    if (s.H < 1 || s.W < 1 || s.crop_h < 1 || s.crop_w < 1) return RAFT_ERR_BAD_SHAPE;
+    if ((size_t)s.H * s.W * 3 > (size_t)INT_MAX) return RAFT_ERR_BAD_SHAPE;
+    int rh = s.H, rw = s.W;
+    if (s.spatial) {
+      if (!(s.scale_x > 0.0 && s.scale_x <= 64.0 && s.scale_y > 0.0 && s.scale_y <= 64.0)) return RAFT_ERR_BAD_ARG;
+      rh = aug_resized(s.H, s.scale_y);
+      rw = aug_resized(s.W, s.scale_x);
+      if (rh < 1 || rw < 1 || (size_t)rh * rw > (size_t)INT_MAX) return RAFT_ERR_BAD_SHAPE;
+    }
+    if (s.y0 < 0 || s.x0 < 0 || s.y0 > rh - s.crop_h || s.x0 > rw - s.crop_w) return RAFT_ERR_BAD_SHAPE;
+    const bool map = sparse && s.spatial;
+    if (check ? s.ws_offset != off : false) return RAFT_ERR_BAD_ARG;
+    if (!check) samples[b].ws_offset = off;
+    off += aug_layout(s.H, s.W, rh, rw, map).total;
+    *max_src = std::max(*max_src, 2 * s.H * s.W);
+    if (map) *max_map = std::max(*max_map, rh * rw);
+    *max_out = std::max(*max_out, s.crop_h * s.crop_w);
+  }
+  *bytes = off;
+  return RAFT_OK;
+}
+
+int raft_b200_augment_workspace_bytes(raft_augment_sample* samples, int B, int sparse, size_t* bytes) {
+  int a, b, c;
+  return augment_layout(samples, nullptr, B, sparse, bytes, &a, &b, &c);
+}
+
+static int augment_run(const raft_augment_sample* host, const raft_augment_sample* dev, int B, int sparse, void* workspace,
+                       size_t workspace_bytes, void* stream) {
+  size_t need;
+  int max_src, max_map, max_out;
+  if (!host) return RAFT_ERR_BAD_ARG;
+  RAFT_TRY(augment_layout(nullptr, host, B, sparse, &need, &max_src, &max_map, &max_out));
+  if (!dev || !workspace || reinterpret_cast<uintptr_t>(workspace) % 256) return RAFT_ERR_BAD_ARG;
+  if (workspace_bytes < need) return RAFT_ERR_WORKSPACE;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
+  auto blocks = [](int n) { return (unsigned)std::min(ceil_div(n, kAugThreads), 4096); };
+  RAFT_TRY(launch(augment_init_kernel, dim3(blocks(max_map), B), kAugThreads, 0, st, dev, ws, sparse));
+  RAFT_TRY(launch(augment_colour_kernel, dim3(blocks(max_src), B), kAugThreads, 0, st, dev, ws));
+  if (sparse) RAFT_TRY(launch(augment_scatter_kernel, dim3(blocks(max_src / 2), B), kAugThreads, 0, st, dev, ws));
+  return launch(augment_gather_kernel, dim3(blocks(max_out), B), kAugThreads, 0, st, dev, ws, sparse);
+}
+
+int raft_b200_augment_dense(const raft_augment_sample* samples_host, const raft_augment_sample* samples_dev, int B,
+                            void* workspace, size_t workspace_bytes, void* stream) {
+  return augment_run(samples_host, samples_dev, B, 0, workspace, workspace_bytes, stream);
+}
+
+int raft_b200_augment_sparse(const raft_augment_sample* samples_host, const raft_augment_sample* samples_dev, int B,
+                             void* workspace, size_t workspace_bytes, void* stream) {
+  return augment_run(samples_host, samples_dev, B, 1, workspace, workspace_bytes, stream);
 }
 
 int raft_b200_update_prepared_bytes(int variant, int corr_channels, int precision, size_t* bytes) {
