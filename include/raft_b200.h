@@ -190,6 +190,38 @@ int raft_b200_augment_sparse(const raft_augment_sample* samples_host, const raft
                              void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Flow visualisation  (tf_raft/datasets/flow_viz.py: make_colorwheel :20-67, flow_uv_to_colors :70-106,
+ * flow_to_image :109-132)
+ * ------------------------------------------------------------------------------------------- */
+
+/* Per-image status bits of raft_b200_flow_to_image.                                                                 */
+enum {
+  RAFT_FLOWVIZ_INF = 1,          /* a component is +-inf (after the clip)                                            */
+  RAFT_FLOWVIZ_NAN = 2,          /* a component is NaN (after the clip)                                              */
+  RAFT_FLOWVIZ_BAD_RAD_MAX = 4   /* the caller's rad_max of this image is negative or not finite                    */
+};
+
+/* The Middlebury colour wheel of B flow fields of H x W pixels -> image (B, H, W, 3) uint8, RGB (BGR when bgr != 0).
+ * Component k of pixel p (flat over B*H*W) is u[p*stride], v[p*stride]: stride 2 with v = u + 1 reads (B, H, W, 2)
+ * flows, stride 1 reads separate (B, H, W) planes.  Per pixel, NumPy 2 dtypes (NEP 50):
+ *   clip != 0: u, v = np.clip(., 0, clip_flow) in float32 (NaN propagates, -0.0 stays -0.0)            (:123-124)
+ *   normalize != 0: u, v /= rad_max[b] + float32(1e-5), float32; rad_max[b] is the caller's (rad_max != NULL) or
+ *     max over image b of sqrt(u*u + v*v) (float32, each operation rounded, no FMA)                      (:127-131)
+ *   rad = sqrt(u*u + v*v); a = float32(atan2((double)-v, (double)-u)) / float32(pi) (correctly rounded atan2);
+ *   fk = (a + 1) / 2 * 54, k0 = floor(fk), k1 = k0 + 1 wrapping 55 to 0 (float32); f = fk - k0 in float64;
+ *   col = (1 - f) * cw[k0] / 255 + f * cw[k1] / 255, then 1 - rad * (1 - col) if rad <= 1 else col * 0.75, and
+ *   floor(255 * col), all float64                                                                          (:85-106)
+ * status[b] (int) collects RAFT_FLOWVIZ_* bits of image b; the reference raises for NaN, and flow_to_image for +-inf
+ * too (an infinite rad_max makes u / rad_max NaN).  A pixel whose angle is NaN is written (0, 0, 0).  work (B
+ * unsigned words) holds the reduction; it is needed only when normalize != 0 and rad_max == NULL.  The call zeroes
+ * work and status on `stream` first.  image must be 4-byte aligned.  RAFT_ERR_BAD_ARG for a null pointer, stride not
+ * 1 or 2, or clip != 0 with a negative or non-finite clip_flow; RAFT_ERR_BAD_SHAPE unless 1 <= B <= 65535, H, W >= 1
+ * and H*W < 2^31.  Two kernels (one without the reduction), asynchronous, no allocation: graph-capturable.           */
+int raft_b200_flow_to_image(const float* u, const float* v, int stride, int B, int H, int W, int clip, float clip_flow,
+                            int normalize, const float* rad_max, int bgr, uint8_t* image, unsigned int* work,
+                            int* status, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Update blocks  (tf_raft/layers/update.py)
  * ------------------------------------------------------------------------------------------- */
 

@@ -13,7 +13,7 @@ from .losses import EndPointError, end_point_error, sequence_loss
 from .model import RAFT, SmallRAFT
 from .checkpoint import load_tf_checkpoint, read_tf_checkpoint, write_tf_checkpoint
 from .preprocess import CropOrPadder, pad_to_multiple, resize_with_crop_or_pad
-from .train import AdamW, CyclicalLearningRate, first_cycle_scaler, inverse_scaler
+from .train import AdamW, CyclicalLearningRate, VisFlowCallback, first_cycle_scaler, inverse_scaler
 from . import datasets
 
 __all__ = ['CorrBlock', 'bilinear_sampler', 'coords_grid', 'fb_occlusion', 'forward_interpolate', 'tfa_sampler', 'upflow8',

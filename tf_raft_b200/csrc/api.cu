@@ -10,6 +10,7 @@
 #include "augment.cuh"
 #include "corr_tc.cuh"
 #include "encoder.cuh"
+#include "flow_viz.cuh"
 #include "train.cuh"
 #include "video.cuh"
 
@@ -495,6 +496,30 @@ int raft_b200_augment_dense(const raft_augment_sample* samples_host, const raft_
 int raft_b200_augment_sparse(const raft_augment_sample* samples_host, const raft_augment_sample* samples_dev, int B,
                              void* workspace, size_t workspace_bytes, void* stream) {
   return augment_run(samples_host, samples_dev, B, 1, workspace, workspace_bytes, stream);
+}
+
+int raft_b200_flow_to_image(const float* u, const float* v, int stride, int B, int H, int W, int clip, float clip_flow,
+                            int normalize, const float* rad_max, int bgr, uint8_t* image, unsigned int* work,
+                            int* status, void* stream) {
+  const bool reduce = normalize && !rad_max;
+  if (!u || !v || !image || !status || (reduce && !work) || (stride != 1 && stride != 2)) return RAFT_ERR_BAD_ARG;
+  if (clip && !(clip_flow >= 0.0f && clip_flow <= FLT_MAX)) return RAFT_ERR_BAD_ARG;
+  if (reinterpret_cast<uintptr_t>(image) % 4) return RAFT_ERR_BAD_ARG;
+  if (B < 1 || B > 65535 || H < 1 || W < 1 || (size_t)H * W > (size_t)INT_MAX) return RAFT_ERR_BAD_SHAPE;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const int hw = H * W;
+  RAFT_CUDA_TRY(cudaMemsetAsync(status, 0, (size_t)B * sizeof(int), st));
+  if (reduce) {
+    RAFT_CUDA_TRY(cudaMemsetAsync(work, 0, (size_t)B * sizeof(unsigned), st));
+    const unsigned gx = (unsigned)std::min(ceil_div(hw, kVizThreads * 8), std::max(1, kNumSMs * 8 / B));
+    RAFT_TRY(launch(flow_radmax_kernel, dim3(gx, B), kVizThreads, 0, st, u, v, stride, hw, clip, clip_flow, work));
+  }
+  VizParams p;
+  p.u = u; p.v = v; p.stride = stride; p.hw = hw; p.npix = (size_t)B * hw;
+  p.clip = clip != 0; p.clip_flow = clip_flow; p.normalize = normalize != 0; p.rad_max = rad_max; p.work = work;
+  p.bgr = bgr != 0; p.out = image; p.status = status;
+  const size_t nblk = (p.npix + kVizPixPerBlock - 1) / kVizPixPerBlock;
+  return launch(flow_colour_kernel, dim3((unsigned)nblk), kVizThreads, 0, st, p);
 }
 
 int raft_b200_update_prepared_bytes(int variant, int corr_channels, int precision, size_t* bytes) {

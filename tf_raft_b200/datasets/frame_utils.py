@@ -3,6 +3,7 @@ evaluation scripts feed `RAFT.test_step` with what these return).
 
 .flo (Middlebury): float32 tag 202021.25, int32 width, int32 height, then height x width x (u, v) float32, little endian.
 KITTI flow PNG: 16-bit RGB, u = (R - 2^15) / 64, v = (G - 2^15) / 64, B = valid flag.
+`write_png` writes the 8- and 16-bit RGB PNGs (KITTI flows, VisFlowCallback's pictures) without an image library.
 """
 import struct
 import zlib
@@ -102,13 +103,23 @@ def write_flow_kitti(path, flow, valid=None):
     flow = np.asarray(flow, dtype=np.float32)
     h, w, _ = flow.shape
     valid = np.ones((h, w), np.float32) if valid is None else np.asarray(valid, np.float32)
-    rgb = np.concatenate([64.0 * flow + 2 ** 15, valid[..., None]], axis=-1).astype(np.uint16)
-    be = rgb.astype('>u2').tobytes()
-    stride = 6 * w
+    write_png(path, np.concatenate([64.0 * flow + 2 ** 15, valid[..., None]], axis=-1).astype(np.uint16))
+
+
+def write_png(path, image):
+    """Non-interlaced RGB PNG of an (H, W, 3) uint8 (8-bit) or uint16 (16-bit) array: filter type 0 rows, one zlib
+    IDAT chunk.  No image library needed."""
+    image = np.asarray(image)
+    if image.ndim != 3 or image.shape[2] != 3 or image.dtype not in (np.uint8, np.uint16):
+        raise ValueError(f'write_png: expected an (H, W, 3) uint8 or uint16 array, got {image.shape} {image.dtype}')
+    h, w, _ = image.shape
+    depth = 8 * image.dtype.itemsize
+    be = image.astype('>u2' if depth == 16 else np.uint8).tobytes()
+    stride = 3 * image.dtype.itemsize * w
     rows = b''.join(b'\x00' + be[y * stride:(y + 1) * stride] for y in range(h))
 
     def chunk(kind, body):
         return struct.pack('>I', len(body)) + kind + body + struct.pack('>I', zlib.crc32(kind + body) & 0xffffffff)
     with open(path, 'wb') as f:
-        f.write(b'\x89PNG\r\n\x1a\n' + chunk(b'IHDR', struct.pack('>IIBBBBB', w, h, 16, 2, 0, 0, 0)) +
+        f.write(b'\x89PNG\r\n\x1a\n' + chunk(b'IHDR', struct.pack('>IIBBBBB', w, h, depth, 2, 0, 0, 0)) +
                 chunk(b'IDAT', zlib.compress(rows)) + chunk(b'IEND', b''))

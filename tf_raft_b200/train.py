@@ -17,15 +17,20 @@ What runs where (DESIGN.md "Training"):
   hand-written tensor-core kernels are forward-only.
 """
 import math
+import os
 
+import numpy as np
 import torch
 import torch.distributed as dist
 import torch.nn.functional as F
 
 from . import _lib
+from .datasets.flow_viz import flow_to_image
+from .datasets.frame_utils import write_png
 from .layers.corr import CorrBlock
 from .layers.extractor import _same_pads, force_ieee_fp32
 from .losses import end_point_error, sequence_loss
+from .preprocess import resize_with_crop_or_pad
 
 force_ieee_fp32()
 
@@ -39,6 +44,55 @@ def first_cycle_scaler(cycle):
 def inverse_scaler(cycle):
     """tf_raft/training.py:18-23."""
     return 1.0 / cycle
+
+
+class VisFlowCallback:
+    """tf_raft/training.py:26-88: at the end of each epoch, writes the model's prediction on a few dataset items as
+    PNGs: image1, image2 and the flow colour wheel stacked vertically, `epoch{e+1:03d}_{i+1:03d}.png` in `logdir`.
+
+    dataset: a sequence whose items begin with (image1, image2), each H x W x 3 in 0..255 (NumPy arrays or tensors);
+    an item with a batch axis raises ValueError.  Item ids are range(num_visualize), or with choose_random
+    `np.random.choice(len(dataset), size=num_visualize, replace=False)`, the reference's call on the global NumPy
+    generator, so a seeded run picks the reference's ids.  Each pair is crop-or-padded to target_size
+    (`resize_with_crop_or_pad`), the model's final prediction (`last_only=True`) is cropped back to H x W and coloured
+    on the GPU by `flow_to_image`.  The images are written as uint8: values are clipped to 0..255 and truncated."""
+
+    def __init__(self, dataset, target_size=(448, 1024), num_visualize=1, choose_random=False,
+                 logdir='predicted_flows'):
+        self.dataset = dataset
+        self.target_size = tuple(target_size)
+        self.num_visualize = num_visualize
+        self.choose_random = choose_random
+        self.logdir = logdir
+        self.model = None
+        os.makedirs(logdir, exist_ok=True)
+
+    def set_model(self, model):
+        self.model = model
+
+    @staticmethod
+    def _uint8(image):
+        image = image.detach().cpu().numpy() if isinstance(image, torch.Tensor) else np.asarray(image)
+        return image if image.dtype == np.uint8 else np.clip(image, 0, 255).astype(np.uint8)
+
+    def on_epoch_end(self, epoch, logs=None):
+        if self.choose_random:
+            vis_ids = np.random.choice(len(self.dataset), size=self.num_visualize, replace=False)
+        else:
+            vis_ids = range(self.num_visualize)
+        device = self.model.device
+        for i in vis_ids:
+            image1, image2, *_ = self.dataset[i]
+            if len(image1.shape) > 3:
+                raise ValueError('target dataset must not be batched')
+            h, w, _ = image1.shape
+            pair = [resize_with_crop_or_pad(torch.as_tensor(np.asarray(im) if not isinstance(im, torch.Tensor) else im,
+                                                            dtype=torch.float32, device=device), *self.target_size)[None]
+                    for im in (image1, image2)]
+            flow = self.model(pair, training=False, last_only=True)[-1][0]
+            flow_img = flow_to_image(resize_with_crop_or_pad(flow, h, w)).cpu().numpy()
+            contents = np.concatenate([self._uint8(image1), self._uint8(image2), flow_img], axis=0)
+            write_png(os.path.join(self.logdir, f'epoch{epoch + 1:03d}_{i + 1:03d}.png'), contents)
 
 
 class CyclicalLearningRate:
