@@ -182,10 +182,70 @@ def corr_rows(f1, f2, qs, levels):
     return [p.permute(0, 2, 3, 1) for p in out]
 
 
+ENCODER_STAGES = {'raft': (64, ((64, 1), (96, 2), (128, 2))), 'small': (32, ((32, 1), (64, 2), (96, 2)))}
+
+
+def encoder_plan(H, W, variant):
+    """The tensor-core convolutions encoder_forward (tf_raft_b200/csrc/encoder.cuh) launches for an H x W image, in order:
+    a Python mirror of its layer sequence and of enc_conv_tc's choices.  Each entry is a dict with the layer name, the
+    kernel size k, the TMA element stride, the input (hin, win) and output (hout, wout) sizes, the pixel tile (tw, th)
+    and the 'same' pads before (pt, pl).  The stem's 7 x 7 stride-2 window is gathered by stem_im2col_kernel into planes
+    of the output's size, so the stem runs as a 1 x 1 stride-1 convolution; 1 x 1 convolutions are 'valid'.  Stride-2
+    layers on an odd input pad one row / column on both sides, on an even input only after (TF 'same')."""
+    c0, stages = ENCODER_STAGES[variant]
+    h, w = -(-H // 2), -(-W // 2)
+    plan = []
+
+    def conv(name, k, stride, hin, win):
+        hout, wout = -(-hin // stride), -(-win // stride)
+        tw, th = tc_tile(hout, wout)
+        # enc_conv_tc narrows a tile whose strided TMA box would pass 256 elements; tc_tile's widest tile is 128, so at
+        # stride 2 the box is at most 256 wide and the rule never fires
+        assert tw * stride <= 256 and th * stride <= 256
+        if k == 1 or stride == 1:
+            pt = pl = (k - 1) // 2
+        else:
+            pt = max((hout - 1) * stride + k - hin, 0) // 2
+            pl = max((wout - 1) * stride + k - win, 0) // 2
+        plan.append(dict(name=name, k=k, stride=stride, hin=hin, win=win, hout=hout, wout=wout, tw=tw, th=th,
+                         pt=pt, pl=pl))
+        return hout, wout
+
+    conv('stem', 1, 1, h, w)
+    for li, (c, s) in enumerate(stages, start=1):
+        for bi, st in enumerate((s, 1)):
+            p = f'layer{li}.{bi}'
+            ho, wo = conv(p + '.conv1', 3, st, h, w)
+            if st != 1:
+                conv(p + '.downsample', 1, st, h, w)
+            conv(p + '.conv2', 3, 1, ho, wo)
+            h, w = ho, wo
+    conv('conv2', 1, 1, h, w)
+    return plan
+
+
+def stride2_combos(H, W, variant, min_tiles=2):
+    """(tw, th, odd input height, odd input width) of the stride-2 convolutions of encoder_plan(H, W, variant) whose
+    output spans at least min_tiles pixel tiles in both directions."""
+    return {(e['tw'], e['th'], e['hin'] % 2, e['win'] % 2) for e in encoder_plan(H, W, variant)
+            if e['stride'] == 2 and -(-e['wout'] // e['tw']) >= min_tiles and -(-e['hout'] // e['th']) >= min_tiles}
+
+
+# (H, W) images for the encoder geometry sweep (tests/test_gpu_encoders.py).  The first ten, a greedy cover found with
+# encoder_plan over H in 8..400 and W in 8..1300, put a stride-2 layer on every (pixel tile, input-height parity,
+# input-width parity) with the layer's output at least two tiles each way, for both encoders.  The last three are the
+# smallest images: at 8 x 8 the last stage is 1 x 1, so instance norm sees one pixel and a zero variance.
+ENCODER_GRIDS = (
+    (17, 1283), (195, 129), (195, 135), (23, 1283), (97, 321), (49, 645), (99, 325), (103, 323), (35, 1029),
+    (87, 1287),
+    (8, 8), (8, 9), (9, 8),
+)
+
+
 def encoder_params(variant, norm_type, out_dim, seed=99, bias_scale=0.05, norm_jitter=0.2):
     """Parameters of a BasicEncoder ('raft') / SmallEncoder ('small') with any norm type, under the prefix 'enc.'."""
     from oracle import weights
-    c0, stages = (64, ((64, 1), (96, 2), (128, 2))) if variant == 'raft' else (32, ((32, 1), (64, 2), (96, 2)))
+    c0, stages = ENCODER_STAGES[variant]
     return weights.draw_params(weights.encoder_shapes('enc', norm_type, c0, stages, out_dim), seed, bias_scale, norm_jitter)
 
 

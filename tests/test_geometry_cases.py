@@ -100,6 +100,43 @@ def test_encoder_params_fit_both_encoders_and_every_norm():
     assert list(p) == list(q) and all(np.array_equal(p[k], q[k]) for k in p)
 
 
+def test_encoder_plan_known_answers():
+    """encoder_plan at the benchmark's 448 x 512: the stem and stage 1 on 224 x 256, stage 2 on 112 x 128 (the 128 x 1
+    tile, whose stride-2 box is 256 elements wide), stage 3 on 56 x 64; even inputs pad the stride-2 3 x 3 convolutions
+    after only."""
+    plan = {e['name']: e for e in cases.encoder_plan(448, 512, 'raft')}
+    assert len(plan) == 1 + 6 * 2 + 2 + 1
+    assert [(e['hout'], e['wout'], e['tw'], e['th']) for e in (plan['stem'], plan['layer2.0.conv1'], plan['conv2'])] == \
+        [(224, 256, 128, 1), (112, 128, 128, 1), (56, 64, 64, 2)]
+    s2 = plan['layer2.0.conv1']
+    assert (s2['stride'], s2['hin'], s2['win'], s2['pt'], s2['pl']) == (2, 224, 256, 0, 0)
+    assert s2['tw'] * s2['stride'] == 256
+    odd = {e['name']: e for e in cases.encoder_plan(70, 98, 'small')}['layer3.0.conv1']      # 18 x 25 -> 9 x 13
+    assert (odd['hin'], odd['win'], odd['hout'], odd['wout'], odd['pt'], odd['pl']) == (18, 25, 9, 13, 0, 1)
+    assert all(e['pt'] == e['pl'] == 0 for e in cases.encoder_plan(71, 99, 'raft') if e['k'] == 1)
+
+
+def test_encoder_grids_reach_every_stride2_tile_and_parity():
+    """Over every image with H in 8..400 and W in 8..1300, the stride-2 convolutions of the encoders reach 20
+    combinations of (pixel tile, odd input height, odd input width) with an output of at least two tiles each way:
+    five tiles times four parities.  ENCODER_GRIDS reaches all of them, and holds the smallest images.  The plan depends
+    on the image only through the stem's output size, so one image per stem size is enumerated."""
+    reach = {}
+    for H in range(8, 401):
+        for W in range(8, 1301):
+            key = (-(-H // 2), -(-W // 2))
+            if key not in reach:
+                reach[key] = cases.stride2_combos(H, W, 'raft')
+    universe = set().union(*reach.values())
+    assert universe == {(tw, 128 // tw, oh, ow) for tw in (128, 64, 32, 16, 8) for oh in (0, 1) for ow in (0, 1)}
+    for variant in ('raft', 'small'):
+        got = set().union(*(cases.stride2_combos(H, W, variant) for H, W in cases.ENCODER_GRIDS))
+        assert got == universe, sorted(universe - got)
+    assert {(8, 8), (8, 9), (9, 8)} <= set(cases.ENCODER_GRIDS)
+    last = cases.encoder_plan(8, 8, 'raft')[-1]
+    assert (last['hin'], last['win']) == (1, 1)                      # stage 3 is one pixel: zero instance-norm variance
+
+
 def test_fp64_encoder_output_shape_on_odd_sizes():
     """rt.encoder pads the stride-2 stages the TensorFlow way: the output is ceil(H / 8) x ceil(W / 8)."""
     p = cases.encoder_params('small', 'instance', 128)

@@ -39,7 +39,9 @@ def T():
 
 
 def test_encoders_are_fp32_grade(T, oracle_run):
-    """The cuDNN encoders must run in IEEE fp32 (PyTorch defaults to TF32 for convolutions)."""
+    """RAFT's encoders as the model runs them under the default precision (f16x2: the native tensor-core encoders)
+    against the fp32 oracle at 448x512, one pair, with zero biases and unit norm parameters.  tests/test_gpu_encoders.py
+    compares the native encoders with the fp64 oracle at every stride-2 geometry and at the production batches."""
     p, im1, im2, _, inter = oracle_run
     model = T.RAFT(iters=ITERS, iters_pred=ITERS)
     model.load_params(p)

@@ -526,10 +526,14 @@ __global__ void pack_weights_kernel(const PackParams p) {
 // Normalisation layers of the encoders (extractor.py:6-16): tfa InstanceNormalization (statistics per
 // image) / Keras BatchNormalization in training mode (statistics over the batch), eps = 1e-3.
 // y is the raw convolution output (G groups x P pixels x C channels, fp32).  ONE pass over y:
-// every thread accumulates shifted sums of its pixels (shift = its first sample, so there is no
-// E[x^2]-E[x]^2 cancellation), partial (n, mean, M2) triples are merged with Chan's formula in a fixed
-// order (deterministic).   part[g][split][{n, mean, M2}][c]
+// every thread starts from its first sample (n = 1, M2 = 0) and folds in the rest in blocks of
+// kNormBlock, each block as sums shifted by the running mean (Welford's update, one block at a time).
+// A sum shifted by a fixed sample would cancel catastrophically when that sample is far from the mean,
+// e.g. one bright pixel: with the running mean as shift, s2 - s1^2/n loses at most a factor
+// (kNormBlock + 1) to cancellation, on the first block only.  Partial (n, mean, M2) triples are merged
+// with Chan's formula in a fixed order (deterministic).   part[g][split][{n, mean, M2}][c]
 // ------------------------------------------------------------------------------------------------
+constexpr int kNormBlock = 8;
 __device__ __forceinline__ void chan_merge(float& na, float& ma, float& m2a, float nb, float mb, float m2b) {
   if (nb == 0.f) return;
   const float n = na + nb, d = mb - ma;
@@ -548,16 +552,24 @@ __global__ void __launch_bounds__(256) norm_stats_kernel(const float* __restrict
   float n = 0.f, mean = 0.f, m2 = 0.f;
   if (pl < lanes && p0 + pl < p1) {
     const float* base = y + ((size_t)g * P) * C + c;
-    const float K = base[(size_t)(p0 + pl) * C];
-    float s1 = 0.f, s2 = 0.f;
-    for (int px = p0 + pl; px < p1; px += lanes) {
-      const float v = base[(size_t)px * C] - K;
-      s1 += v;
-      s2 += v * v;
-      n += 1.f;
+    mean = base[(size_t)(p0 + pl) * C];
+    n = 1.f;
+    for (int px = p0 + pl + lanes; px < p1;) {
+      // with the block's sums s1, s2 of (v - mean) and n' = n + nb:  mean' = mean + s1 / n',  M2' = M2 + s2 - s1^2 / n'
+      float s1 = 0.f, s2 = 0.f;
+#pragma unroll
+      for (int k = 0; k < kNormBlock; ++k, px += lanes) {
+        if (px < p1) {
+          const float v = base[(size_t)px * C] - mean;
+          s1 += v;
+          s2 += v * v;
+          n += 1.f;
+        }
+      }
+      const float r = s1 / n;
+      mean += r;
+      m2 += relu_nan(s2 - s1 * r);                     // a NaN sample keeps the variance NaN, not 0
     }
-    mean = K + s1 / n;
-    m2 = relu_nan(s2 - s1 * s1 / n);                   // a NaN sample keeps the variance NaN, not 0
   }
   red[0][threadIdx.x] = n; red[1][threadIdx.x] = mean; red[2][threadIdx.x] = m2;
   __syncthreads();
