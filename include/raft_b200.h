@@ -222,6 +222,56 @@ int raft_b200_flow_to_image(const float* u, const float* v, int stride, int B, i
                             int* status, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Evaluation data  (tf_raft/datasets/frame_utils.py:102-107 readFlowKITTI; tf_raft/losses/losses.py:24-43
+ * end_point_error, with the KITTI outlier rule of RAFT's evaluate.py)
+ * ------------------------------------------------------------------------------------------- */
+
+/* One 16-bit RGB, non-interlaced PNG (a KITTI / HD1K flow map) after zlib inflation: h rows of 1 filter byte + 6 * w
+ * bytes start at data + offset.  flow (h, w, 2) float32, 8-byte aligned; valid (h, w) float32.  Device pointers.     */
+typedef struct raft_png16_image {
+  size_t offset;
+  int h, w;
+  float* flow;
+  float* valid;
+} raft_png16_image;
+
+/* Decodes n such images in one launch, one CTA per image, rows in order: PNG filters 0-4 undone per byte lane (bpp 6),
+ * then flow = (RGB16 - 2^15) / 64 and valid = B16, exactly readFlowKITTI's float32 values.  status[i] (int, device) is
+ * 0, or 1 + the first row of image i whose filter byte is not 0-4 (decoding of that image stops there).  The call
+ * zeroes status on `stream` first.  images_host and images_dev hold the same array (host copy for checks and the grid,
+ * device copy read by the kernel).  RAFT_ERR_BAD_ARG for a null pointer or a misaligned flow; RAFT_ERR_BAD_SHAPE
+ * unless 1 <= n <= 2^31 - 1, 1 <= h, 1 <= w <= 16384, h * w < 2^31 and every image's rows lie inside data_bytes.
+ * Asynchronous, no allocation: graph-capturable.                                                                     */
+int raft_b200_png16_flow_decode(const uint8_t* data, size_t data_bytes, const raft_png16_image* images_host,
+                                const raft_png16_image* images_dev, int n, int* status, void* stream);
+
+/* Per-image record of raft_b200_flow_metrics: counts[b][k] over the pixels of image b that the mask keeps.             */
+enum {
+  RAFT_METRIC_N = 0,             /* pixels kept                                                                        */
+  RAFT_METRIC_LT1 = 1,           /* epe < 1                                                                            */
+  RAFT_METRIC_LT3 = 2,           /* epe < 3                                                                            */
+  RAFT_METRIC_LT5 = 3,           /* epe < 5                                                                            */
+  RAFT_METRIC_OUTLIER = 4,       /* epe > 3 and epe / mag > float32(0.05)                                              */
+  RAFT_METRIC_COUNTS = 5
+};
+
+/* Workspace of raft_b200_flow_metrics for B images of H x W pixels.                                                 */
+int raft_b200_flow_metrics_workspace_bytes(int B, int H, int W, size_t* bytes);
+
+/* End-point-error records of B flow pairs.  pred, gt (B, H, W, 2) float32, 8-byte aligned; valid (B, H, W) float32 or
+ * NULL (every pixel valid).  Per pixel, float32 with every operation rounded and none fused:
+ *   mag = sqrt(g0*g0 + g1*g1); kept = valid != 0 (NaN counts as nonzero) && (!use_max_flow || mag < max_flow);
+ *   epe = sqrt(d0*d0 + d1*d1), d = pred - gt; outlier = epe > 3 && epe / mag > float32(0.05).
+ * counts (B, RAFT_METRIC_COUNTS) int64 and sums (B) float64 (the sum of epe over kept pixels; a NaN epe enters it and
+ * fails every comparison).  The reduction has a fixed order that depends on H * W only: runs are bit-identical and an
+ * image's record does not depend on the rest of the batch.  RAFT_ERR_BAD_ARG for a null or misaligned pointer;
+ * RAFT_ERR_BAD_SHAPE unless 1 <= B <= 65535, H, W >= 1 and H * W < 2^31; RAFT_ERR_WORKSPACE if workspace_bytes is
+ * below raft_b200_flow_metrics_workspace_bytes.  Two kernels, asynchronous, no allocation: graph-capturable.          */
+int raft_b200_flow_metrics(const float* pred, const float* gt, const float* valid, int B, int H, int W, int use_max_flow,
+                           float max_flow, void* workspace, size_t workspace_bytes, long long* counts, double* sums,
+                           void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Update blocks  (tf_raft/layers/update.py)
  * ------------------------------------------------------------------------------------------- */
 

@@ -83,7 +83,10 @@ _SIGNATURES = {
     'raft_b200_augment_dense': (_i, [_vp, _vp, _i, _vp, _sz, _vp]),
     'raft_b200_augment_sparse': (_i, [_vp, _vp, _i, _vp, _sz, _vp]),
     'raft_b200_flow_to_image': (_i, [_vp, _vp, _i, _i, _i, _i, _i, ctypes.c_float, _i, _vp, _i, _vp, _vp, _vp, _vp]),
-    'raft_b200_update_prepared_bytes': (_i, [_i, _i, _i, ctypes.POINTER(_sz)]),
+    'raft_b200_png16_flow_decode': (_i, [_vp, _sz, _vp, _vp, _i, _vp, _vp]),
+    'raft_b200_flow_metrics_workspace_bytes': (_i, [_i, _i, _i, ctypes.POINTER(_sz)]),
+    'raft_b200_flow_metrics': (_i, [_vp, _vp, _vp, _i, _i, _i, _i, ctypes.c_float, _vp, _sz, _vp, _vp, _vp]),
+    'raft_b200_update_prepared_bytes':(_i, [_i, _i, _i, ctypes.POINTER(_sz)]),
     'raft_b200_update_prepare': (_i, [_i, _vp, _vp, _sz, _i, _vp]),
     'raft_b200_update_workspace_bytes': (_i, [_i, _i, _i, _i, _i, ctypes.POINTER(_sz)]),
     'raft_b200_update_basic': (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _sz, _i, _vp]),

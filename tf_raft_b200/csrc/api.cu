@@ -9,6 +9,7 @@
 
 #include "augment.cuh"
 #include "corr_tc.cuh"
+#include "dataset.cuh"
 #include "encoder.cuh"
 #include "flow_viz.cuh"
 #include "train.cuh"
@@ -520,6 +521,55 @@ int raft_b200_flow_to_image(const float* u, const float* v, int stride, int B, i
   p.bgr = bgr != 0; p.out = image; p.status = status;
   const size_t nblk = (p.npix + kVizPixPerBlock - 1) / kVizPixPerBlock;
   return launch(flow_colour_kernel, dim3((unsigned)nblk), kVizThreads, 0, st, p);
+}
+
+int raft_b200_png16_flow_decode(const uint8_t* data, size_t data_bytes, const raft_png16_image* images_host,
+                                const raft_png16_image* images_dev, int n, int* status, void* stream) {
+  if (!data || !images_host || !images_dev || !status) return RAFT_ERR_BAD_ARG;
+  if (n < 1) return RAFT_ERR_BAD_SHAPE;
+  int max_w = 1;
+  for (int i = 0; i < n; ++i) {
+    const raft_png16_image& im = images_host[i];
+    if (!im.flow || !im.valid || reinterpret_cast<uintptr_t>(im.flow) % sizeof(float2)) return RAFT_ERR_BAD_ARG;
+    if (im.h < 1 || im.w < 1 || im.w > kPngMaxWidth || (size_t)im.h * im.w > (size_t)INT_MAX) return RAFT_ERR_BAD_SHAPE;
+    const size_t rows = (size_t)im.h * (1 + 6 * (size_t)im.w);
+    if (im.offset > data_bytes || rows > data_bytes - im.offset) return RAFT_ERR_BAD_SHAPE;
+    max_w = std::max(max_w, im.w);
+  }
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  PngParams p;
+  p.data = data; p.images = images_dev; p.status = status; p.row_bytes = round_up(6 * max_w, 16);
+  const size_t smem = 2 * (size_t)p.row_bytes;
+  RAFT_CUDA_TRY(cudaFuncSetAttribute(png16_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  RAFT_CUDA_TRY(cudaMemsetAsync(status, 0, (size_t)n * sizeof(int), st));
+  return launch(png16_decode_kernel, dim3((unsigned)n), kPngThreads, smem, st, p);
+}
+
+int raft_b200_flow_metrics_workspace_bytes(int B, int H, int W, size_t* bytes) {
+  if (!bytes) return RAFT_ERR_BAD_ARG;
+  if (B < 1 || B > 65535 || H < 1 || W < 1 || (size_t)H * W > (size_t)INT_MAX - kMetChunk) return RAFT_ERR_BAD_SHAPE;
+  *bytes = (size_t)B * ceil_div(H * W, kMetChunk) * sizeof(MetricPartial);
+  return RAFT_OK;
+}
+
+int raft_b200_flow_metrics(const float* pred, const float* gt, const float* valid, int B, int H, int W, int use_max_flow,
+                           float max_flow, void* workspace, size_t workspace_bytes, long long* counts, double* sums,
+                           void* stream) {
+  if (!pred || !gt || !workspace || !counts || !sums) return RAFT_ERR_BAD_ARG;
+  if ((reinterpret_cast<uintptr_t>(pred) | reinterpret_cast<uintptr_t>(gt)) % sizeof(float2) ||
+      reinterpret_cast<uintptr_t>(workspace) % alignof(MetricPartial) || reinterpret_cast<uintptr_t>(counts) % 8 ||
+      reinterpret_cast<uintptr_t>(sums) % 8)
+    return RAFT_ERR_BAD_ARG;
+  size_t need;
+  RAFT_TRY(raft_b200_flow_metrics_workspace_bytes(B, H, W, &need));
+  if (workspace_bytes < need) return RAFT_ERR_WORKSPACE;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const int hw = H * W, nchunk = ceil_div(hw, kMetChunk);
+  MetricPartial* part = reinterpret_cast<MetricPartial*>(workspace);
+  RAFT_TRY(launch(flow_metrics_partial_kernel, dim3((unsigned)nchunk, (unsigned)B), kMetThreads, 0, st,
+                  reinterpret_cast<const float2*>(pred), reinterpret_cast<const float2*>(gt), valid, hw, use_max_flow != 0,
+                  max_flow, part));
+  return launch(flow_metrics_final_kernel, dim3((unsigned)B), kMetThreads, 0, st, part, nchunk, counts, sums);
 }
 
 int raft_b200_update_prepared_bytes(int variant, int corr_channels, int precision, size_t* bytes) {

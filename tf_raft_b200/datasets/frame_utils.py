@@ -1,10 +1,12 @@
-"""Flow file readers / writers -- host-side mirror of tf_raft/datasets/frame_utils.py:12-31, 83-107 (NumPy only; the
-evaluation scripts feed `RAFT.test_step` with what these return).
+"""Flow file readers / writers -- host-side mirror of tf_raft/datasets/frame_utils.py:12-68, 83-107, 123-137 (NumPy,
+and PIL for frames; the evaluation scripts feed `RAFT.test_step` with what these return).
 
 .flo (Middlebury): float32 tag 202021.25, int32 width, int32 height, then height x width x (u, v) float32, little endian.
 KITTI flow PNG: 16-bit RGB, u = (R - 2^15) / 64, v = (G - 2^15) / 64, B = valid flag.
 `write_png` writes the 8- and 16-bit RGB PNGs (KITTI flows, VisFlowCallback's pictures) without an image library.
 """
+import os
+import re
 import struct
 import zlib
 
@@ -89,6 +91,70 @@ def _read_png16_rgb(path):
         out[y] = cur
         prev = cur
     return out.reshape(h, w, 3, 2).astype(np.uint16) @ np.array([256, 1], dtype=np.uint16)
+
+
+def inflate_png16(path):
+    """The host half of a KITTI flow PNG read: chunks parsed, IDATs joined and inflated -> (filtered scanlines (bytes),
+    h, w).  The rows are checked for length and filter bytes 0-4 here; `read_flow_kitti_batch` undoes the filters on
+    the GPU.  Raises ValueError naming the file for anything but a well-formed non-interlaced 16-bit RGB PNG."""
+    try:
+        raw = open(path, 'rb').read()
+        ihdr, idat = None, []
+        for kind, body in _png_chunks(raw):
+            if kind == b'IHDR':
+                ihdr = struct.unpack('>IIBBBBB', body)
+            elif kind == b'IDAT':
+                idat.append(body)
+        if ihdr is None:
+            raise ValueError('no IHDR chunk')
+        w, h, depth, ctype, _, _, interlace = ihdr
+        if depth != 16 or ctype != 2 or interlace != 0:
+            raise ValueError(f'expected a non-interlaced 16-bit RGB PNG (KITTI flow), got depth {depth} colour type '
+                             f'{ctype} interlace {interlace}')
+        rows = zlib.decompress(b''.join(idat))
+    except (struct.error, zlib.error, ValueError) as e:
+        raise ValueError(f'{path}: {e}') from None
+    if h < 1 or w < 1 or len(rows) != h * (1 + 6 * w):
+        raise ValueError(f'{path}: {len(rows)} bytes of scanlines, expected {h} x (1 + 6 x {w})')
+    filters = np.frombuffer(rows, dtype=np.uint8)[::1 + 6 * w]
+    if filters.max() > 4:
+        raise ValueError(f'{path}: unknown PNG filter type {int(filters.max())} in row {int(np.argmax(filters > 4))}')
+    return rows, h, w
+
+
+def read_pfm(path):
+    """frame_utils.py:33-68 readPFM: 'PF' (3 channels) or 'Pf' (1), width and height, then a scale whose sign gives the
+    byte order (negative: little endian); rows are stored bottom-up, so the array is flipped.  -> float32 (H, W[, 3])."""
+    with open(path, 'rb') as f:
+        header = f.readline().rstrip()
+        if header not in (b'PF', b'Pf'):
+            raise ValueError(f'{path}: not a PFM file')
+        dims = re.match(rb'^(\d+)\s(\d+)\s$', f.readline())
+        if not dims:
+            raise ValueError(f'{path}: malformed PFM header')
+        width, height = map(int, dims.groups())
+        scale = float(f.readline().rstrip())
+        data = np.fromfile(f, ('<' if scale < 0 else '>') + 'f')
+    shape = (height, width, 3) if header == b'PF' else (height, width)
+    return np.flipud(np.reshape(data, shape))
+
+
+def read_gen(path, pil=False):
+    """frame_utils.py:123-137 read_gen: dispatch on the extension.  .png / .jpeg / .ppm / .jpg -> PIL.Image (opened
+    lazily, as the reference); .bin / .raw -> np.load; .flo -> read_flow; .pfm -> read_pfm as float32, a colour PFM
+    without its last channel; anything else -> [].  `pil` is accepted and ignored, as in the reference."""
+    ext = os.path.splitext(path)[-1]
+    if ext in ('.png', '.jpeg', '.ppm', '.jpg'):
+        from PIL import Image
+        return Image.open(path)
+    if ext in ('.bin', '.raw'):
+        return np.load(path)
+    if ext == '.flo':
+        return read_flow(path).astype(np.float32)
+    if ext == '.pfm':
+        flow = read_pfm(path).astype(np.float32)
+        return flow if flow.ndim == 2 else flow[:, :, :-1]
+    return []
 
 
 def read_flow_kitti(path):
