@@ -371,6 +371,26 @@ int raft_b200_encoder_forward(int variant, int norm_type, int out_dim, const voi
 int raft_b200_context_split(const float* cnet, int npix, int hidden, int context, float* net, float* inp,
                             void* stream);
 
+/* The encoders of one inference forward, model.py:74-86, as concurrent branches forked from `stream` and joined back
+ * into it before the call returns:
+ *   A: fnet(image1);
+ *   B: fnet(image2);
+ *   C: cnet(image1), then the context split into net / inp.
+ * fnet runs at the device's greatest stream priority, cnet at its least.  image1's stem im2col planes are built once, by
+ * A, and read by C.  Every output equals, bit for bit, what raft_b200_encoder_forward (training = 0, image_norm = 1) on
+ * each image batch and raft_b200_context_split compute.
+ *   image1, image2 : (N, H, W, 3), values 0..255
+ *   fmap1, fmap2   : (N, ceil(H/8), ceil(W/8), fnet_dim);  net : (..., hidden);  inp : (..., context)
+ *   workspace      : raft_b200_encode_pair_workspace_bytes(variant, N, H, W, hidden + context)
+ * The side streams and events are created on a host thread's first call for a device; that call must not be under
+ * CUDA-graph capture (RAFT_ERR_UNSUPPORTED).  Later calls allocate, create and synchronise nothing, so a capture
+ * records the call as a graph with three parallel branches.                                                        */
+int raft_b200_encode_pair_workspace_bytes(int variant, int N, int H, int W, int cnet_dim, size_t* bytes);
+int raft_b200_encode_pair(int variant, const void* fnet_prepared, int fnet_norm, int fnet_dim, const void* cnet_prepared,
+                          int cnet_norm, int hidden, int context, const float* image1, const float* image2, int N, int H,
+                          int W, float* fmap1, float* fmap2, float* net, float* inp, void* workspace, size_t workspace_bytes,
+                          void* stream);
+
 /* One keras Conv2D(cout, (kh, kw), 1, 'same') + optional activation on its own (fp32 FFMA path): the building block
  * behind the stand-alone FlowHead / ConvGRU / SepConvGRU / *MotionEncoder layers of update.py:5-106 when they are
  * used outside the fused update block.  x (B,H,W,cin), kernel HWIO, out (B,H,W,out_stride) written at channel out_c0.

@@ -98,6 +98,9 @@ _SIGNATURES = {
     'raft_b200_encoder_workspace_bytes': (_i, [_i, _i, _i, _i, ctypes.POINTER(_sz)]),
     'raft_b200_encoder_forward': (_i, [_i, _i, _i, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _sz, _vp]),
     'raft_b200_context_split': (_i, [_vp, _i, _i, _i, _vp, _vp, _vp]),
+    'raft_b200_encode_pair_workspace_bytes': (_i, [_i, _i, _i, _i, _i, ctypes.POINTER(_sz)]),
+    'raft_b200_encode_pair': (_i, [_i, _vp, _i, _i, _vp, _i, _i, _i, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _sz,
+                                   _vp]),
     'raft_b200_conv2d': (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _vp]),
     'raft_b200_forward_loop': (_i, [_i, _vp, ctypes.POINTER(_vp), _i, _i, _vp, _vp, _vp, ctypes.POINTER(_vp), _i,
                                     _i, _i, _i, _vp, _sz, _i, _vp]),

@@ -152,6 +152,57 @@ static int corr_build_tc(const float* f1, const float* f2, int B, int h, int w, 
   return launch(corr_tc_kernel, grid, kTcThreads, kCorrSmemBytes, st, p);
 }
 
+// ------------------------------------------------------------------------------------------------
+// Concurrent encode of an image pair (raft_b200_encode_pair)
+// ------------------------------------------------------------------------------------------------
+// Workspace: one encoder workspace per branch, then cnet's raw output (before the context split).
+struct PairWs {
+  void* enc[3];
+  size_t enc_bytes;
+  const __half *stem_hi, *stem_lo;           // image1's stem planes, built in branch A's workspace
+  float* cnet_out;
+  size_t total;
+};
+static PairWs pair_ws_layout(void* base, int variant, int N, int H, int W, int cnet_dim) {
+  PairWs P;
+  memset(&P, 0, sizeof(P));
+  uint8_t* b8 = reinterpret_cast<uint8_t*>(base);
+  P.enc_bytes = align_up(enc_ws_layout(nullptr, variant, N, H, W).total, 1024);
+  for (int i = 0; i < 3; ++i) P.enc[i] = b8 + i * P.enc_bytes;
+  const EncWs E = enc_ws_layout(P.enc[0], variant, N, H, W);
+  P.stem_hi = E.Ih; P.stem_lo = E.Il;
+  P.cnet_out = reinterpret_cast<float*>(b8 + 3 * P.enc_bytes);
+  P.total = 3 * P.enc_bytes + (size_t)N * ceil_div(H, 8) * ceil_div(W, 8) * cnet_dim * sizeof(float);
+  return P;
+}
+
+// The three side streams (two at the device's greatest priority for fnet, one at its least for cnet) and the fork / join
+// events, created on first use per host thread and device -- never inside a call that is being captured, so that a
+// captured call contains no stream or event creation.  Per thread, so that two threads never interleave their records
+// and waits on the same events.
+struct PairStreams { cudaStream_t s[3]; cudaEvent_t fork, stem, a, b, c; bool ready; };
+static int pair_streams(cudaStream_t caller, PairStreams** out) {
+  static thread_local PairStreams tab[64];
+  int dev = 0;
+  RAFT_CUDA_TRY(cudaGetDevice(&dev));
+  if (dev < 0 || dev >= 64) return RAFT_ERR_UNSUPPORTED;
+  PairStreams& ps = tab[dev];
+  if (!ps.ready) {
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    RAFT_CUDA_TRY(cudaStreamIsCapturing(caller, &cs));
+    if (cs != cudaStreamCaptureStatusNone) return RAFT_ERR_UNSUPPORTED;      // the first call must run eagerly
+    int least = 0, greatest = 0;
+    RAFT_CUDA_TRY(cudaDeviceGetStreamPriorityRange(&least, &greatest));
+    for (int i = 0; i < 3; ++i)
+      RAFT_CUDA_TRY(cudaStreamCreateWithPriority(&ps.s[i], cudaStreamNonBlocking, i < 2 ? greatest : least));
+    for (cudaEvent_t* e : {&ps.fork, &ps.stem, &ps.a, &ps.b, &ps.c})
+      RAFT_CUDA_TRY(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
+    ps.ready = true;
+  }
+  *out = &ps;
+  return RAFT_OK;
+}
+
 // Per-pair setup shared by the update_* entry points and the loop: zero the fp16 planes (their
 // padded channels must hold exact zeros), stage inp and the hidden state in operand format.
 static int update_begin(const UpdateCtx& c, const float* h, const float* inp) {
@@ -695,6 +746,60 @@ int raft_b200_context_split(const float* cnet, int npix, int hidden, int context
   if (npix < 1 || hidden < 1 || context < 1) return RAFT_ERR_BAD_SHAPE;
   return launch(context_split_kernel, grid_for((size_t)npix * (hidden + context)), 256, 0, reinterpret_cast<cudaStream_t>(stream),
                 cnet, (size_t)npix, hidden, context, net, inp);
+}
+
+int raft_b200_encode_pair_workspace_bytes(int variant, int N, int H, int W, int cnet_dim, size_t* bytes) {
+  if (!bytes) return RAFT_ERR_BAD_ARG;
+  RAFT_TRY(check_variant(variant));
+  RAFT_TRY(check_dims(N, H, W));
+  if (cnet_dim < 1) return RAFT_ERR_BAD_SHAPE;
+  *bytes = pair_ws_layout(nullptr, variant, N, H, W, cnet_dim).total;
+  return RAFT_OK;
+}
+
+int raft_b200_encode_pair(int variant, const void* fnet_prepared, int fnet_norm, int fnet_dim, const void* cnet_prepared,
+                          int cnet_norm, int hidden, int context, const float* image1, const float* image2, int N, int H,
+                          int W, float* fmap1, float* fmap2, float* net, float* inp, void* workspace, size_t workspace_bytes,
+                          void* stream) {
+  if (!fnet_prepared || !cnet_prepared || !image1 || !image2 || !fmap1 || !fmap2 || !net || !inp || !workspace)
+    return RAFT_ERR_BAD_ARG;
+  RAFT_TRY(check_variant(variant));
+  if (fnet_norm < 0 || fnet_norm > 2 || cnet_norm < 0 || cnet_norm > 2) return RAFT_ERR_BAD_ARG;
+  RAFT_TRY(check_dims(N, H, W));
+  const int cnet_dim = hidden + context;
+  for (int d : {fnet_dim, cnet_dim})
+    if (d < 32 || d > 256 || d % 32) return RAFT_ERR_BAD_SHAPE;
+  if (hidden < 1 || context < 1 || H < 8 || W < 8) return RAFT_ERR_BAD_SHAPE;
+  const int h = ceil_div(H, 8), w = ceil_div(W, 8);
+  const PairWs P = pair_ws_layout(workspace, variant, N, H, W, cnet_dim);
+  if (P.total > workspace_bytes) return RAFT_ERR_WORKSPACE;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  PairStreams* ps = nullptr;
+  RAFT_TRY(pair_streams(st, &ps));
+  cudaStream_t sa = ps->s[0], sb = ps->s[1], sc = ps->s[2];
+  const size_t enc_bytes = P.enc_bytes;
+
+  // Fork.  Branch A: fnet(image1); B: fnet(image2); C: cnet(image1) and the context split.  A builds image1's stem planes
+  // first and C reads them from A's workspace.
+  RAFT_CUDA_TRY(cudaEventRecord(ps->fork, st));
+  for (cudaStream_t s : {sa, sb, sc}) RAFT_CUDA_TRY(cudaStreamWaitEvent(s, ps->fork, 0));
+  int status = encoder_stem_im2col(variant, image1, N, H, W, 1, P.enc[0], sa);
+  if (!status) status = (int)cudaEventRecord(ps->stem, sa);
+  if (!status) status = encoder_forward(variant, fnet_norm, fnet_dim, fnet_prepared, image2, N, H, W, 0, 1, fmap2, P.enc[1],
+                                        enc_bytes, sb);
+  if (!status) status = (int)cudaStreamWaitEvent(sc, ps->stem, 0);
+  if (!status) status = encoder_forward(variant, cnet_norm, cnet_dim, cnet_prepared, image1, N, H, W, 0, 1, P.cnet_out, P.enc[2],
+                                        enc_bytes, sc, P.stem_hi, P.stem_lo);
+  if (!status) status = launch(context_split_kernel, grid_for((size_t)N * h * w * cnet_dim), 256, 0, sc, P.cnet_out,
+                               (size_t)N * h * w, hidden, context, net, inp);
+  if (!status) status = encoder_forward(variant, fnet_norm, fnet_dim, fnet_prepared, image1, N, H, W, 0, 1, fmap1, P.enc[0],
+                                        enc_bytes, sa, P.stem_hi, P.stem_lo);
+  // Join every branch back into the caller's stream, also after an error: a capture must not be left forked.
+  RAFT_CUDA_TRY(cudaEventRecord(ps->a, sa));
+  RAFT_CUDA_TRY(cudaEventRecord(ps->b, sb));
+  RAFT_CUDA_TRY(cudaEventRecord(ps->c, sc));
+  for (cudaEvent_t e : {ps->a, ps->b, ps->c}) RAFT_CUDA_TRY(cudaStreamWaitEvent(st, e, 0));
+  return status ? status : raft_launch_status();
 }
 
 int raft_b200_conv2d(const float* x, const float* kernel, const float* bias, int B, int H, int W, int cin, int kh,

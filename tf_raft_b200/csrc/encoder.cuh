@@ -226,8 +226,29 @@ inline int enc_conv_tc(const EncCtx& c, const TcWeightSlot& cs, int cout, const 
   return tc_launch(p, nsplit, c.st);
 }
 
+// The stem's operand: the 7x7 s2 input window of every output pixel as 192-channel fp16 planes (E.Ih / E.Il of `ws`).
+// It depends on the images alone, so encoders of the same images can share it (raft_b200_encode_pair).
+inline int encoder_stem_im2col(int variant, const float* images, int N, int H, int W, int image_norm, void* ws,
+                               cudaStream_t st) {
+  const EncWs E = enc_ws_layout(ws, variant, N, H, W);
+  const int h = (H + 1) / 2, w = (W + 1) / 2;
+  const size_t npix = (size_t)N * h * w;
+  const int tot_h = (h - 1) * 2 + 7 - H, tot_w = (w - 1) * 2 + 7 - W;
+  const float* src = images;
+  if (image_norm) {                                 // normalise once (O32 is free until the first ResBlock finishes)
+    const size_t nimg = (size_t)N * H * W * 3;
+    RAFT_TRY(launch(image_norm_kernel, grid_for(nimg), 256, 0, st, images, E.O32, nimg));
+    src = E.O32;
+  }
+  return launch(stem_im2col_kernel, grid_for(npix * 24), 256, 0, st, src, N, H, W, h, w, (tot_h > 0 ? tot_h : 0) / 2,
+                (tot_w > 0 ? tot_w : 0) / 2, 0, E.Ih, E.Il);
+}
+
+// stem_hi / stem_lo: the stem planes encoder_stem_im2col built for these images (in this or another workspace of the same
+// shape), or null to build them here.
 inline int encoder_forward(int variant, int norm_type, int out_dim, const void* prepared, const float* images, int N,
-                           int H, int W, int training, int image_norm, float* out, void* ws, size_t ws_bytes, cudaStream_t st) {
+                           int H, int W, int training, int image_norm, float* out, void* ws, size_t ws_bytes, cudaStream_t st,
+                           const __half* stem_hi = nullptr, const __half* stem_lo = nullptr) {
   EncCtx c;
   c.prep = reinterpret_cast<const uint8_t*>(prepared);
   c.L = enc_layout(variant, out_dim);
@@ -246,20 +267,15 @@ inline int encoder_forward(int variant, int norm_type, int out_dim, const void* 
   int h = (H + 1) / 2, w = (W + 1) / 2;
   {
     const size_t npix = (size_t)N * h * w;
-    const int tot_h = (h - 1) * 2 + 7 - H, tot_w = (w - 1) * 2 + 7 - W;
-    const float* src = images;
-    if (image_norm) {                                 // normalise once (O32 is free until the first ResBlock finishes)
-      const size_t nimg = (size_t)N * H * W * 3;
-      RAFT_TRY(launch(image_norm_kernel, grid_for(nimg), 256, 0, st, images, E.O32, nimg));
-      src = E.O32;
+    if (!stem_hi) {
+      RAFT_TRY(encoder_stem_im2col(variant, images, N, H, W, image_norm, ws, st));
+      stem_hi = E.Ih; stem_lo = E.Il;
     }
-    RAFT_TRY(launch(stem_im2col_kernel, grid_for(npix * 24), 256, 0, st, src, N, H, W, h, w, (tot_h > 0 ? tot_h : 0) / 2,
-                    (tot_w > 0 ? tot_w : 0) / 2, 0, E.Ih, E.Il));
     if (!c.stats && pad64(S.c0) != S.c0) {
       RAFT_CUDA_TRY(cudaMemsetAsync(E.Xh, 0, npix * pad64(S.c0) * 2, st));
       RAFT_CUDA_TRY(cudaMemsetAsync(E.Xl, 0, npix * pad64(S.c0) * 2, st));
     }
-    RAFT_TRY(enc_conv_tc(c, L.conv1, S.c0, &L.norm1, E.Ih, E.Il, h, w, h, w, 1, 1, nullptr, c.stats ? E.Y32 : E.X32, E.Xh, E.Xl));
+    RAFT_TRY(enc_conv_tc(c, L.conv1, S.c0, &L.norm1, stem_hi, stem_lo, h, w, h, w, 1, 1, nullptr, c.stats ? E.Y32 : E.X32, E.Xh, E.Xl));
     if (c.stats) RAFT_TRY(enc_norm_apply(c, L.norm1, E.Y32, npix, h * w, 1, nullptr, nullptr, nullptr, nullptr, E.Xh, E.Xl));
   }
 

@@ -4,8 +4,10 @@
 `iters` (training) or `iters_pred` (inference) flow predictions (B, H, W, 2), like the reference
 (model.py:68-109 / 190-226).  The whole iteration loop (lookup -> update block -> coords += delta ->
 upsample) is ONE call into libraft_b200.so (raft_b200_forward_loop); the correlation pyramid is
-another (raft_b200_corr_pyramid_build).  Optionally the loop is replayed from a CUDA graph.
+another (raft_b200_corr_pyramid_build); in inference on the native encoders, so are the encoders, run as concurrent
+stream branches (raft_b200_encode_pair).  Optionally the whole forward is replayed from a CUDA graph.
 """
+import ctypes
 from collections import OrderedDict
 
 import torch
@@ -35,6 +37,7 @@ class RAFT:
         self.encoder_backend = encoder_backend
         self._build_layers(seed)
         self._graphs = {}
+        self._pair_ws = {}
         self.flow_metrics = None
         self.optimizer = None
         self._trainer = None
@@ -92,6 +95,8 @@ class RAFT:
     # -- forward ----------------------------------------------------------------------------------
     def _encode(self, image1, image2, training):
         # model.py:70-71 (2*(x/255)-1) happens inside the encoders' first load (raw_image=True)
+        if not training and self.fnet.backend == self.cnet.backend == 'native':
+            return self._encode_pair(image1, image2)
         fmap1, fmap2 = self.fnet([image1, image2], training=training, raw_image=True)     # :74
         net, inp = self._context(image1, training)
         return fmap1, fmap2, net, inp
@@ -106,6 +111,37 @@ class RAFT:
                                                           self.context_dim, _lib.ptr(net), _lib.ptr(inp),
                                                           _lib.stream()), 'context_split')
         return net, inp
+
+    def _encode_pair(self, image1, image2):
+        """The inference encode on the native encoders as one call, raft_b200_encode_pair: fnet(image1), fnet(image2)
+        and cnet(image1) run as concurrent branches (one branch's norm and im2col passes overlap another's
+        convolutions).  Every image's encoder output is independent of the batch it runs in, so this computes the bytes
+        of the separate fnet([image1, image2]) and `_context(image1)` calls.  Returns (fmap1, fmap2, net, inp)."""
+        bs, H, W, _ = image1.shape
+        h, w = -(-H // 8), -(-W // 8)
+        dev = image1.device
+        L = _lib.lib()
+        key = (bs, H, W)
+        if key not in self._pair_ws:
+            nbytes = ctypes.c_size_t()
+            _lib.check(L.raft_b200_encode_pair_workspace_bytes(self._variant, bs, H, W, self.hidden_dim + self.context_dim,
+                                                               ctypes.byref(nbytes)), 'encode_pair_workspace_bytes')
+            self._pair_ws = {key: _lib.workspace(nbytes.value, dev)}      # keep one shape at a time
+        ws = self._pair_ws[key]
+        fmap1 = torch.empty((bs, h, w, self.fnet.output_dim), dtype=torch.float32, device=dev)
+        fmap2 = torch.empty_like(fmap1)
+        net = torch.empty((bs, h, w, self.hidden_dim), dtype=torch.float32, device=dev)
+        inp = torch.empty((bs, h, w, self.context_dim), dtype=torch.float32, device=dev)
+        fnet, cnet = self.fnet, self.cnet
+        # The call joins its side streams back into the current stream before it returns, so the tensors above (allocated
+        # on the current stream) need no record_stream.
+        with torch.cuda.device(dev):
+            _lib.check(L.raft_b200_encode_pair(
+                self._variant, _lib.ptr(fnet.prepared()), _lib.NORM_TYPES[fnet.norm_type], fnet.output_dim,
+                _lib.ptr(cnet.prepared()), _lib.NORM_TYPES[cnet.norm_type], self.hidden_dim, self.context_dim,
+                _lib.ptr(image1), _lib.ptr(image2), bs, H, W, _lib.ptr(fmap1), _lib.ptr(fmap2), _lib.ptr(net), _lib.ptr(inp),
+                _lib.ptr(ws), ws.numel(), _lib.stream()), 'encode_pair')
+        return fmap1, fmap2, net, inp
 
     def _loop(self, corr_block, net, inp, coords1, flow_ups, b, h, w):
         ub = self.update_block
@@ -170,7 +206,7 @@ class RAFT:
                 outs = fn(*statics)
             # The captured kernels hold raw addresses of the encoder / update-block workspaces; those caches keep one
             # shape at a time, so the graph entry owns references to the buffers it was captured with.
-            keep = [list(m._ws.values()) for m in (self.fnet, self.cnet, self.update_block)]
+            keep = [list(m._ws.values()) for m in (self.fnet, self.cnet, self.update_block)] + [list(self._pair_ws.values())]
             entry = (graph, statics, outs, self._last, keep)
             self._graphs[key] = entry
         graph, statics, outs, last, _keep = entry
