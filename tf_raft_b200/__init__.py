@@ -11,9 +11,11 @@ from .layers.extractor import BasicEncoder, SmallEncoder
 from .layers.update import BasicUpdateBlock, SmallUpdateBlock
 from .losses import EndPointError, end_point_error, sequence_loss
 from .model import RAFT, SmallRAFT
-from .checkpoint import load_tf_checkpoint, read_tf_checkpoint, write_tf_checkpoint
+from .checkpoint import load_tf_checkpoint, param_to_tf_key, read_tf_checkpoint, tf_key_to_param, write_tf_checkpoint
 from .preprocess import CropOrPadder, pad_to_multiple, resize_with_crop_or_pad
-from .train import AdamW, CyclicalLearningRate, VisFlowCallback, first_cycle_scaler, inverse_scaler
+from .fit import Callback, History
+from .train import (AdamW, CyclicalLearningRate, ModelCheckpoint, TensorBoard, VisFlowCallback, first_cycle_scaler,
+                    inverse_scaler)
 from .evaluation import FlowMetrics, evaluate, flow_metrics
 from . import datasets
 
@@ -21,4 +23,5 @@ __all__ = ['CorrBlock', 'bilinear_sampler', 'coords_grid', 'fb_occlusion', 'forw
            'BasicEncoder', 'SmallEncoder',
            'BasicUpdateBlock', 'SmallUpdateBlock', 'RAFT', 'SmallRAFT', 'sequence_loss', 'end_point_error',
            'resize_with_crop_or_pad', 'CropOrPadder', 'pad_to_multiple', 'load_tf_checkpoint', 'read_tf_checkpoint',
-           'write_tf_checkpoint', 'FlowMetrics', 'evaluate', 'flow_metrics']
+           'write_tf_checkpoint', 'param_to_tf_key', 'tf_key_to_param', 'FlowMetrics', 'evaluate', 'flow_metrics',
+           'Callback', 'History', 'ModelCheckpoint', 'TensorBoard']

@@ -317,6 +317,31 @@ def tf_key_to_param(key):
     return '.'.join(out)
 
 
+def param_to_tf_key(name):
+    """The inverse of `tf_key_to_param`: `fnet.layer2.0.downsample.1.gamma` ->
+    `fnet/layer2/layer_with_weights-0/downsample/layer_with_weights-1/gamma/.ATTRIBUTES/VARIABLE_VALUE`, the key Keras's
+    `save_weights` gives the variable.  Numeric components are children of a keras Sequential (`layer_with_weights-N`,
+    N counting weight-owning children only, through `_SEQUENTIAL_CHILDREN`)."""
+    parts, out = name.split('.'), []
+    for i, part in enumerate(parts):
+        if part.isdigit():
+            n = int(part)
+            children = _SEQUENTIAL_CHILDREN.get(parts[i - 1] if i else '')
+            out.append(f'layer_with_weights-{children.index(n) if children else n}')
+        else:
+            out.append(part)
+    return '/'.join(out) + _SUFFIX
+
+
+# Keras's names for the optimiser's state in an object-graph checkpoint (OptimizerV2 `iterations`, Adam's slots)
+OPTIMIZER_ITER_KEY = 'optimizer/iter' + _SUFFIX
+
+
+def optimizer_slot_key(name, slot):
+    """`fnet.conv1.kernel`, 'm' -> `fnet/conv1/kernel/.OPTIMIZER_SLOT/optimizer/m/.ATTRIBUTES/VARIABLE_VALUE`."""
+    return param_to_tf_key(name)[:-len(_SUFFIX)] + f'/.OPTIMIZER_SLOT/optimizer/{slot}' + _SUFFIX
+
+
 def load_tf_checkpoint(prefix, verify=False, expect=None):
     """Checkpoint -> `{param name: ndarray}` for `RAFT.load_params` / `SmallRAFT.load_params`.
 

@@ -116,8 +116,12 @@ class FlowDataset:
         valid = None if self.augmentor is not None else _dense_valid(flow).astype(np.float32)
         return img1, img2, flow, valid
 
-    def batches(self, batch_size, *, target_size=None, workers=4, device=None, drop_last=False):
+    def batches(self, batch_size, *, target_size=None, workers=4, device=None, drop_last=False, repeat=False):
         """Batches of the items in index order, read by `workers` threads ahead of the consumer.
+
+        `repeat=True` (training mode only): the item stream never ends, item k being `k % len`, and a batch may
+        straddle the wrap -- the reference's `.batch()` over its endless generator (`__call__`); bound it with
+        `RAFT.fit`'s `steps_per_epoch`.
 
         Training mode (the dataset has an augmentor): yields `(image1, image2, flow, valid)` CUDA batches from
         `augmentor.batch`, ready for `RAFT.train_step`.  The augmentation parameters are drawn on the consuming thread
@@ -133,6 +137,8 @@ class FlowDataset:
             raise ValueError('batch_size must be >= 1')
         if self.is_test and self.augmentor is not None:
             raise ValueError('a test dataset has no flows to augment')
+        if repeat and (self.augmentor is None or len(self) == 0):
+            raise ValueError('repeat=True needs a non-empty training dataset (one with an augmentor)')
         device = torch.device(device if device is not None else
                               (self.augmentor.device if self.augmentor is not None else 'cuda'))
         if device.type != 'cuda':
@@ -145,8 +151,8 @@ class FlowDataset:
 
             def take():
                 nonlocal nxt
-                while nxt < n and len(ahead) < depth:
-                    ahead.append(pool.submit(self._load, nxt))
+                while (repeat or nxt < n) and len(ahead) < depth:
+                    ahead.append(pool.submit(self._load, nxt % n))
                     nxt += 1
                 return ahead.popleft().result() if ahead else None
 

@@ -10,6 +10,7 @@ stream branches (raft_b200_encode_pair).  Optionally the whole forward is replay
 import ctypes
 from collections import OrderedDict
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -42,6 +43,7 @@ class RAFT:
         self.optimizer = None
         self._trainer = None
         self._params_stale = False
+        self._pending_slots = None                         # optimiser state of load_weights awaiting the Trainer
 
     def _encoder_backend(self):
         # the all-FFMA reference configuration keeps cuDNN IEEE-fp32 encoders; the product path is native
@@ -65,6 +67,74 @@ class RAFT:
         self._graphs.clear()
         self._trainer = None                               # a training state built on the old values is void
         self._params_stale = False
+        self._pending_slots = None
+
+    def save_weights(self, filepath):
+        """Keras's `model.save_weights(filepath)` in its TensorFlow format: a tensor bundle at prefix `filepath`
+        (`filepath.index`, `filepath.data-00000-of-00001`) whose keys are the reference's object-graph keys
+        (`checkpoint.param_to_tf_key`), BatchNorm moving statistics included.  Once `train_step` has run (or optimiser
+        state was loaded), Adam's moments are saved under `<variable>/.OPTIMIZER_SLOT/optimizer/m|v/...` and the step
+        count under `optimizer/iter` (int64), so that `load_weights` resumes the run.
+
+        Not written: TensorFlow's `_CHECKPOINTABLE_OBJECT_GRAPH` proto.  `load_weights` and `load_tf_checkpoint` here
+        read these files; TensorFlow's own `load_weights` needs that proto and cannot."""
+        from .checkpoint import OPTIMIZER_ITER_KEY, optimizer_slot_key, param_to_tf_key, write_tf_checkpoint
+        tensors = {param_to_tf_key(k): v.detach().cpu().numpy() for k, v in self.state_dict().items()}
+        slots = self._pending_slots
+        if self._trainer is not None:
+            flat = self._trainer.flat
+            slots = {'iter': self.optimizer.iterations}
+            for name, buf in (('m', flat.m), ('v', flat.v)):
+                host = buf.cpu()
+                slots[name] = {k: view.numpy() for k, view in flat.slot(host).items()}
+        if slots is not None:
+            for name in ('m', 'v'):
+                tensors.update((optimizer_slot_key(k, name), a) for k, a in slots[name].items())
+            tensors[OPTIMIZER_ITER_KEY] = np.array(slots['iter'], dtype=np.int64)
+        write_tf_checkpoint(filepath, tensors)
+
+    def load_weights(self, filepath):
+        """Loads what `save_weights` (or a TensorFlow-written tensor bundle with the reference's keys) holds at prefix
+        `filepath`: the parameters through `load_tf_checkpoint(filepath, expect=self.state_dict())`.  When the file also
+        holds Adam's moments of every trainable variable and `optimizer/iter`, they are applied when the training state
+        is built -- at once if `compile` has run, else at `compile` -- and `optimizer.iterations` is set, so the
+        learning-rate schedule continues where the saved run stopped (the reference's `resume`).  Without them only
+        the weights load."""
+        from .checkpoint import OPTIMIZER_ITER_KEY, load_tf_checkpoint, optimizer_slot_key, read_tf_checkpoint
+        self.load_params(load_tf_checkpoint(filepath, expect=self.state_dict()))
+        tensors = read_tf_checkpoint(filepath)
+        shapes = {k: tuple(v.shape) for k, v in self.state_dict().items()
+                  if not (k.endswith('.moving_mean') or k.endswith('.moving_variance'))}
+        keys = {(k, name): optimizer_slot_key(k, name) for k in shapes for name in ('m', 'v')}
+        found = [key for key in keys.values() if key in tensors]
+        if not found and OPTIMIZER_ITER_KEY not in tensors:
+            return
+        missing = [key for key in keys.values() if key not in tensors]
+        if OPTIMIZER_ITER_KEY not in tensors:
+            missing.append(OPTIMIZER_ITER_KEY)
+        bad = [key for (k, _), key in keys.items() if key in tensors and tuple(tensors[key].shape) != shapes[k]]
+        if missing or bad:
+            raise ValueError(f'{filepath}: incomplete optimiser state -- missing {missing[:4]}'
+                             f'{"..." if len(missing) > 4 else ""}, mis-shaped {bad[:4]}')
+        self._pending_slots = {'iter': int(tensors[OPTIMIZER_ITER_KEY]),
+                               'm': {k: tensors[keys[k, 'm']] for k in shapes},
+                               'v': {k: tensors[keys[k, 'v']] for k in shapes}}
+        if self.optimizer is not None:
+            self._build_trainer()
+
+    def _build_trainer(self):
+        """The training state of `train_step`, with the optimiser state `load_weights` left pending applied to it."""
+        from .train import AdamW, Trainer
+        if not isinstance(self.optimizer, AdamW):
+            raise TypeError('optimizer must be tf_raft_b200.train.AdamW (tfa.optimizers.AdamW semantics)')
+        self._trainer = Trainer(self)
+        slots, self._pending_slots = self._pending_slots, None
+        if slots is not None:
+            flat = self._trainer.flat
+            for name, buf in (('m', flat.m), ('v', flat.v)):
+                for k, view in flat.slot(buf).items():
+                    view.copy_(torch.from_numpy(np.ascontiguousarray(slots[name][k], dtype=np.float32)))
+            self.optimizer.iterations = slots['iter']
 
     def state_dict(self):
         self._sync_trained_params()
@@ -366,6 +436,15 @@ class RAFT:
         self.loss = loss
         self.epe = epe
         self.flow_metrics = OrderedDict((k, [0.0, 0]) for k in ('loss', 'epe', 'u1', 'u3', 'u5'))
+        if self._pending_slots is not None and optimizer is not None:
+            self._build_trainer()
+
+    def fit(self, x, epochs=1, callbacks=None, steps_per_epoch=None, validation_data=None, validation_steps=None,
+            verbose=1):
+        """Keras's `Model.fit` as the reference's training scripts use it; see `tf_raft_b200.fit.fit`."""
+        from .fit import fit
+        return fit(self, x, epochs=epochs, callbacks=callbacks, steps_per_epoch=steps_per_epoch,
+                   validation_data=validation_data, validation_steps=validation_steps, verbose=verbose)
 
     def _metric_update(self, key, value):
         m = self.flow_metrics[key]
@@ -380,13 +459,13 @@ class RAFT:
         optimizer.apply_gradients, metrics.  data = (image1, image2, flow_gt, valid) on the GPU.  Under an initialised
         torch.distributed process group the gradients are all-reduced (one flat NCCL call) and the context encoder's
         BatchNorm statistics are taken over the global batch (tf_raft_b200/train.py)."""
-        from .train import AdamW, Trainer
+        from .train import AdamW
         if self.flow_metrics is None or getattr(self, 'optimizer', None) is None:
             raise RuntimeError('compile(optimizer=..., clip_norm=...) before train_step, as in train_chairs.py:92-98')
         if not isinstance(self.optimizer, AdamW):
             raise TypeError('optimizer must be tf_raft_b200.train.AdamW (tfa.optimizers.AdamW semantics)')
         if self._trainer is None:
-            self._trainer = Trainer(self)
+            self._build_trainer()
         loss, info = self._trainer.step(data, self.optimizer, self.clip_norm, self.loss, self.epe)
         self._params_stale = True                      # the layers' own copies are refreshed on the next inference call
         self._metric_update('loss', loss)

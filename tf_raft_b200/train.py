@@ -18,6 +18,10 @@ What runs where (DESIGN.md "Training"):
 """
 import math
 import os
+import socket
+import struct
+import time
+import warnings
 
 import numpy as np
 import torch
@@ -25,8 +29,10 @@ import torch.distributed as dist
 import torch.nn.functional as F
 
 from . import _lib
+from .checkpoint import _field, _mask, _put_varint, crc32c
 from .datasets.flow_viz import flow_to_image
 from .datasets.frame_utils import write_png
+from .fit import Callback
 from .layers.corr import CorrBlock
 from .layers.extractor import _same_pads, force_ieee_fp32
 from .losses import end_point_error, sequence_loss
@@ -46,7 +52,7 @@ def inverse_scaler(cycle):
     return 1.0 / cycle
 
 
-class VisFlowCallback:
+class VisFlowCallback(Callback):
     """tf_raft/training.py:26-88: at the end of each epoch, writes the model's prediction on a few dataset items as
     PNGs: image1, image2 and the flow colour wheel stacked vertically, `epoch{e+1:03d}_{i+1:03d}.png` in `logdir`.
 
@@ -66,9 +72,6 @@ class VisFlowCallback:
         self.logdir = logdir
         self.model = None
         os.makedirs(logdir, exist_ok=True)
-
-    def set_model(self, model):
-        self.model = model
 
     @staticmethod
     def _uint8(image):
@@ -93,6 +96,118 @@ class VisFlowCallback:
             flow_img = flow_to_image(resize_with_crop_or_pad(flow, h, w)).cpu().numpy()
             contents = np.concatenate([self._uint8(image1), self._uint8(image2), flow_img], axis=0)
             write_png(os.path.join(self.logdir, f'epoch{epoch + 1:03d}_{i + 1:03d}.png'), contents)
+
+
+class ModelCheckpoint(Callback):
+    """tf.keras.callbacks.ModelCheckpoint (TensorFlow 2.3) with save_freq='epoch', as the reference's scripts use it
+    (train_chairs.py:113-119): at the end of each epoch, `model.save_weights(filepath.format(epoch=epoch + 1, **logs))`.
+
+    save_best_only: save only when `logs[monitor]` strictly improves on the best value so far, which starts at +inf
+    (mode 'min') or -inf ('max'); 'auto' is 'max' when 'acc' is in the monitor's name, else 'min'.  A missing monitor
+    warns and does not save.  Only `save_weights_only=True` is supported (no SavedModel)."""
+
+    def __init__(self, filepath, monitor='val_loss', verbose=0, save_best_only=False, save_weights_only=False,
+                 mode='auto'):
+        super().__init__()
+        if not save_weights_only:
+            raise ValueError('ModelCheckpoint saves weights only (save_weights_only=True); there is no SavedModel')
+        if mode not in ('auto', 'min', 'max'):
+            warnings.warn(f'ModelCheckpoint mode {mode} is unknown, fallback to auto mode.')
+            mode = 'auto'
+        if mode == 'auto':
+            mode = 'max' if 'acc' in monitor else 'min'
+        self.filepath = os.fspath(filepath)
+        self.monitor = monitor
+        self.verbose = verbose
+        self.save_best_only = save_best_only
+        self.monitor_op = np.less if mode == 'min' else np.greater
+        self.best = np.inf if mode == 'min' else -np.inf
+
+    def on_epoch_end(self, epoch, logs=None):
+        logs = logs or {}
+        filepath = self.filepath.format(epoch=epoch + 1, **logs)
+        if self.save_best_only:
+            current = logs.get(self.monitor)
+            if current is None:
+                warnings.warn(f'Can save best model only with {self.monitor} available, skipping.')
+                return
+            if not self.monitor_op(current, self.best):
+                if self.verbose:
+                    print(f'\nEpoch {epoch + 1:05d}: {self.monitor} did not improve from {self.best:.5f}')
+                return
+            if self.verbose:
+                print(f'\nEpoch {epoch + 1:05d}: {self.monitor} improved from {self.best:.5f} to {current:.5f}, '
+                      f'saving model to {filepath}')
+            self.best = current
+        elif self.verbose:
+            print(f'\nEpoch {epoch + 1:05d}: saving model to {filepath}')
+        self.model.save_weights(filepath)
+
+
+class _EventWriter:
+    """One TensorBoard event file: TFRecord framing (uint64 length, masked crc32c of the length, the `Event` proto,
+    masked crc32c of the proto), first record `file_version: "brain.Event:2"`."""
+
+    _count = 0
+
+    def __init__(self, logdir):
+        os.makedirs(logdir, exist_ok=True)
+        _EventWriter._count += 1
+        name = f'events.out.tfevents.{int(time.time()):010d}.{socket.gethostname()}.{os.getpid()}.{self._count}.v2'
+        self.path = os.path.join(logdir, name)
+        self.file = open(self.path, 'wb')
+        # Event: wall_time = 1 (double), step = 2 (int64), file_version = 3 (string), summary = 5
+        self._write(_field(1, 1, struct.pack('<d', time.time())) + _field(3, 2, _bytes(b'brain.Event:2')))
+
+    def _write(self, event):
+        length = struct.pack('<Q', len(event))
+        self.file.write(length + struct.pack('<I', _mask(crc32c(length))) + event +
+                        struct.pack('<I', _mask(crc32c(event))))
+
+    def scalar(self, tag, value, step):
+        """Summary{value = 1 {tag = 1, simple_value = 2 (float)}} at `step`."""
+        summary_value = _field(1, 2, _bytes(tag.encode('utf-8'))) + _field(2, 5, struct.pack('<f', float(value)))
+        self._write(_field(1, 1, struct.pack('<d', time.time())) + _field(2, 0, _put_varint(int(step))) +
+                    _field(5, 2, _bytes(_field(1, 2, _bytes(summary_value)))))
+
+    def close(self):
+        self.file.close()
+
+
+def _bytes(payload):
+    return _put_varint(len(payload)) + payload
+
+
+class TensorBoard(Callback):
+    """tf.keras.callbacks.TensorBoard (TensorFlow 2.3) with update_freq='epoch', scalars only: at the end of each epoch
+    every log `name` becomes the scalar `epoch_<name>` at step = epoch index, the training logs in
+    `log_dir/train`, the `val_` logs (prefix stripped) in `log_dir/validation`, one event per scalar.  No graph,
+    histograms, images or profiling.  Keras's `tf.summary.scalar` stores the value as a tensor with scalar-plugin
+    metadata; this writes the `simple_value` field, which TensorBoard's scalar dashboard reads as well.  These
+    semantics come from reading TensorFlow 2.3's Keras sources, not from a TensorFlow run."""
+
+    def __init__(self, log_dir='logs'):
+        super().__init__()
+        self.log_dir = os.fspath(log_dir)
+        self._writers = {}
+
+    def on_epoch_end(self, epoch, logs=None):
+        logs = logs or {}
+        for name, items in (('train', {k: v for k, v in logs.items() if not k.startswith('val_')}),
+                            ('validation', {k[4:]: v for k, v in logs.items() if k.startswith('val_')})):
+            if not items:
+                continue
+            if name not in self._writers:
+                self._writers[name] = _EventWriter(os.path.join(self.log_dir, name))
+            writer = self._writers[name]
+            for k, v in items.items():
+                writer.scalar('epoch_' + k, v, epoch)
+            writer.file.flush()
+
+    def on_train_end(self, logs=None):
+        for writer in self._writers.values():
+            writer.close()
+        self._writers = {}
 
 
 class CyclicalLearningRate:
@@ -159,6 +274,10 @@ class FlatState:
             self.views[k] = leaf
         self._norm = torch.zeros(1, dtype=torch.float32, device=device)
         self._part = torch.zeros(1024, dtype=torch.float32, device=device)
+
+    def slot(self, buf):
+        """`{name: view}` of a buffer in this layout (self.m, self.v, or a host copy of one), shaped as the variables."""
+        return {k: buf[o:o + v.numel()].view(v.shape) for (k, v), o in zip(self.views.items(), self.offsets)}
 
     def zero_grad(self):
         self.g.zero_()
