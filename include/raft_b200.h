@@ -271,6 +271,32 @@ int raft_b200_flow_metrics(const float* pred, const float* gt, const float* vali
                            float max_flow, void* workspace, size_t workspace_bytes, long long* counts, double* sums,
                            void* stream);
 
+/* Element type and fill of one raft_b200_pad_batch plane.                                                           */
+typedef enum raft_pad_dtype { RAFT_PAD_U8 = 0, RAFT_PAD_F32 = 1 } raft_pad_dtype;
+typedef enum raft_pad_mode { RAFT_PAD_ZERO = 0, RAFT_PAD_REPLICATE = 1 } raft_pad_mode;
+
+/* One plane of an evaluation batch: src (h, w, c) is placed with its pixel (0, 0) at (top, left) of dst (H, W, c);
+ * a negative top or left crops.  Both dense row-major, of element type dtype, device memory.                         */
+typedef struct raft_pad_plane {
+  const void* src;
+  void* dst;
+  int h, w, c;
+  int H, W;
+  int top, left;
+  int dtype;                    /* raft_pad_dtype                                                                   */
+  int mode;                     /* raft_pad_mode                                                                    */
+} raft_pad_plane;
+
+/* Writes n planes of any sizes in one launch (RAFT's InputPadder and the reference's CropOrPadder, evaluate.py /
+ * dataset.py:323-334).  For every destination pixel, with sy = y - top, sx = x - left:
+ *   RAFT_PAD_REPLICATE: dst(y, x) = src(clamp(sy, 0, h-1), clamp(sx, 0, w-1))   (F.pad mode='replicate', np.pad 'edge')
+ *   RAFT_PAD_ZERO:      dst(y, x) = src(sy, sx) inside the source, 0 outside it
+ * Pure copies: the output is bit-exact.  dst must not overlap any src.  planes_host and planes_dev hold the same array
+ * (host copy for checks and the grid, device copy read by the kernel).  RAFT_ERR_BAD_ARG for a null pointer, an
+ * unknown dtype or mode, or a float32 plane that is not 4-byte aligned; RAFT_ERR_BAD_SHAPE unless 1 <= n <= 65535,
+ * h, w, c, H, W >= 1 and h * w * c, H * W * c <= 2^31 - 1.  Asynchronous, no allocation: graph-capturable.         */
+int raft_b200_pad_batch(const raft_pad_plane* planes_host, const raft_pad_plane* planes_dev, int n, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Update blocks  (tf_raft/layers/update.py)
  * ------------------------------------------------------------------------------------------- */

@@ -4,8 +4,15 @@
     python scripts/evaluate.py kitti --root datasets/KITTI --checkpoint checkpoints/model
 
 Defaults follow RAFT's evaluate.py: Sintel is pooled over pixels without the max-flow test ('pixel'), KITTI is averaged
-per image with Fl-all ('image'); chairs and things use the reference's Keras metric ('keras', max_flow 400).  Frames
-are zero-padded to a multiple of 8 (the reference's CropOrPadder), not edge-replicated as in RAFT's InputPadder.
+per image with Fl-all ('image'); chairs and things use the reference's Keras metric ('keras', max_flow 400).
+
+Padding: by default frames are zero-padded to a multiple of 8 and centred (the reference's CropOrPadder).  RAFT's
+published numbers use `--padding replicate` (InputPadder: edge replication), with `--pad-mode kitti` (all vertical
+padding at the bottom) for KITTI; `--warm-start` evaluates Sintel scene by scene, each pair after a scene's first
+started from the previous pair's forward-interpolated flow, as RAFT produced its Sintel test results:
+
+    python scripts/evaluate.py sintel --root ... --checkpoint ... --padding replicate --warm-start --iters 32
+    python scripts/evaluate.py kitti --root ... --checkpoint ... --padding replicate --pad-mode kitti
 """
 import argparse
 import json
@@ -46,6 +53,12 @@ def main():
     ap.add_argument('--workers', type=int, default=8)
     ap.add_argument('--protocol', choices=T.evaluation.PROTOCOLS, default=None)
     ap.add_argument('--max-flow', type=float, default=-1, help='ground-truth magnitude cut; 0 turns it off')
+    ap.add_argument('--padding', choices=('zero', 'replicate'), default='zero',
+                    help="'replicate' is RAFT's InputPadder; 'zero' the reference's CropOrPadder")
+    ap.add_argument('--pad-mode', choices=('sintel', 'kitti'), default=None,
+                    help="'kitti' puts all vertical padding at the bottom (default 'sintel': centred)")
+    ap.add_argument('--warm-start', action='store_true',
+                    help='scene by scene at batch 1, each pair started from the previous one (Sintel only)')
     args = ap.parse_args()
     if args.dstype is None:
         args.dstype = 'frames_cleanpass' if args.dataset == 'things' else 'clean'
@@ -56,9 +69,12 @@ def main():
     model = (T.SmallRAFT if args.small else T.RAFT)(iters_pred=args.iters)
     model.load_params(T.load_tf_checkpoint(args.checkpoint, expect=model.state_dict()))
     ds = dataset(args.dataset, args)
-    res = T.evaluate(model, ds, batch_size=args.batch_size, max_flow=max_flow, protocol=protocol, workers=args.workers)
+    res = T.evaluate(model, ds, batch_size=1 if args.warm_start else args.batch_size, max_flow=max_flow,
+                     protocol=protocol, workers=args.workers, padding=args.padding, pad_mode=args.pad_mode,
+                     warm_start=args.warm_start)
     print(json.dumps({'dataset': args.dataset, 'pairs': len(ds), 'protocol': protocol, 'max_flow': max_flow,
-                      'iters': args.iters, **res}))
+                      'iters': args.iters, 'padding': args.padding, 'pad_mode': args.pad_mode or 'sintel',
+                      'warm_start': args.warm_start, **res}))
 
 
 if __name__ == '__main__':

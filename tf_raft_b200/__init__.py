@@ -12,16 +12,18 @@ from .layers.update import BasicUpdateBlock, SmallUpdateBlock
 from .losses import EndPointError, end_point_error, sequence_loss
 from .model import RAFT, SmallRAFT
 from .checkpoint import load_tf_checkpoint, param_to_tf_key, read_tf_checkpoint, tf_key_to_param, write_tf_checkpoint
-from .preprocess import CropOrPadder, pad_to_multiple, resize_with_crop_or_pad
+from .preprocess import CropOrPadder, InputPadder, pad_to_multiple, resize_with_crop_or_pad
 from .fit import Callback, History
 from .train import (AdamW, CyclicalLearningRate, ModelCheckpoint, TensorBoard, VisFlowCallback, first_cycle_scaler,
                     inverse_scaler)
 from .evaluation import FlowMetrics, evaluate, flow_metrics
 from . import datasets
+from .submission import create_kitti_submission, create_sintel_submission
 
 __all__ = ['CorrBlock', 'bilinear_sampler', 'coords_grid', 'fb_occlusion', 'forward_interpolate', 'tfa_sampler', 'upflow8',
            'BasicEncoder', 'SmallEncoder',
            'BasicUpdateBlock', 'SmallUpdateBlock', 'RAFT', 'SmallRAFT', 'sequence_loss', 'end_point_error',
-           'resize_with_crop_or_pad', 'CropOrPadder', 'pad_to_multiple', 'load_tf_checkpoint', 'read_tf_checkpoint',
-           'write_tf_checkpoint', 'param_to_tf_key', 'tf_key_to_param', 'FlowMetrics', 'evaluate', 'flow_metrics',
-           'Callback', 'History', 'ModelCheckpoint', 'TensorBoard']
+           'resize_with_crop_or_pad', 'CropOrPadder', 'InputPadder', 'pad_to_multiple', 'load_tf_checkpoint',
+           'read_tf_checkpoint', 'write_tf_checkpoint', 'param_to_tf_key', 'tf_key_to_param', 'FlowMetrics', 'evaluate', 'flow_metrics',
+           'Callback', 'History', 'ModelCheckpoint', 'TensorBoard', 'create_sintel_submission',
+           'create_kitti_submission']

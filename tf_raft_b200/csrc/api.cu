@@ -12,6 +12,7 @@
 #include "dataset.cuh"
 #include "encoder.cuh"
 #include "flow_viz.cuh"
+#include "pad.cuh"
 #include "train.cuh"
 #include "video.cuh"
 
@@ -621,6 +622,26 @@ int raft_b200_flow_metrics(const float* pred, const float* gt, const float* vali
                   reinterpret_cast<const float2*>(pred), reinterpret_cast<const float2*>(gt), valid, hw, use_max_flow != 0,
                   max_flow, part));
   return launch(flow_metrics_final_kernel, dim3((unsigned)B), kMetThreads, 0, st, part, nchunk, counts, sums);
+}
+
+int raft_b200_pad_batch(const raft_pad_plane* planes_host, const raft_pad_plane* planes_dev, int n, void* stream) {
+  if (!planes_host || !planes_dev) return RAFT_ERR_BAD_ARG;
+  if (n < 1 || n > 65535) return RAFT_ERR_BAD_SHAPE;
+  int max_h = 1;
+  for (int i = 0; i < n; ++i) {
+    const raft_pad_plane& p = planes_host[i];
+    if (!p.src || !p.dst || (p.dtype != RAFT_PAD_U8 && p.dtype != RAFT_PAD_F32)) return RAFT_ERR_BAD_ARG;
+    if (p.mode != RAFT_PAD_ZERO && p.mode != RAFT_PAD_REPLICATE) return RAFT_ERR_BAD_ARG;
+    if (p.dtype == RAFT_PAD_F32 &&
+        (reinterpret_cast<uintptr_t>(p.src) | reinterpret_cast<uintptr_t>(p.dst)) % sizeof(float))
+      return RAFT_ERR_BAD_ARG;
+    if (p.h < 1 || p.w < 1 || p.c < 1 || p.H < 1 || p.W < 1) return RAFT_ERR_BAD_SHAPE;
+    if ((size_t)p.h * p.w * p.c > (size_t)INT_MAX || (size_t)p.H * p.W * p.c > (size_t)INT_MAX) return RAFT_ERR_BAD_SHAPE;
+    max_h = std::max(max_h, p.H);
+  }
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  return launch(pad_planes_kernel, dim3((unsigned)std::min(max_h, kPadMaxRowBlocks), (unsigned)n), kPadThreads, 0, st,
+                planes_dev);
 }
 
 int raft_b200_update_prepared_bytes(int variant, int corr_channels, int precision, size_t* bytes) {

@@ -19,7 +19,7 @@ from glob import glob
 import numpy as np
 import torch
 
-from ..preprocess import resize_with_crop_or_pad
+from ..preprocess import PAD_MODES, REPLICATE, ZERO, pad_planes, placement, resize_with_crop_or_pad
 from . import frame_utils
 from .augmentor import FlowAugmentor, SparseFlowAugmentor
 from .png16 import check_png16_status, decode_png16
@@ -116,7 +116,8 @@ class FlowDataset:
         valid = None if self.augmentor is not None else _dense_valid(flow).astype(np.float32)
         return img1, img2, flow, valid
 
-    def batches(self, batch_size, *, target_size=None, workers=4, device=None, drop_last=False, repeat=False):
+    def batches(self, batch_size, *, target_size=None, workers=4, device=None, drop_last=False, repeat=False,
+                padding='zero', pad_mode='sintel'):
         """Batches of the items in index order, read by `workers` threads ahead of the consumer.
 
         `repeat=True` (training mode only): the item stream never ends, item k being `k % len`, and a batch may
@@ -132,6 +133,12 @@ class FlowDataset:
         item's original (H, W).  With `target_size=None` each item gets the smallest centred padding to a multiple of 8,
         and a batch closes early when the padded shape changes.  Test datasets yield flow = valid = None.
 
+        `padding='replicate'` fills the frames' padding by edge replication, as RAFT's InputPadder does; it needs a
+        target no smaller than any frame (no axis cropped), which `target_size=None` always is.  `pad_mode='kitti'`
+        puts all vertical padding at the bottom (RAFT's KITTI mode) instead of centring it.  Flow and valid are always
+        zero-padded at the frames' placement, so padded pixels stay invalid.  Any choice but the default pads every
+        plane of the batch with one raft_b200_pad_batch launch.
+
         Host buffers are pinned; the upload of a batch runs on a copy stream and overlaps the consumer's GPU work."""
         if batch_size < 1:
             raise ValueError('batch_size must be >= 1')
@@ -139,10 +146,11 @@ class FlowDataset:
             raise ValueError('a test dataset has no flows to augment')
         if repeat and (self.augmentor is None or len(self) == 0):
             raise ValueError('repeat=True needs a non-empty training dataset (one with an augmentor)')
-        device = torch.device(device if device is not None else
-                              (self.augmentor.device if self.augmentor is not None else 'cuda'))
-        if device.type != 'cuda':
-            raise RuntimeError('FlowDataset.batches feeds CUDA tensors only (sm_90a); there is no CPU fallback')
+        _check_padding(padding, pad_mode)
+        if self.augmentor is not None and (padding, pad_mode) != ('zero', 'sintel'):
+            raise ValueError('padding and pad_mode apply to evaluation batches; this dataset has an augmentor')
+        device = self._device(device if device is not None else
+                              (self.augmentor.device if self.augmentor is not None else None))
         up = _Uploader(device)
         with concurrent.futures.ThreadPoolExecutor(max(1, int(workers))) as pool:
             ahead = collections.deque()
@@ -175,22 +183,36 @@ class FlowDataset:
             else:
                 pending = take()
                 while pending is not None:
-                    shape = self._padded(pending[0].shape[:2], target_size)
+                    shape = self._padded(pending[0].shape[:2], target_size, padding)
                     items = [pending]
                     pending = take()
                     while pending is not None and len(items) < batch_size and \
-                            self._padded(pending[0].shape[:2], target_size) == shape:
+                            self._padded(pending[0].shape[:2], target_size, padding) == shape:
                         items.append(pending)
                         pending = take()
                     if drop_last and len(items) < batch_size:
                         continue
-                    yield self._eval_batch(up, items, shape)
+                    if (padding, pad_mode) == ('zero', 'sintel'):
+                        yield self._eval_batch(up, items, shape)
+                    else:
+                        yield self._eval_batch_padded(up, items, shape, padding, pad_mode)
         up.finish()
 
     @staticmethod
-    def _padded(hw, target_size):
+    def _device(device):
+        device = torch.device(device if device is not None else 'cuda')
+        if device.type != 'cuda':
+            raise RuntimeError('FlowDataset.batches feeds CUDA tensors only (sm_90a); there is no CPU fallback')
+        return device
+
+    @staticmethod
+    def _padded(hw, target_size, padding='zero'):
         if target_size is not None:
-            return tuple(int(s) for s in target_size)
+            shape = tuple(int(s) for s in target_size)
+            if padding == 'replicate' and (shape[0] < hw[0] or shape[1] < hw[1]):
+                raise ValueError(f"padding='replicate' cannot crop: a {hw[0]}x{hw[1]} frame is larger than "
+                                 f"target_size {shape}")
+            return shape
         return tuple(-(-int(s) // 8) * 8 for s in hw)
 
     def _eval_batch(self, up, items, shape):
@@ -204,6 +226,138 @@ class FlowDataset:
             valid = torch.stack([resize_with_crop_or_pad(s[3].unsqueeze(-1), th, tw).squeeze(-1) for s in samples])
         up.release()
         return img1, img2, flow, valid, [tuple(it[0].shape[:2]) for it in items]
+
+    def _eval_batch_padded(self, up, items, shape, padding, pad_mode):
+        """`_eval_batch` with the pad kernel: frames replicate- or zero-padded, flow / valid zero-padded, all placed
+        by `preprocess.placement(..., pad_mode)`, in one launch."""
+        th, tw = shape
+        samples = up.stage(items)
+        B, dev = len(samples), up.device
+        img1 = torch.empty((B, th, tw, 3), dtype=torch.uint8, device=dev)
+        img2 = torch.empty_like(img1)
+        flow = valid = None
+        if not self.is_test:
+            flow = torch.empty((B, th, tw, 2), dtype=torch.float32, device=dev)
+            valid = torch.empty((B, th, tw), dtype=torch.float32, device=dev)
+        mode = REPLICATE if padding == 'replicate' else ZERO
+        jobs = []
+        for k, s in enumerate(samples):
+            top, left = placement(*s[0].shape[:2], th, tw, pad_mode)
+            jobs += [(s[0], img1[k], top, left, mode), (s[1], img2[k], top, left, mode)]
+            if not self.is_test:
+                jobs += [(s[2], flow[k], top, left, ZERO), (s[3], valid[k], top, left, ZERO)]
+        pad_planes(jobs)
+        up.release()
+        return img1, img2, flow, valid, [tuple(it[0].shape[:2]) for it in items]
+
+    # ------------------------------------------------------------------ the sequence loader (warm starts)
+    def scenes(self):
+        """The dataset's items as scenes of chained pairs: [(first index, number of pairs), ...] in index order.
+
+        Items chain when item k's second frame is item k+1's first frame.  A scene is a run of items with one scene name
+        in `extra_info` ((scene, frame index) entries, as MpiSintel has).  ValueError unless every item has such an
+        entry, the items of a scene chain, and each scene is one run: KITTI's pairs do not chain, and a shuffled or
+        repeated dataset no longer does."""
+        n = len(self.image_list)
+        if len(self.extra_info) != n or not all(isinstance(e, (tuple, list)) and len(e) == 2 for e in self.extra_info):
+            raise ValueError('sequences need (scene, frame index) extra_info for every item, as MpiSintel has; this '
+                             'dataset has none, or `+` / `*` / shuffle() left it out of step with the items')
+        runs, seen = [], set()
+        for k in range(n):
+            scene = self.extra_info[k][0]
+            if k and scene == self.extra_info[k - 1][0]:
+                if self.image_list[k - 1][1] != self.image_list[k][0]:
+                    raise ValueError(f'items {k - 1} and {k} of scene {scene!r} do not chain: '
+                                     f'{self.image_list[k - 1][1]} is not {self.image_list[k][0]}')
+                runs[-1][1] += 1
+            else:
+                if scene in seen:
+                    raise ValueError(f'scene {scene!r} comes back at item {k}: its items are not one run')
+                seen.add(scene)
+                runs.append([k, 1])
+        return [tuple(r) for r in runs]
+
+    def _load_step(self, index, first):
+        """Worker side of `sequences`: item `index`'s first frame (first=True), or its second frame with its ground
+        truth as `_load` reads it."""
+        if first:
+            return (_frame(self.image_list[index][0]),)
+        frame = _frame(self.image_list[index][1])
+        if self.is_test:
+            return (frame,)
+        path = self.flow_list[index]
+        if self.sparse:
+            return frame, ('png16', path, frame_utils.inflate_png16(path))
+        flow = np.array(frame_utils.read_gen(path)).astype(np.float32)
+        return frame, flow, _dense_valid(flow).astype(np.float32)
+
+    def sequences(self, *, target_size=None, padding='zero', pad_mode='sintel', workers=4, device=None, chunk=8):
+        """One scene at a time (see `scenes`), each frame decoded once, for warm-started evaluation.
+
+        Yields `(frames, flow, valid, size, indices)` per scene of T frames: frames (T, H', W', 3) uint8, flow
+        (T-1, H', W', 2) and valid (T-1, H', W') float32 -- pair k's ground truth -- or None for a test split, the
+        frames' original (H, W), and the dataset indices of the T-1 pairs.  Padding as in `batches` (one
+        raft_b200_pad_batch launch per `chunk` frames); `target_size=None` pads to the next multiple of 8.  Frames are
+        read by `workers` threads ahead of the consumer, across scene boundaries, and uploaded as `batches` does.  A
+        frame whose size differs from its scene's first raises ValueError."""
+        if self.augmentor is not None:
+            raise ValueError('sequences serve evaluation; this dataset has an augmentor')
+        _check_padding(padding, pad_mode)
+        if chunk < 1:
+            raise ValueError('chunk must be >= 1')
+        runs = self.scenes()
+        device = self._device(device)
+        up = _Uploader(device)
+        jobs = [(i0 + max(t - 1, 0), t == 0) for i0, n in runs for t in range(n + 1)]
+        with concurrent.futures.ThreadPoolExecutor(max(1, int(workers))) as pool:
+            ahead = collections.deque()
+            nxt, depth = 0, max(2 * chunk, 2 * max(1, int(workers)))
+
+            def take():
+                nonlocal nxt
+                while nxt < len(jobs) and len(ahead) < depth:
+                    ahead.append(pool.submit(self._load_step, *jobs[nxt]))
+                    nxt += 1
+                return ahead.popleft().result()
+
+            for i0, n in runs:
+                steps = [take()]
+                size = steps[0][0].shape[:2]
+                th, tw = self._padded(size, target_size, padding)
+                top, left = placement(*size, th, tw, pad_mode)
+                frames = torch.empty((n + 1, th, tw, 3), dtype=torch.uint8, device=device)
+                flow = valid = None
+                if not self.is_test:
+                    flow = torch.empty((n, th, tw, 2), dtype=torch.float32, device=device)
+                    valid = torch.empty((n, th, tw), dtype=torch.float32, device=device)
+                mode = REPLICATE if padding == 'replicate' else ZERO
+                t0 = 0
+                for t in range(n + 1):
+                    if t:
+                        steps.append(take())
+                        if steps[-1][0].shape[:2] != size:
+                            raise ValueError(f'{self.image_list[i0 + t - 1][1]}: {steps[-1][0].shape[:2]} frame in '
+                                             f'a scene of {size} frames')
+                    if len(steps) < chunk and t < n:
+                        continue
+                    planes = []
+                    for k, s in enumerate(up.stage(steps)):
+                        planes.append((s[0], frames[t0 + k], top, left, mode))
+                        if t0 + k and not self.is_test:
+                            planes += [(s[1], flow[t0 + k - 1], top, left, ZERO),
+                                       (s[2], valid[t0 + k - 1], top, left, ZERO)]
+                    pad_planes(planes)
+                    up.release()
+                    t0, steps = t + 1, []
+                yield frames, flow, valid, tuple(size), list(range(i0, i0 + n))
+        up.finish()
+
+
+def _check_padding(padding, pad_mode):
+    if padding not in ('zero', 'replicate'):
+        raise ValueError(f"unknown padding {padding!r}; expected 'zero' or 'replicate'")
+    if pad_mode not in PAD_MODES:
+        raise ValueError(f'unknown pad_mode {pad_mode!r}; expected one of {PAD_MODES}')
 
 
 class _Uploader:

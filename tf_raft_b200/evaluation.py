@@ -20,6 +20,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from .preprocess import placement
 
 PROTOCOLS = ('keras', 'pixel', 'image')
 _KEYS = ('epe', 'u1', 'u3', 'u5', 'fl_all')
@@ -112,6 +113,12 @@ class FlowMetrics:
         self._sums.append(sums)
         self.batch_sizes.append(int(counts.shape[0]))
 
+    def add_records(self, counts, sums):
+        """One batch of records already computed by `flow_metrics` (counts (B, 5), sums (B,), on the device)."""
+        self._counts.append(counts)
+        self._sums.append(sums)
+        self.batch_sizes.append(int(counts.shape[0]))
+
     def records(self):
         """-> (counts (N, 5) int64, sums (N,) float64) as NumPy, one read-back."""
         if not self._counts:
@@ -123,26 +130,74 @@ class FlowMetrics:
         return aggregate(counts, sums, self.batch_sizes, protocol or self.protocol)
 
 
+def _window(size, shape, pad_mode):
+    """(y0, y1, x0, x1): where an original `size` frame lies in its padded `shape` (clipped where it was cropped)."""
+    (h, w), (H, W) = size, shape
+    top, left = placement(h, w, H, W, pad_mode)
+    return max(top, 0), min(top + h, H), max(left, 0), min(left + w, W)
+
+
+def _score_unpadded(pred, flow, valid, sizes, pad_mode, max_flow):
+    """Records of a padded batch scored inside each item's original rectangle, one `flow_metrics` call per run of
+    items that share it.  -> (counts (B, 5), sums (B,)) on the device."""
+    counts, sums, k = [], [], 0
+    while k < len(sizes):
+        win = _window(sizes[k], pred.shape[1:3], pad_mode)
+        e = k + 1
+        while e < len(sizes) and _window(sizes[e], pred.shape[1:3], pad_mode) == win:
+            e += 1
+        y0, y1, x0, x1 = win
+        c, s = flow_metrics(pred[k:e, y0:y1, x0:x1], flow[k:e, y0:y1, x0:x1], valid[k:e, y0:y1, x0:x1], max_flow)
+        counts.append(c)
+        sums.append(s)
+        k = e
+    return torch.cat(counts), torch.cat(sums)
+
+
 def evaluate(model, dataset, *, batch_size=1, target_size=None, max_flow=400, protocol='keras', workers=4,
-             per_image=False):
+             per_image=False, padding='zero', pad_mode=None, warm_start=False):
     """Score `model` on `dataset` (a `tf_raft_b200.datasets` FlowDataset without augmentor).
 
     Runs `model([image1, image2], training=False, last_only=True)` over `dataset.batches(batch_size,
-    target_size=target_size, workers=workers)` -- frames crop-or-padded with zeros, padded pixels invalid -- and
-    returns the chosen aggregation: {'epe', 'u1', 'u3', 'u5', 'fl_all', 'pixels'}.  per_image=True adds 'records':
-    {'counts' (N, 5) [n, <1, <3, <5, outlier], 'sums' (N,) EPE sums} in dataset order.
+    target_size=target_size, workers=workers, padding=padding, pad_mode=pad_mode)` and returns the chosen aggregation:
+    {'epe', 'u1', 'u3', 'u5', 'fl_all', 'pixels'}.  per_image=True adds 'records': {'counts' (N, 5) [n, <1, <3, <5,
+    outlier], 'sums' (N,) EPE sums} in dataset order.
 
-    Zero padding is what the reference's CropOrPadder does.  Published RAFT numbers pad by edge replication
-    (InputPadder), so the two are not directly comparable."""
+    The default, zero padding centred (the reference's CropOrPadder), scores the padded prediction against the padded
+    ground truth, whose padded pixels are invalid.  `padding='replicate'` is RAFT's protocol (InputPadder; `pad_mode`
+    None means 'sintel', 'kitti' pads at the bottom): every choice but the default scores the prediction inside each
+    frame's original rectangle against the original ground truth, as RAFT's pad, predict, unpad, score does.  The
+    kept pixels are the same either way; only the order of the fp64 EPE sum differs.  Published RAFT numbers use
+    replicate padding; zero padding changes the encoders' input everywhere, not only at the border, so its numbers are
+    not directly comparable to them.
+
+    `warm_start=True` (batch_size 1 only) runs `model.predict_video(frames, warm_start=True)` over each scene of
+    `dataset.sequences(...)`, each frame decoded once: from the second pair of a scene on, the loop starts from the
+    forward-interpolated low-resolution flow of the previous pair, taken on the padded grid; it resets at each scene.
+    The records still come back in dataset order, one 'keras' batch per pair."""
     if dataset.augmentor is not None:
         raise ValueError('evaluate needs a dataset without aug_params')
     if dataset.is_test:
         raise ValueError('evaluate needs ground truth; this is a test split')
+    pad_mode = 'sintel' if pad_mode is None else pad_mode
+    if warm_start and batch_size != 1:
+        raise ValueError('warm_start=True evaluates one scene at a time, at batch_size 1')
     metrics = FlowMetrics(max_flow=max_flow, protocol=protocol)
-    for image1, image2, flow, valid, _ in dataset.batches(batch_size, target_size=target_size, workers=workers,
-                                                           device=model.device):
-        pred = model([image1, image2], training=False, last_only=True)[-1]
-        metrics.update_state(flow, pred, valid)
+    if warm_start:
+        for frames, flow, valid, size, _ in dataset.sequences(target_size=target_size, padding=padding,
+                                                              pad_mode=pad_mode, workers=workers, device=model.device):
+            preds = model.predict_video((f[None] for f in frames), warm_start=True)
+            for t, pred in enumerate(preds):
+                metrics.add_records(*_score_unpadded(pred, flow[t:t + 1], valid[t:t + 1], [size], pad_mode, max_flow))
+    else:
+        for image1, image2, flow, valid, sizes in dataset.batches(batch_size, target_size=target_size, workers=workers,
+                                                                  device=model.device, padding=padding,
+                                                                  pad_mode=pad_mode):
+            pred = model([image1, image2], training=False, last_only=True)[-1]
+            if (padding, pad_mode) == ('zero', 'sintel'):
+                metrics.update_state(flow, pred, valid)
+            else:
+                metrics.add_records(*_score_unpadded(pred, flow, valid, sizes, pad_mode, max_flow))
     counts, sums = metrics.records()
     out = aggregate(counts, sums, metrics.batch_sizes, protocol)
     if per_image:
