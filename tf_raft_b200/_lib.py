@@ -153,6 +153,22 @@ def stream():
     return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
+def call(name, device, *args):
+    """raft_b200_<name>(*args, stream) with the status checked: the one way the package launches library work.
+    `device` is the device of the tensors whose pointers are in `args`; the call runs with it current and on its
+    current stream, so pointers and stream cannot come from different devices."""
+    fn = getattr(lib(), 'raft_b200_' + name)
+    with torch.cuda.device(device):
+        check(fn(*args, stream()), name)
+
+
+def query_bytes(name, *args):
+    """The size_t result of a raft_b200_<name>(*args, size_t *out) size query (no device work, no stream)."""
+    nbytes = ctypes.c_size_t()
+    check(getattr(lib(), 'raft_b200_' + name)(*args, ctypes.byref(nbytes)), name)
+    return nbytes.value
+
+
 def require_cuda(*tensors):
     for t in tensors:
         if t is None:
@@ -174,6 +190,24 @@ def f32c(t):
 
 def workspace(nbytes, device):
     return torch.empty(max(int(nbytes), 16), dtype=torch.uint8, device=device)
+
+
+class WorkspaceCache:
+    """A layer's workspace by problem shape, one shape kept at a time: a new shape's buffer replaces the old one.
+    Kernels captured into a CUDA graph hold a buffer's raw address, so whoever captures one keeps `buffers()` alive
+    for as long as the graph (RAFT._graph_run)."""
+
+    def __init__(self):
+        self._held = {}
+
+    def get(self, key, device, nbytes):
+        """The buffer for `key`; on a miss, `nbytes()` gives the size to allocate on `device`."""
+        if key not in self._held:
+            self._held = {key: workspace(nbytes(), device)}
+        return self._held[key]
+
+    def buffers(self):
+        return list(self._held.values())
 
 
 def launch_count():

@@ -205,15 +205,11 @@ class _Augmentor:
             for r, rect in enumerate(p.rects):
                 for j in range(4):
                     a.rect[r][j] = int(rect[j])
-        lib = _lib.lib()
-        nbytes = ctypes.c_size_t()
-        with torch.cuda.device(dev):
-            _lib.check(lib.raft_b200_augment_workspace_bytes(arr, b, int(self._sparse), ctypes.byref(nbytes)),
-                       'augment_workspace_bytes')
-            ws = _lib.workspace(nbytes.value, dev)
-            arr_dev = torch.frombuffer(bytearray(arr), dtype=torch.uint8).to(dev)
-            fn = lib.raft_b200_augment_sparse if self._sparse else lib.raft_b200_augment_dense
-            _lib.check(fn(arr, _lib.ptr(arr_dev), b, _lib.ptr(ws), nbytes.value, _lib.stream()), 'augment')
+        nbytes = _lib.query_bytes('augment_workspace_bytes', arr, b, int(self._sparse))
+        ws = _lib.workspace(nbytes, dev)
+        arr_dev = torch.frombuffer(bytearray(arr), dtype=torch.uint8).to(dev)
+        _lib.call('augment_sparse' if self._sparse else 'augment_dense', dev, arr, _lib.ptr(arr_dev), b, _lib.ptr(ws),
+                  nbytes)
         return img1, img2, flow, valid
 
 

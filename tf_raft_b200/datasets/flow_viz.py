@@ -52,11 +52,9 @@ def _run(u, v, stride, b, h, w, clip_flow, normalize, rad_max, bgr, device):
     status = torch.empty(b, dtype=torch.int32, device=device)
     work = torch.empty(b, dtype=torch.int32, device=device) if normalize and rad_max is None else None
     clip = clip_flow is not None
-    with torch.cuda.device(device):
-        _lib.check(_lib.lib().raft_b200_flow_to_image(
-            _lib.ptr(u), _lib.ptr(v), stride, b, h, w, int(clip), float(clip_flow) if clip else 0.0, int(normalize),
-            _lib.ptr(rad_max), int(bool(bgr)), _lib.ptr(image), _lib.ptr(work), _lib.ptr(status), _lib.stream()),
-            'flow_to_image')
+    _lib.call('flow_to_image', device, _lib.ptr(u), _lib.ptr(v), stride, b, h, w, int(clip),
+              float(clip_flow) if clip else 0.0, int(normalize), _lib.ptr(rad_max), int(bool(bgr)), _lib.ptr(image),
+              _lib.ptr(work), _lib.ptr(status))
     return image, status.cpu()                                   # the one synchronisation of a call
 
 

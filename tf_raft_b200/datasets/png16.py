@@ -51,14 +51,12 @@ def decode_png16(data, layout, names, *, status_host=None):
         arr[i].flow, arr[i].valid = flow.data_ptr(), valid.data_ptr()
         result.append((flow, valid))
     status = torch.empty(n, dtype=torch.int32, device=dev)
-    with torch.cuda.device(dev):
-        arr_dev = torch.frombuffer(bytearray(arr), dtype=torch.uint8).to(dev, non_blocking=False)
-        _lib.check(_lib.lib().raft_b200_png16_flow_decode(_lib.ptr(data), data.numel(), arr, _lib.ptr(arr_dev), n,
-                                                          _lib.ptr(status), _lib.stream()), 'png16_flow_decode')
-        if status_host is None:
-            check_png16_status(status.cpu(), names)
-        else:
-            status_host.copy_(status, non_blocking=True)
+    arr_dev = torch.frombuffer(bytearray(arr), dtype=torch.uint8).to(dev, non_blocking=False)
+    _lib.call('png16_flow_decode', dev, _lib.ptr(data), data.numel(), arr, _lib.ptr(arr_dev), n, _lib.ptr(status))
+    if status_host is None:
+        check_png16_status(status.cpu(), names)
+    else:
+        status_host.copy_(status, non_blocking=True)
     return result
 
 
@@ -87,8 +85,6 @@ def read_flow_kitti_batch(paths, device='cuda'):
     hv = host.numpy()
     for off, (rows, _, _) in zip(offsets, inflated):
         hv[off:off + len(rows)] = np.frombuffer(rows, dtype=np.uint8)
-    device = torch.device(device)
-    with torch.cuda.device(device):
-        data = host.to(device, non_blocking=True)
-        decoded = decode_png16(data, [(off, h, w) for off in offsets], paths)
-        return torch.stack([f for f, _ in decoded]), torch.stack([v for _, v in decoded])
+    data = host.to(device, non_blocking=True)
+    decoded = decode_png16(data, [(off, h, w) for off in offsets], paths)
+    return torch.stack([f for f, _ in decoded]), torch.stack([v for _, v in decoded])

@@ -13,7 +13,6 @@ records on the device and aggregates them three ways:
 An outlier is epe > 3 and epe / |gt| > 0.05 (RAFT's validate_kitti).  A ratio over no pixels is NaN, as the reference's
 mean of an empty tensor.
 """
-import ctypes
 import math
 
 import numpy as np
@@ -39,17 +38,11 @@ def flow_metrics(pred, gt, valid=None, max_flow=400):
         valid = _lib.f32c(torch.as_tensor(valid, device=gt.device))
         if tuple(valid.shape) != (B, H, W):
             raise ValueError(f'flow_metrics: expected valid of shape {(B, H, W)}, got {tuple(valid.shape)}')
-    lib = _lib.lib()
-    nbytes = ctypes.c_size_t()
-    _lib.check(lib.raft_b200_flow_metrics_workspace_bytes(B, H, W, ctypes.byref(nbytes)), 'flow_metrics_workspace_bytes')
     counts = torch.empty((B, 5), dtype=torch.int64, device=gt.device)
     sums = torch.empty(B, dtype=torch.float64, device=gt.device)
-    with torch.cuda.device(gt.device):
-        ws = _lib.workspace(nbytes.value, gt.device)
-        _lib.check(lib.raft_b200_flow_metrics(_lib.ptr(pred), _lib.ptr(gt), _lib.ptr(valid), B, H, W,
-                                              int(max_flow is not None), float(0 if max_flow is None else max_flow),
-                                              _lib.ptr(ws), ws.numel(), _lib.ptr(counts), _lib.ptr(sums),
-                                              _lib.stream()), 'flow_metrics')
+    ws = _lib.workspace(_lib.query_bytes('flow_metrics_workspace_bytes', B, H, W), gt.device)
+    _lib.call('flow_metrics', gt.device, _lib.ptr(pred), _lib.ptr(gt), _lib.ptr(valid), B, H, W, int(max_flow is not None),
+              float(0 if max_flow is None else max_flow), _lib.ptr(ws), ws.numel(), _lib.ptr(counts), _lib.ptr(sums))
     return counts, sums
 
 

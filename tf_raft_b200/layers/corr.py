@@ -36,8 +36,7 @@ def bilinear_sampler(image, coords):
         raise ValueError('bilinear_sampler expects a single-channel image (M, H, W, 1)')
     p = coords.shape[1] * coords.shape[2]
     out = torch.empty(coords.shape[:-1] + (1,), dtype=torch.float32, device=image.device)
-    _lib.check(_lib.lib().raft_b200_bilinear_sampler(_lib.ptr(image), _lib.ptr(coords), m, h, w, p, _lib.ptr(out),
-                                                     _lib.stream()), 'bilinear_sampler')
+    _lib.call('bilinear_sampler', image.device, _lib.ptr(image), _lib.ptr(coords), m, h, w, p, _lib.ptr(out))
     return out
 
 
@@ -45,9 +44,7 @@ def coords_grid(batch_size, height, width, device=None):
     """Reference corr.py:72-90 -> (B, H, W, 2) with [..., 0] = x, [..., 1] = y."""
     device = torch.device('cuda') if device is None else torch.device(device)
     out = torch.empty((batch_size, height, width, 2), dtype=torch.float32, device=device)
-    with torch.cuda.device(out.device):
-        _lib.check(_lib.lib().raft_b200_coords_grid(batch_size, height, width, _lib.ptr(out), _lib.stream()),
-                   'coords_grid')
+    _lib.call('coords_grid', out.device, batch_size, height, width, _lib.ptr(out))
     return out
 
 
@@ -69,9 +66,7 @@ def forward_interpolate(flow):
     flow = _flow_field(flow, 'forward_interpolate')
     b, h, w, _ = flow.shape
     out = torch.empty_like(flow)
-    with torch.cuda.device(flow.device):
-        _lib.check(_lib.lib().raft_b200_forward_interpolate(_lib.ptr(flow), b, h, w, _lib.ptr(out), _lib.stream()),
-                   'forward_interpolate')
+    _lib.call('forward_interpolate', flow.device, _lib.ptr(flow), b, h, w, _lib.ptr(out))
     return out
 
 
@@ -102,9 +97,8 @@ def fb_occlusion(flow_fw, flow_bw, alpha1=0.01, alpha2=0.5):
     b, h, w, _ = flow_fw.shape
     occ_fw = torch.empty((b, h, w), dtype=torch.bool, device=flow_fw.device)
     occ_bw = torch.empty_like(occ_fw)
-    with torch.cuda.device(flow_fw.device):
-        _lib.check(_lib.lib().raft_b200_fb_occlusion(_lib.ptr(flow_fw), _lib.ptr(flow_bw), b, h, w, a1, a2,
-                                                     _lib.ptr(occ_fw), _lib.ptr(occ_bw), _lib.stream()), 'fb_occlusion')
+    _lib.call('fb_occlusion', flow_fw.device, _lib.ptr(flow_fw), _lib.ptr(flow_bw), b, h, w, a1, a2, _lib.ptr(occ_fw),
+              _lib.ptr(occ_bw))
     return occ_fw, occ_bw
 
 
@@ -113,9 +107,7 @@ def coords_init(flow_init):
     flow_init = _flow_field(flow_init, 'coords_init')
     b, h, w, _ = flow_init.shape
     out = torch.empty_like(flow_init)
-    with torch.cuda.device(flow_init.device):
-        _lib.check(_lib.lib().raft_b200_coords_init(_lib.ptr(flow_init), b, h, w, _lib.ptr(out), _lib.stream()),
-                   'coords_init')
+    _lib.call('coords_init', flow_init.device, _lib.ptr(flow_init), b, h, w, _lib.ptr(out))
     return out
 
 
@@ -126,7 +118,7 @@ def upflow8(flow, mode='bilinear'):
     flow = _lib.f32c(flow)
     b, h, w, _ = flow.shape
     out = torch.empty((b, 8 * h, 8 * w, 2), dtype=torch.float32, device=flow.device)
-    _lib.check(_lib.lib().raft_b200_upflow8(_lib.ptr(flow), b, h, w, _lib.ptr(out), _lib.stream()), 'upflow8')
+    _lib.call('upflow8', flow.device, _lib.ptr(flow), b, h, w, _lib.ptr(out))
     return out
 
 
@@ -148,19 +140,13 @@ class CorrBlock:
         if f1.shape != f2.shape or f1.dim() != 4:
             raise ValueError(f'fmap1/fmap2 must both be (B, h, w, C); got {tuple(f1.shape)} and {tuple(f2.shape)}')
         b, h, w, c = f1.shape
-        L = _lib.lib()
         sizes = (ctypes.c_size_t * num_levels)()
-        _lib.check(L.raft_b200_corr_pyramid_sizes(b, h, w, num_levels, sizes), 'corr_pyramid_sizes')
+        _lib.check(_lib.lib().raft_b200_corr_pyramid_sizes(b, h, w, num_levels, sizes), 'corr_pyramid_sizes')
         self.corr_pyramid = [torch.empty((b * h * w, h >> l, w >> l, 1), dtype=torch.float32, device=f1.device)
                              for l in range(num_levels)]
-        nbytes = ctypes.c_size_t()
-        _lib.check(L.raft_b200_corr_workspace_bytes(b, h, w, c, num_levels, self.precision, ctypes.byref(nbytes)),
-                   'corr_workspace_bytes')
-        ws = _lib.workspace(nbytes.value, f1.device)
-        with torch.cuda.device(f1.device):
-            _lib.check(L.raft_b200_corr_pyramid_build(_lib.ptr(f1), _lib.ptr(f2), b, h, w, c, num_levels,
-                                                      _lib.ptr_array(self.corr_pyramid), _lib.ptr(ws), ws.numel(),
-                                                      self.precision, _lib.stream()), 'corr_pyramid_build')
+        ws = _lib.workspace(_lib.query_bytes('corr_workspace_bytes', b, h, w, c, num_levels, self.precision), f1.device)
+        _lib.call('corr_pyramid_build', f1.device, _lib.ptr(f1), _lib.ptr(f2), b, h, w, c, num_levels,
+                  _lib.ptr_array(self.corr_pyramid), _lib.ptr(ws), ws.numel(), self.precision)
         self._ws = ws          # keep alive until the stream has consumed it
         self._shape = (b, h, w)
 
@@ -172,10 +158,8 @@ class CorrBlock:
             raise ValueError(f'coords shape {tuple(coords.shape)} does not match the correlation volume {self._shape}')
         nch = self.num_levels * (2 * self.radius + 1) ** 2
         out = torch.empty((b, h, w, nch), dtype=torch.float32, device=coords.device)
-        with torch.cuda.device(coords.device):
-            _lib.check(_lib.lib().raft_b200_corr_lookup(_lib.ptr_array(self.corr_pyramid), _lib.ptr(coords), b, h, w,
-                                                        self.num_levels, self.radius, _lib.ptr(out), nch,
-                                                        _lib.stream()), 'corr_lookup')
+        _lib.call('corr_lookup', coords.device, _lib.ptr_array(self.corr_pyramid), _lib.ptr(coords), b, h, w,
+                  self.num_levels, self.radius, _lib.ptr(out), nch)
         return out
 
     def correlation(self, fmap1, fmap2):

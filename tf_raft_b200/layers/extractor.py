@@ -9,13 +9,13 @@ independent GPU cross-check of the native path, never selected implicitly.
 Parameter names are the reference's Keras attribute paths, kernels HWIO, NHWC tensors at the interface.
 """
 import ctypes
-import math
 import os
 
 import torch
 import torch.nn.functional as F
 
 from .. import _lib
+from ._params import _Params
 
 
 def force_ieee_fp32():
@@ -30,84 +30,6 @@ def force_ieee_fp32():
 
 
 force_ieee_fp32()
-
-
-def _same_pads(n_in, k, s):
-    n_out = -(-n_in // s)
-    total = max((n_out - 1) * s + k - n_in, 0)
-    return total // 2, total - total // 2
-
-
-def _glorot(shape, gen):
-    kh, kw, cin, cout = shape
-    limit = math.sqrt(6.0 / (kh * kw * cin + kh * kw * cout))
-    return torch.empty(shape).uniform_(-limit, limit, generator=gen)
-
-
-class _Params:
-    """Named parameter store shared by the layer classes below."""
-
-    def __init__(self, device):
-        self.device = torch.device(device)
-        self.params = {}
-        self._nchw_cache = {}
-
-    def add_conv(self, name, kh, kw, cin, cout, gen):
-        self.params[name + '.kernel'] = _glorot((kh, kw, cin, cout), gen).to(self.device)
-        self.params[name + '.bias'] = torch.zeros(cout, device=self.device)
-
-    def add_norm(self, name, norm_type, c):
-        if norm_type is None:
-            return
-        self.params[name + '.gamma'] = torch.ones(c, device=self.device)
-        self.params[name + '.beta'] = torch.zeros(c, device=self.device)
-        if norm_type == 'batch':
-            self.params[name + '.moving_mean'] = torch.zeros(c, device=self.device)
-            self.params[name + '.moving_variance'] = torch.ones(c, device=self.device)
-
-    def load(self, params, prefix=''):
-        for name in self.params:
-            src = torch.as_tensor(params[prefix + name], dtype=torch.float32)
-            if tuple(src.shape) != tuple(self.params[name].shape):
-                raise ValueError(f'{prefix + name}: expected {tuple(self.params[name].shape)}, got {tuple(src.shape)}')
-            self.params[name] = src.to(self.device).contiguous()
-        self._nchw_cache.clear()
-
-    def conv(self, x, name, stride=1, padding='same'):
-        """Keras Conv2D on an NCHW tensor (HWIO kernel, cross-correlation, TF padding rules)."""
-        w = self._nchw_cache.get(name)
-        if w is None:
-            w = self.params[name + '.kernel'].permute(3, 2, 0, 1).contiguous()
-            self._nchw_cache[name] = w
-        if padding == 'same':
-            pt, pb = _same_pads(x.shape[2], w.shape[2], stride)
-            pl, pr = _same_pads(x.shape[3], w.shape[3], stride)
-            if pt or pb or pl or pr:
-                x = F.pad(x, (pl, pr, pt, pb))
-        return F.conv2d(x, w, self.params[name + '.bias'], stride=stride)
-
-    def norm(self, x, name, norm_type, training):
-        eps = 1e-3        # tfa InstanceNormalization and keras BatchNormalization both default to 1e-3
-        if norm_type is None:
-            return x
-        g = self.params[name + '.gamma'].view(1, -1, 1, 1)
-        b = self.params[name + '.beta'].view(1, -1, 1, 1)
-        if norm_type == 'instance':
-            mean = x.mean(dim=(2, 3), keepdim=True)
-            var = x.var(dim=(2, 3), unbiased=False, keepdim=True)
-        elif norm_type == 'batch':
-            if training:
-                mean = x.mean(dim=(0, 2, 3), keepdim=True)
-                var = x.var(dim=(0, 2, 3), unbiased=False, keepdim=True)
-                mom, n = 0.99, x.shape[0] * x.shape[2] * x.shape[3]      # keras fused update: n / (n - 1) (DESIGN.md §9)
-                self.params[name + '.moving_mean'].mul_(mom).add_((1 - mom) * mean.flatten())
-                self.params[name + '.moving_variance'].mul_(mom).add_((1 - mom) * n / max(n - 1, 1) * var.flatten())
-            else:
-                mean = self.params[name + '.moving_mean'].view(1, -1, 1, 1)
-                var = self.params[name + '.moving_variance'].view(1, -1, 1, 1)
-        else:
-            raise ValueError(f'Invalid norm_type specified: {norm_type}')
-        return (x - mean) * torch.rsqrt(var + eps) * g + b
 
 
 def Normalization(norm_type, groups=None):
@@ -131,29 +53,27 @@ class _Encoder:
         if self.backend not in ('native', 'torch'):
             raise ValueError(f'unknown encoder backend {self.backend!r}')
         self._prepared = None
-        self._ws = {}
+        self.workspaces = _lib.WorkspaceCache()
         self.output_dim = output_dim
         self.norm_type = Normalization(norm_type)
         self.drop_rate = drop_rate
-        gen = torch.Generator(device='cpu')
-        gen.manual_seed(0 if seed is None else seed)
-        self.store = _Params(device)
+        self.store = _Params(device, seed)
         s = self.store
-        s.add_conv('conv1', 7, 7, 3, self._c0, gen)
+        s.add_conv('conv1', 7, 7, 3, self._c0)
         s.add_norm('norm1', norm_type, self._c0)
         cin = self._c0
         for li, (c, stride) in enumerate(self._stages, start=1):
             for bi, st in enumerate((stride, 1)):
                 p = f'layer{li}.{bi}'
-                s.add_conv(p + '.conv1', 3, 3, cin, c, gen)
-                s.add_conv(p + '.conv2', 3, 3, c, c, gen)
+                s.add_conv(p + '.conv1', 3, 3, cin, c)
+                s.add_conv(p + '.conv2', 3, 3, c, c)
                 s.add_norm(p + '.norm1', norm_type, c)
                 s.add_norm(p + '.norm2', norm_type, c)
                 if st != 1:
-                    s.add_conv(p + '.downsample.0', 1, 1, cin, c, gen)
+                    s.add_conv(p + '.downsample.0', 1, 1, cin, c)
                     s.add_norm(p + '.downsample.1', norm_type, c)
                 cin = c
-        s.add_conv('conv2', 1, 1, cin, output_dim, gen)
+        s.add_conv('conv2', 1, 1, cin, output_dim)
 
     @property
     def params(self):
@@ -164,7 +84,7 @@ class _Encoder:
         self._prepared = None
 
     def state_dict(self, prefix=''):
-        return {prefix + k: v for k, v in self.store.params.items()}
+        return self.store.state_dict(prefix)
 
     # -- native path --------------------------------------------------------------------------------
     def _conv_struct(self, name):
@@ -182,7 +102,6 @@ class _Encoder:
 
     def prepared(self):
         if self._prepared is None:
-            L = _lib.lib()
             w = _lib.RaftEncoderWeights()
             w.conv1 = self._conv_struct('conv1')
             w.norm1 = self._norm_struct('norm1')
@@ -198,14 +117,10 @@ class _Encoder:
                         blk.downsample_norm = self._norm_struct(p + '.downsample.1')
                     k += 1
             w.conv2 = self._conv_struct('conv2')
-            nbytes = ctypes.c_size_t()
-            _lib.check(L.raft_b200_encoder_prepared_bytes(self._variant, self.output_dim, ctypes.byref(nbytes)),
-                       'encoder_prepared_bytes')
-            blob = _lib.workspace(nbytes.value, self.store.device)
-            with torch.cuda.device(self.store.device):
-                _lib.check(L.raft_b200_encoder_prepare(self._variant, _lib.NORM_TYPES[self.norm_type], self.output_dim,
-                                                       ctypes.cast(ctypes.pointer(w), ctypes.c_void_p), _lib.ptr(blob),
-                                                       blob.numel(), _lib.stream()), 'encoder_prepare')
+            blob = _lib.workspace(_lib.query_bytes('encoder_prepared_bytes', self._variant, self.output_dim),
+                                  self.store.device)
+            _lib.call('encoder_prepare', blob.device, self._variant, _lib.NORM_TYPES[self.norm_type], self.output_dim,
+                      ctypes.cast(ctypes.pointer(w), ctypes.c_void_p), _lib.ptr(blob), blob.numel())
             self._prepared = blob
         return self._prepared
 
@@ -214,20 +129,12 @@ class _Encoder:
         n, h, w, c = x.shape
         if c != 3:
             raise ValueError(f'encoder input must be (N, H, W, 3); got {tuple(x.shape)}')
-        L = _lib.lib()
-        key = (n, h, w)
-        if key not in self._ws:
-            nbytes = ctypes.c_size_t()
-            _lib.check(L.raft_b200_encoder_workspace_bytes(self._variant, n, h, w, ctypes.byref(nbytes)),
-                       'encoder_workspace_bytes')
-            self._ws = {key: _lib.workspace(nbytes.value, x.device)}
-        ws = self._ws[key]
+        ws = self.workspaces.get((n, h, w), x.device,
+                          lambda: _lib.query_bytes('encoder_workspace_bytes', self._variant, n, h, w))
         out = torch.empty((n, -(-h // 8), -(-w // 8), self.output_dim), dtype=torch.float32, device=x.device)
-        with torch.cuda.device(x.device):
-            _lib.check(L.raft_b200_encoder_forward(self._variant, _lib.NORM_TYPES[self.norm_type], self.output_dim,
-                                                   _lib.ptr(self.prepared()), _lib.ptr(x), n, h, w, int(bool(training)),
-                                                   int(bool(raw_image)), _lib.ptr(out), _lib.ptr(ws), ws.numel(),
-                                                   _lib.stream()), 'encoder_forward')
+        _lib.call('encoder_forward', x.device, self._variant, _lib.NORM_TYPES[self.norm_type], self.output_dim,
+                  _lib.ptr(self.prepared()), _lib.ptr(x), n, h, w, int(bool(training)), int(bool(raw_image)),
+                  _lib.ptr(out), _lib.ptr(ws), ws.numel())
         return out
 
     def _res_block(self, x, p, stride, training):

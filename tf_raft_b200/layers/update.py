@@ -12,11 +12,11 @@ block ('encoder.convc1.kernel', 'gru.convz1.bias', 'flow_head.conv1.kernel', 'ma
 kernels in HWIO layout exactly as Keras stores them.
 """
 import ctypes
-import math
 
 import torch
 
 from .. import _lib
+from ._params import _Params
 
 # (name, kh, kw, cin, cout) in the member order of raft_basic_weights / raft_small_weights.
 BASIC_CONVS = (
@@ -35,15 +35,26 @@ SMALL_CONVS = (
 )
 
 
-def glorot_uniform_(t, gen):
-    """Keras default kernel initialiser on an HWIO tensor: U(-l, l), l = sqrt(6 / (fan_in + fan_out))."""
-    kh, kw, cin, cout = t.shape
-    limit = math.sqrt(6.0 / (kh * kw * cin + kh * kw * cout))
-    return t.uniform_(-limit, limit, generator=gen)
-
-
-class _UpdateBlock:
+class _ConvParams:
+    """The parameters of the convolutions `_convs`, (name, kh, kw, cin, cout) each, initialised in that order."""
     _convs = ()
+
+    def __init__(self, *, device=None, seed=None):
+        self.device = torch.device('cuda' if device is None else device)
+        self.store = _Params(self.device, seed)
+        for conv in self._convs:
+            self.store.add_conv(*conv)
+
+    @property
+    def params(self):
+        return self.store.params
+
+    def load_params(self, params, prefix=''):
+        """Copy `{prefix+name: array}` (NumPy or torch, HWIO kernels) into the layer."""
+        self.store.load(params, prefix)
+
+
+class _UpdateBlock(_ConvParams):
     _variant = None
     _hidden = 0
     _context = 0
@@ -55,29 +66,17 @@ class _UpdateBlock:
                              f'(the only value the reference models use); got {filters}')
         self.filters = filters
         self.precision = _lib.resolve_precision(precision)
-        self.device = torch.device('cuda' if device is None else device)
-        gen = torch.Generator(device='cpu')
-        gen.manual_seed(0 if seed is None else seed)
-        self.params = {}
-        for name, kh, kw, cin, cout in self._convs:
-            self.params[name + '.kernel'] = glorot_uniform_(torch.empty(kh, kw, cin, cout), gen).to(self.device)
-            self.params[name + '.bias'] = torch.zeros(cout, device=self.device)
+        super().__init__(device=device, seed=seed)
         self._prepared = None
-        self._ws = {}
+        self.workspaces = _lib.WorkspaceCache()
 
     # -- parameters -------------------------------------------------------------------------
     def load_params(self, params, prefix=''):
-        """Copy `{prefix+name: array}` (NumPy or torch, HWIO kernels) into the block."""
-        for name in self.params:
-            src = params[prefix + name]
-            src = torch.as_tensor(src, dtype=torch.float32)
-            if tuple(src.shape) != tuple(self.params[name].shape):
-                raise ValueError(f'{prefix + name}: expected shape {tuple(self.params[name].shape)}, got {tuple(src.shape)}')
-            self.params[name] = src.to(self.device).contiguous()
+        super().load_params(params, prefix)
         self._prepared = None
 
     def state_dict(self, prefix=''):
-        return {prefix + k: v for k, v in self.params.items()}
+        return self.store.state_dict(prefix)
 
     def _weights_struct(self):
         arr = (_lib.RaftConv * len(self._convs))()
@@ -89,26 +88,17 @@ class _UpdateBlock:
     def prepared(self):
         """Device blob of re-laid-out weights (built once per parameter set)."""
         if self._prepared is None:
-            L = _lib.lib()
-            nbytes = ctypes.c_size_t()
-            _lib.check(L.raft_b200_update_prepared_bytes(self._variant, self._corr_ch, self.precision,
-                                                         ctypes.byref(nbytes)), 'update_prepared_bytes')
-            blob = _lib.workspace(nbytes.value, self.device)
+            nbytes = _lib.query_bytes('update_prepared_bytes', self._variant, self._corr_ch, self.precision)
+            blob = _lib.workspace(nbytes, self.device)
             arr = self._weights_struct()
-            with torch.cuda.device(self.device):
-                _lib.check(L.raft_b200_update_prepare(self._variant, ctypes.cast(arr, ctypes.c_void_p), _lib.ptr(blob),
-                                                      blob.numel(), self.precision, _lib.stream()), 'update_prepare')
+            _lib.call('update_prepare', blob.device, self._variant, ctypes.cast(arr, ctypes.c_void_p), _lib.ptr(blob),
+                      blob.numel(), self.precision)
             self._prepared = blob
         return self._prepared
 
     def workspace(self, b, h, w):
-        key = (b, h, w)
-        if key not in self._ws:
-            nbytes = ctypes.c_size_t()
-            _lib.check(_lib.lib().raft_b200_update_workspace_bytes(self._variant, b, h, w, self.precision,
-                                                                   ctypes.byref(nbytes)), 'update_workspace_bytes')
-            self._ws = {key: _lib.workspace(nbytes.value, self.device)}     # keep one shape at a time
-        return self._ws[key]
+        return self.workspaces.get((b, h, w), self.device, lambda: _lib.query_bytes(
+            'update_workspace_bytes', self._variant, b, h, w, self.precision))
 
     def _check_inputs(self, inputs):
         net, inp, corr, flow = inputs
@@ -136,11 +126,9 @@ class BasicUpdateBlock(_UpdateBlock):
         mask = torch.empty((b, h, w, 576), dtype=torch.float32, device=net.device) if compute_mask else None
         delta = torch.empty((b, h, w, 2), dtype=torch.float32, device=net.device)
         ws = self.workspace(b, h, w)
-        with torch.cuda.device(net.device):
-            _lib.check(_lib.lib().raft_b200_update_basic(
-                _lib.ptr(self.prepared()), _lib.ptr(net), _lib.ptr(inp), _lib.ptr(corr), _lib.ptr(flow),
-                _lib.ptr(net_out), _lib.ptr(mask), _lib.ptr(delta), b, h, w, _lib.ptr(ws), ws.numel(),
-                self.precision, _lib.stream()), 'update_basic')
+        _lib.call('update_basic', net.device, _lib.ptr(self.prepared()), _lib.ptr(net), _lib.ptr(inp), _lib.ptr(corr),
+                  _lib.ptr(flow), _lib.ptr(net_out), _lib.ptr(mask), _lib.ptr(delta), b, h, w, _lib.ptr(ws), ws.numel(),
+                  self.precision)
         return net_out, mask, delta
 
 
@@ -158,11 +146,8 @@ class SmallUpdateBlock(_UpdateBlock):
         net_out = torch.empty_like(net)
         delta = torch.empty((b, h, w, 2), dtype=torch.float32, device=net.device)
         ws = self.workspace(b, h, w)
-        with torch.cuda.device(net.device):
-            _lib.check(_lib.lib().raft_b200_update_small(
-                _lib.ptr(self.prepared()), _lib.ptr(net), _lib.ptr(inp), _lib.ptr(corr), _lib.ptr(flow),
-                _lib.ptr(net_out), _lib.ptr(delta), b, h, w, _lib.ptr(ws), ws.numel(), self.precision,
-                _lib.stream()), 'update_small')
+        _lib.call('update_small', net.device, _lib.ptr(self.prepared()), _lib.ptr(net), _lib.ptr(inp), _lib.ptr(corr),
+                  _lib.ptr(flow), _lib.ptr(net_out), _lib.ptr(delta), b, h, w, _lib.ptr(ws), ws.numel(), self.precision)
         return net_out, None, delta
 
 
@@ -174,25 +159,7 @@ class SmallUpdateBlock(_UpdateBlock):
 _ACT = {None: 0, 'relu': 1, 'sigmoid': 2, 'tanh': 3}
 
 
-class _ConvLayers:
-    _spec = ()          # (name, kh, kw, cin, cout)
-
-    def __init__(self, *, device=None, seed=None):
-        self.device = torch.device('cuda' if device is None else device)
-        gen = torch.Generator(device='cpu')
-        gen.manual_seed(0 if seed is None else seed)
-        self.params = {}
-        for name, kh, kw, cin, cout in self._spec:
-            self.params[name + '.kernel'] = glorot_uniform_(torch.empty(kh, kw, cin, cout), gen).to(self.device)
-            self.params[name + '.bias'] = torch.zeros(cout, device=self.device)
-
-    def load_params(self, params, prefix=''):
-        for name in self.params:
-            src = torch.as_tensor(params[prefix + name], dtype=torch.float32)
-            if tuple(src.shape) != tuple(self.params[name].shape):
-                raise ValueError(f'{prefix + name}: expected {tuple(self.params[name].shape)}, got {tuple(src.shape)}')
-            self.params[name] = src.to(self.device).contiguous()
-
+class _ConvLayers(_ConvParams):
     def _conv(self, x, name, act=None, out=None, out_c0=0):
         x = _lib.f32c(x)
         k, b = self.params[name + '.kernel'], self.params[name + '.bias']
@@ -202,9 +169,8 @@ class _ConvLayers:
             raise ValueError(f'{name}: expected {cin} input channels, got {c}')
         if out is None:
             out = torch.empty((bsz, h, w, cout), dtype=torch.float32, device=x.device)
-        with torch.cuda.device(x.device):
-            _lib.check(_lib.lib().raft_b200_conv2d(_lib.ptr(x), _lib.ptr(k), _lib.ptr(b), bsz, h, w, cin, kh, kw, cout,
-                                                   _ACT[act], _lib.ptr(out), out.shape[-1], out_c0, _lib.stream()), 'conv2d')
+        _lib.call('conv2d', x.device, _lib.ptr(x), _lib.ptr(k), _lib.ptr(b), bsz, h, w, cin, kh, kw, cout, _ACT[act],
+                  _lib.ptr(out), out.shape[-1], out_c0)
         return out
 
 
@@ -213,7 +179,7 @@ class FlowHead(_ConvLayers):
 
     def __init__(self, filters=256, in_channels=128, **kw):
         self.filters = filters
-        self._spec = (('conv1', 3, 3, in_channels, filters), ('conv2', 3, 3, filters, 2))
+        self._convs = (('conv1', 3, 3, in_channels, filters), ('conv2', 3, 3, filters, 2))
         super().__init__(**kw)
 
     def __call__(self, inputs):
@@ -227,7 +193,7 @@ class ConvGRU(_ConvLayers):
     def __init__(self, filters=128, in_channels=None, **kw):
         self.filters = filters
         cin = filters + (in_channels if in_channels is not None else {96: 146, 128: 256}.get(filters, filters))
-        self._spec = tuple((f'conv{g}{sfx}', kh, kwd, cin, filters) for sfx, kh, kwd in self._taps for g in 'zrq')
+        self._convs = tuple((f'conv{g}{sfx}', kh, kwd, cin, filters) for sfx, kh, kwd in self._taps for g in 'zrq')
         super().__init__(**kw)
 
     def _step(self, h, x, sfx):
@@ -252,7 +218,7 @@ class SepConvGRU(ConvGRU):
 
 class SmallMotionEncoder(_ConvLayers):
     """Reference update.py:70-85 -> concat([conv(...), flow]) with 82 channels."""
-    _spec = (('convc1', 1, 1, 196, 96), ('convf1', 7, 7, 2, 64), ('convf2', 3, 3, 64, 32), ('conv', 3, 3, 128, 80))
+    _convs = (('convc1', 1, 1, 196, 96), ('convf1', 7, 7, 2, 64), ('convf2', 3, 3, 64, 32), ('conv', 3, 3, 128, 80))
 
     def __call__(self, inputs):
         flow, corr = inputs
@@ -264,7 +230,7 @@ class SmallMotionEncoder(_ConvLayers):
 
 class BasicMotionEncoder(_ConvLayers):
     """Reference update.py:88-106 -> concat([conv(...), flow]) with 128 channels."""
-    _spec = (('convc1', 1, 1, 324, 256), ('convc2', 3, 3, 256, 192), ('convf1', 7, 7, 2, 128),
+    _convs = (('convc1', 1, 1, 324, 256), ('convc2', 3, 3, 256, 192), ('convf1', 7, 7, 2, 128),
              ('convf2', 3, 3, 128, 64), ('conv', 3, 3, 256, 126))
 
     def __call__(self, inputs):

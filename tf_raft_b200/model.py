@@ -7,7 +7,6 @@ upsample) is ONE call into libraft_b200.so (raft_b200_forward_loop); the correla
 another (raft_b200_corr_pyramid_build); in inference on the native encoders, so are the encoders, run as concurrent
 stream branches (raft_b200_encode_pair).  Optionally the whole forward is replayed from a CUDA graph.
 """
-import ctypes
 from collections import OrderedDict
 
 import numpy as np
@@ -38,7 +37,7 @@ class RAFT:
         self.encoder_backend = encoder_backend
         self._build_layers(seed)
         self._graphs = {}
-        self._pair_ws = {}
+        self._pair_ws = _lib.WorkspaceCache()
         self.flow_metrics = None
         self.optimizer = None
         self._trainer = None
@@ -157,9 +156,7 @@ class RAFT:
         if tuple(mask.shape) != (b, h, w, 576):
             raise ValueError(f'mask: expected {(b, h, w, 576)}, got {tuple(mask.shape)}')
         out = torch.empty((b, 8 * h, 8 * w, 2), dtype=torch.float32, device=flow.device)
-        with torch.cuda.device(flow.device):
-            _lib.check(_lib.lib().raft_b200_upsample_convex(_lib.ptr(flow), _lib.ptr(mask), b, h, w, _lib.ptr(out),
-                                                            _lib.stream()), 'upsample_convex')
+        _lib.call('upsample_convex', flow.device, _lib.ptr(flow), _lib.ptr(mask), b, h, w, _lib.ptr(out))
         return out
 
     # -- forward ----------------------------------------------------------------------------------
@@ -176,10 +173,8 @@ class RAFT:
         b, h, w, _ = cnet.shape
         net = torch.empty((b, h, w, self.hidden_dim), dtype=torch.float32, device=cnet.device)
         inp = torch.empty((b, h, w, self.context_dim), dtype=torch.float32, device=cnet.device)
-        with torch.cuda.device(cnet.device):                                              # :84-86
-            _lib.check(_lib.lib().raft_b200_context_split(_lib.ptr(cnet), b * h * w, self.hidden_dim,
-                                                          self.context_dim, _lib.ptr(net), _lib.ptr(inp),
-                                                          _lib.stream()), 'context_split')
+        _lib.call('context_split', cnet.device, _lib.ptr(cnet), b * h * w, self.hidden_dim, self.context_dim,
+                  _lib.ptr(net), _lib.ptr(inp))                                           # :84-86
         return net, inp
 
     def _encode_pair(self, image1, image2):
@@ -190,14 +185,8 @@ class RAFT:
         bs, H, W, _ = image1.shape
         h, w = -(-H // 8), -(-W // 8)
         dev = image1.device
-        L = _lib.lib()
-        key = (bs, H, W)
-        if key not in self._pair_ws:
-            nbytes = ctypes.c_size_t()
-            _lib.check(L.raft_b200_encode_pair_workspace_bytes(self._variant, bs, H, W, self.hidden_dim + self.context_dim,
-                                                               ctypes.byref(nbytes)), 'encode_pair_workspace_bytes')
-            self._pair_ws = {key: _lib.workspace(nbytes.value, dev)}      # keep one shape at a time
-        ws = self._pair_ws[key]
+        ws = self._pair_ws.get((bs, H, W), dev, lambda: _lib.query_bytes(
+            'encode_pair_workspace_bytes', self._variant, bs, H, W, self.hidden_dim + self.context_dim))
         fmap1 = torch.empty((bs, h, w, self.fnet.output_dim), dtype=torch.float32, device=dev)
         fmap2 = torch.empty_like(fmap1)
         net = torch.empty((bs, h, w, self.hidden_dim), dtype=torch.float32, device=dev)
@@ -205,22 +194,19 @@ class RAFT:
         fnet, cnet = self.fnet, self.cnet
         # The call joins its side streams back into the current stream before it returns, so the tensors above (allocated
         # on the current stream) need no record_stream.
-        with torch.cuda.device(dev):
-            _lib.check(L.raft_b200_encode_pair(
-                self._variant, _lib.ptr(fnet.prepared()), _lib.NORM_TYPES[fnet.norm_type], fnet.output_dim,
-                _lib.ptr(cnet.prepared()), _lib.NORM_TYPES[cnet.norm_type], self.hidden_dim, self.context_dim,
-                _lib.ptr(image1), _lib.ptr(image2), bs, H, W, _lib.ptr(fmap1), _lib.ptr(fmap2), _lib.ptr(net), _lib.ptr(inp),
-                _lib.ptr(ws), ws.numel(), _lib.stream()), 'encode_pair')
+        _lib.call('encode_pair', dev, self._variant, _lib.ptr(fnet.prepared()), _lib.NORM_TYPES[fnet.norm_type],
+                  fnet.output_dim, _lib.ptr(cnet.prepared()), _lib.NORM_TYPES[cnet.norm_type], self.hidden_dim,
+                  self.context_dim, _lib.ptr(image1), _lib.ptr(image2), bs, H, W, _lib.ptr(fmap1), _lib.ptr(fmap2),
+                  _lib.ptr(net), _lib.ptr(inp), _lib.ptr(ws), ws.numel())
         return fmap1, fmap2, net, inp
 
     def _loop(self, corr_block, net, inp, coords1, flow_ups, b, h, w):
         ub = self.update_block
         ws = ub.workspace(b, h, w)
-        with torch.cuda.device(self.device):
-            _lib.check(_lib.lib().raft_b200_forward_loop(
-                self._variant, _lib.ptr(ub.prepared()), _lib.ptr_array(corr_block.corr_pyramid), self.corr_levels,
-                self.corr_radius, _lib.ptr(net), _lib.ptr(inp), _lib.ptr(coords1), _lib.ptr_array(flow_ups),
-                len(flow_ups), b, h, w, _lib.ptr(ws), ws.numel(), self.precision, _lib.stream()), 'forward_loop')
+        _lib.call('forward_loop', net.device, self._variant, _lib.ptr(ub.prepared()),
+                  _lib.ptr_array(corr_block.corr_pyramid), self.corr_levels, self.corr_radius, _lib.ptr(net), _lib.ptr(inp),
+                  _lib.ptr(coords1), _lib.ptr_array(flow_ups), len(flow_ups), b, h, w, _lib.ptr(ws), ws.numel(),
+                  self.precision)
 
     def __call__(self, inputs, training, *, last_only=False, flow_init=None):
         """inputs = [image1, image2], each (B, H, W, 3) float in 0..255 on the GPU.
@@ -276,7 +262,8 @@ class RAFT:
                 outs = fn(*statics)
             # The captured kernels hold raw addresses of the encoder / update-block workspaces; those caches keep one
             # shape at a time, so the graph entry owns references to the buffers it was captured with.
-            keep = [list(m._ws.values()) for m in (self.fnet, self.cnet, self.update_block)] + [list(self._pair_ws.values())]
+            keep = [c.buffers() for c in (self.fnet.workspaces, self.cnet.workspaces, self.update_block.workspaces,
+                                            self._pair_ws)]
             entry = (graph, statics, outs, self._last, keep)
             self._graphs[key] = entry
         graph, statics, outs, last, _keep = entry

@@ -55,9 +55,8 @@ def pad_planes(jobs):
         p.src, p.dst = src.data_ptr(), dst.data_ptr()
         p.h, p.w, p.c, p.H, p.W = src.shape[0], src.shape[1], c, dst.shape[0], dst.shape[1]
         p.top, p.left, p.dtype, p.mode = int(top), int(left), _DTYPES[src.dtype], int(mode)
-    with torch.cuda.device(device):
-        arr_dev = torch.frombuffer(bytearray(arr), dtype=torch.uint8).pin_memory().to(device, non_blocking=True)
-        _lib.check(_lib.lib().raft_b200_pad_batch(arr, _lib.ptr(arr_dev), len(jobs), _lib.stream()), 'pad_batch')
+    arr_dev = torch.frombuffer(bytearray(arr), dtype=torch.uint8).pin_memory().to(device, non_blocking=True)
+    _lib.call('pad_batch', device, arr, _lib.ptr(arr_dev), len(jobs))
 
 
 def input_padding(h, w, mode='sintel'):

@@ -34,7 +34,8 @@ from .datasets.flow_viz import flow_to_image
 from .datasets.frame_utils import write_png
 from .fit import Callback
 from .layers.corr import CorrBlock
-from .layers.extractor import _same_pads, force_ieee_fp32
+from .layers._params import _same_pads
+from .layers.extractor import force_ieee_fp32
 from .losses import end_point_error, sequence_loss
 from .preprocess import resize_with_crop_or_pad
 
@@ -284,9 +285,8 @@ class FlatState:
 
     def global_norm(self):
         """sqrt(sum g^2) over every trainable variable (tf.linalg.global_norm), on the device."""
-        with torch.cuda.device(self.g.device):
-            _lib.check(_lib.lib().raft_b200_sumsq(_lib.ptr(self.g), self.g.numel(), _lib.ptr(self._part), self._part.numel(),
-                                                  _lib.ptr(self._norm), _lib.stream()), 'sumsq')
+        _lib.call('sumsq', self.g.device, _lib.ptr(self.g), self.g.numel(), _lib.ptr(self._part), self._part.numel(),
+                  _lib.ptr(self._norm))
         return self._norm                                                    # device scalar: sum of squares
 
     def apply(self, opt, clip_norm):
@@ -296,11 +296,9 @@ class FlatState:
         t = opt.iterations
         lr = opt.lr() if not callable(opt.learning_rate) else float(opt.learning_rate(t - 1))
         lr_t = lr * math.sqrt(1 - opt.beta_2 ** t) / (1 - opt.beta_1 ** t)
-        with torch.cuda.device(self.g.device):
-            _lib.check(_lib.lib().raft_b200_adamw_step(
-                _lib.ptr(self.p), _lib.ptr(self.g), _lib.ptr(self.m), _lib.ptr(self.v), self.p.numel(), _lib.ptr(sumsq),
-                float(clip_norm if clip_norm else 0.0), float(lr_t), float(opt.beta_1), float(opt.beta_2),
-                float(opt.epsilon), float(opt.weight_decay), _lib.stream()), 'adamw_step')
+        _lib.call('adamw_step', self.g.device, _lib.ptr(self.p), _lib.ptr(self.g), _lib.ptr(self.m), _lib.ptr(self.v),
+                  self.p.numel(), _lib.ptr(sumsq), float(clip_norm if clip_norm else 0.0), float(lr_t), float(opt.beta_1),
+                  float(opt.beta_2), float(opt.epsilon), float(opt.weight_decay))
 
 
 # ------------------------------------------------------------------------------------------------ autograd pieces
@@ -314,9 +312,8 @@ class _Lookup(torch.autograd.Function):
         levels = len(pyramid)
         nch = levels * (2 * radius + 1) ** 2
         out = torch.empty((b, h, w, nch), dtype=torch.float32, device=coords.device)
-        with torch.cuda.device(coords.device):
-            _lib.check(_lib.lib().raft_b200_corr_lookup(_lib.ptr_array(pyramid), _lib.ptr(coords), b, h, w, levels, radius,
-                                                        _lib.ptr(out), nch, _lib.stream()), 'corr_lookup')
+        _lib.call('corr_lookup', coords.device, _lib.ptr_array(pyramid), _lib.ptr(coords), b, h, w, levels, radius,
+                  _lib.ptr(out), nch)
         ctx.save_for_backward(coords, *pyramid)
         ctx.radius = radius
         return out
@@ -329,10 +326,8 @@ class _Lookup(torch.autograd.Function):
         grad_out = grad_out.contiguous()
         g_coords = torch.zeros_like(coords)
         g_pyr = [torch.zeros_like(p) for p in pyramid]
-        with torch.cuda.device(coords.device):
-            _lib.check(_lib.lib().raft_b200_corr_lookup_backward(
-                _lib.ptr_array(pyramid), _lib.ptr(coords), _lib.ptr(grad_out), b, h, w, levels, ctx.radius,
-                _lib.ptr(g_coords), _lib.ptr_array(g_pyr), _lib.stream()), 'corr_lookup_backward')
+        _lib.call('corr_lookup_backward', coords.device, _lib.ptr_array(pyramid), _lib.ptr(coords), _lib.ptr(grad_out),
+                  b, h, w, levels, ctx.radius, _lib.ptr(g_coords), _lib.ptr_array(g_pyr))
         return (g_coords, None) + tuple(g_pyr)
 
 
