@@ -39,6 +39,8 @@ struct alignas(64) MegaParams {
   unsigned int* next_item;        // work-list cursor (zeroed with the flags): CTAs claim items with atomicAdd
 };
 constexpr int kMegaQueue = 16;    // per-CTA ring of claimed item numbers (producer -> consumers)
+// The producer publishes an item before its first ring wait, so it runs at most nstages + 1 items ahead of the consumers.
+static_assert(kMegaMaxStages + 1 < kMegaQueue, "the item queue must hold the producer's lead over the consumers");
 
 #if defined(__CUDA_ARCH__)
 __device__ __forceinline__ unsigned int ld_acquire_gpu(const unsigned int* p) {
