@@ -139,6 +139,35 @@ int raft_b200_coords_init(const float* flow_init, int B, int h, int w, float* co
 int raft_b200_fb_occlusion(const float* flow_fw, const float* flow_bw, int B, int H, int W, float alpha1, float alpha2,
                            uint8_t* occ_fw, uint8_t* occ_bw, void* stream);
 
+/* Self-supervised training (an addition beyond the reference; DESIGN.md section 9.1).
+ *
+ * raft_b200_census: images (B, H, W, 3) float32 in 0..255 -> out (B, H, W, 48) float32, 16-byte aligned.  With
+ * g = (0.2989 R + 0.5870 G + 0.1140 B) / 255 (0 outside the frame) and the offsets (dy, dx) of [-3, 3]^2 \ {(0, 0)} in
+ * row-major order, channel k of pixel (x, y) is t / sqrt(0.81 + t^2), t = g(y + dy, x + dx) - g(y, x).  Every
+ * operation is one rounded fp32 operation in that order, no FMA.                                                    */
+int raft_b200_census(const float* images, int B, int H, int W, float* out, void* stream);
+
+/* raft_b200_unsup_loss: one direction's share of the self-supervised loss and its gradient, all n predictions in one
+ * pass.  census_t / census_s: raft_b200_census of the target (the image the flows start from) and of the source;
+ * image_t: the target image (B, H, W, 3); occ: (B, H, W) forward-backward occlusion of the target's pixels
+ * (raft_b200_fb_occlusion); flows: (n, B, H, W, 2) predictions, 8-byte aligned.  With m = !occ and the pixel at least
+ * 3 px from every border, gamma_i = gamma^(n-1-i), and for prediction i at pixel x:
+ *   D_i(x) = sum_c d^2 / (0.1 + d^2), d = census_t(x) - bilinear sample of census_s at x + F_i(x) (fb_occlusion's
+ *            corner rule; a landing outside the closed frame contributes 0),
+ *   L_c = sum_i gamma_i sum_x m (D_i + 0.01)^0.4 / max(sum_x m, 1),
+ *   L_s = sum_i gamma_i (S_h + S_v) / 2, S_h (S_v) the mean over horizontal (vertical) neighbour pairs of
+ *         exp(-edge_weight * mean_c |I_c(x') - I_c(x)| / 255) * (|dFx| + |dFy|) / 2,
+ * it writes sums[0] = L_c, sums[1] = L_s, sums[2] = sum_x m, sums[3] = census_weight / 2 * L_c +
+ * smoothness_weight / 2 * L_s (fp64), and grad (n, B, H, W, 2) = d sums[3] / d flows (d|u|/du = 0 at 0).
+ * partials: device scratch of npartials doubles, at least 4; the call uses 4 per CTA of a grid of
+ * min(npartials / 4, ceil(B*H*W / 256), 1056) CTAs and adds them in a fixed order, so two calls with the same
+ * inputs and npartials give the same bits.  H, W >= 2 (RAFT_ERR_BAD_SHAPE otherwise); weights and gamma finite and
+ * >= 0 (RAFT_ERR_BAD_ARG otherwise).                                                                                */
+int raft_b200_unsup_loss(const float* census_t, const float* census_s, const float* image_t, const uint8_t* occ,
+                         const float* flows, int n, int B, int H, int W, float census_weight, float smoothness_weight,
+                         float edge_weight, float gamma, double* partials, size_t npartials, double* sums, float* grad,
+                         void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Training augmentation  (tf_raft/datasets/augmentor.py FlowAugmentor :9-129, SparseFlowAugmentor :132-267, given
  * their random draws; dataset.py:102's dense valid)

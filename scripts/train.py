@@ -2,6 +2,7 @@
 
     python scripts/train.py chairs configs/train_chairs.yml [--small] [--seed S] [--workers N]
     python scripts/train.py sintel configs/train_sintel.yml
+    python scripts/train.py chairs configs/train_chairs.yml --self-supervised
 
 The config keys are the reference's: data.root (and data.split_txt for chairs), augment.* (the augmentor's
 arguments), model.iters / iters_pred / resume, train.epochs / batch_size / learning_rate / weight_decay / clip_norm,
@@ -16,6 +17,10 @@ save_best_only=True) callbacks writing to <logdir>/<timestamp>/{history, predict
 config saved beside them as config.yml.  The timestamp has seconds (the reference's has minutes), so that two runs
 started in the same minute do not share a directory.  `model.resume` names a checkpoint prefix written by a previous
 run; its weights, Adam moments and step count are restored, so the learning-rate schedule continues.
+
+`--self-supervised` compiles with `UnsupervisedLoss()` (DESIGN.md section 9.1): the training batches' ground truth is not
+used by the loss (the epe metrics of the forward prediction are still logged); the config, datasets, validation (val_epe
+against ground truth) and callbacks are the same.
 """
 import argparse
 import os
@@ -57,7 +62,7 @@ def need(config, path):
     return node
 
 
-def train(name, config, logdir, small=False, workers=4):
+def train(name, config, logdir, small=False, workers=4, self_supervised=False):
     root = need(config, 'data.root')
     aug_params = need(config, 'augment')
     iters, iters_pred, resume = (need(config, 'model.' + k) for k in ('iters', 'iters_pred', 'resume'))
@@ -89,7 +94,8 @@ def train(name, config, logdir, small=False, workers=4):
                                        step_size=1000, scale_fn=T.first_cycle_scaler, scale_mode='cycle')
     optimizer = T.AdamW(weight_decay=weight_decay, learning_rate=scheduler)
     raft = (T.SmallRAFT if small else T.RAFT)(drop_rate=0, iters=iters, iters_pred=iters_pred)
-    raft.compile(optimizer=optimizer, clip_norm=clip_norm, loss=T.sequence_loss, epe=T.end_point_error)
+    loss = T.UnsupervisedLoss() if self_supervised else T.sequence_loss
+    raft.compile(optimizer=optimizer, clip_norm=clip_norm, loss=loss, epe=T.end_point_error)
     if resume:
         print(f'Restoring pretrained weights from {resume} ...', end=' ')
         raft.load_weights(resume)
@@ -115,6 +121,8 @@ def main():
     parser.add_argument('--small', action='store_true', help='SmallRAFT instead of RAFT')
     parser.add_argument('--seed', type=int, default=None, help='seed np.random and random before the first shuffle')
     parser.add_argument('--workers', type=int, default=4, help='loader threads')
+    parser.add_argument('--self-supervised', action='store_true',
+                        help='train with UnsupervisedLoss (census + smoothness, both directions) instead of ground truth')
     args = parser.parse_args()
 
     with open(args.config) as f:
@@ -130,7 +138,7 @@ def main():
     if args.seed is not None:
         np.random.seed(args.seed)
         random.seed(args.seed)
-    train(args.dataset, config, logdir, small=args.small, workers=args.workers)
+    train(args.dataset, config, logdir, small=args.small, workers=args.workers, self_supervised=args.self_supervised)
 
 
 if __name__ == '__main__':

@@ -9,7 +9,7 @@ from .layers.corr import (CorrBlock, bilinear_sampler, coords_grid, fb_occlusion
                           upflow8)
 from .layers.extractor import BasicEncoder, SmallEncoder
 from .layers.update import BasicUpdateBlock, SmallUpdateBlock
-from .losses import EndPointError, end_point_error, sequence_loss
+from .losses import EndPointError, UnsupervisedLoss, end_point_error, sequence_loss
 from .model import RAFT, SmallRAFT
 from .checkpoint import load_tf_checkpoint, param_to_tf_key, read_tf_checkpoint, tf_key_to_param, write_tf_checkpoint
 from .preprocess import CropOrPadder, InputPadder, pad_to_multiple, resize_with_crop_or_pad
@@ -22,7 +22,7 @@ from .submission import create_kitti_submission, create_sintel_submission
 
 __all__ = ['CorrBlock', 'bilinear_sampler', 'coords_grid', 'fb_occlusion', 'forward_interpolate', 'tfa_sampler', 'upflow8',
            'BasicEncoder', 'SmallEncoder',
-           'BasicUpdateBlock', 'SmallUpdateBlock', 'RAFT', 'SmallRAFT', 'sequence_loss', 'end_point_error',
+           'BasicUpdateBlock', 'SmallUpdateBlock', 'RAFT', 'SmallRAFT', 'sequence_loss', 'end_point_error', 'UnsupervisedLoss',
            'resize_with_crop_or_pad', 'CropOrPadder', 'InputPadder', 'pad_to_multiple', 'load_tf_checkpoint',
            'read_tf_checkpoint', 'write_tf_checkpoint', 'param_to_tf_key', 'tf_key_to_param', 'FlowMetrics', 'evaluate', 'flow_metrics',
            'Callback', 'History', 'ModelCheckpoint', 'TensorBoard', 'create_sintel_submission',

@@ -14,6 +14,7 @@
 #include "flow_viz.cuh"
 #include "pad.cuh"
 #include "train.cuh"
+#include "unsup.cuh"
 #include "video.cuh"
 
 namespace raft {
@@ -481,6 +482,45 @@ int raft_b200_fb_occlusion(const float* flow_fw, const float* flow_bw, int B, in
   return launch(fb_occlusion_kernel, grid_for(2 * (size_t)B * H * W), 256, 0, reinterpret_cast<cudaStream_t>(stream),
                 reinterpret_cast<const float2*>(flow_fw), reinterpret_cast<const float2*>(flow_bw), B, H, W, alpha1, alpha2,
                 occ_fw, occ_bw);
+}
+
+int raft_b200_census(const float* images, int B, int H, int W, float* out, void* stream) {
+  if (!images || !out || reinterpret_cast<uintptr_t>(out) % 16) return RAFT_ERR_BAD_ARG;
+  RAFT_TRY(check_dims(B, H, W));
+  return launch(census_kernel, grid_for((size_t)B * H * W), 256, 0, reinterpret_cast<cudaStream_t>(stream), images, B, H,
+                W, out);
+}
+
+int raft_b200_unsup_loss(const float* census_t, const float* census_s, const float* image_t, const uint8_t* occ,
+                         const float* flows, int n, int B, int H, int W, float census_weight, float smoothness_weight,
+                         float edge_weight, float gamma, double* partials, size_t npartials, double* sums, float* grad,
+                         void* stream) {
+  if (!census_t || !census_s || !image_t || !occ || !flows || !partials || !sums || !grad || npartials < 4)
+    return RAFT_ERR_BAD_ARG;
+  for (float v : {census_weight, smoothness_weight, edge_weight, gamma})
+    if (!(v >= 0.0f && v <= FLT_MAX)) return RAFT_ERR_BAD_ARG;
+  if ((reinterpret_cast<uintptr_t>(census_t) | reinterpret_cast<uintptr_t>(census_s)) % 16 ||
+      (reinterpret_cast<uintptr_t>(flows) | reinterpret_cast<uintptr_t>(grad)) % sizeof(float2) ||
+      (reinterpret_cast<uintptr_t>(partials) | reinterpret_cast<uintptr_t>(sums)) % sizeof(double))
+    return RAFT_ERR_BAD_ARG;
+  RAFT_TRY(check_dims(B, H, W));
+  if (n < 1 || H < 2 || W < 2) return RAFT_ERR_BAD_SHAPE;
+  const size_t npix = (size_t)B * H * W;
+  const int blocks = (int)std::min<size_t>(std::min<size_t>(npartials / 4, (npix + kUnsupThreads - 1) / kUnsupThreads),
+                                           (size_t)kUnsupMaxBlocks);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  RAFT_TRY(launch(unsup_mask_count_kernel, blocks, kUnsupThreads, 0, st, occ, B, H, W, partials));
+  UnsupParams p;
+  p.ct = census_t; p.cs = census_s; p.img = image_t; p.occ = occ;
+  p.flows = reinterpret_cast<const float2*>(flows); p.grad = reinterpret_cast<float2*>(grad); p.partials = partials;
+  p.n = n; p.B = B; p.H = H; p.W = W;
+  p.gamma = gamma; p.edge = edge_weight; p.census_half = 0.5f * census_weight;
+  const double n_h = (double)B * H * (W - 1), n_v = (double)B * (H - 1) * W;
+  p.sh_scale = (float)(0.25 * smoothness_weight / n_h);
+  p.sv_scale = (float)(0.25 * smoothness_weight / n_v);
+  RAFT_TRY(launch(unsup_loss_partial_kernel, blocks, kUnsupThreads, 0, st, p));
+  return launch(unsup_loss_final_kernel, 1, kUnsupThreads, 0, st, partials, blocks, n_h, n_v, 0.5 * census_weight,
+                0.5 * smoothness_weight, sums);
 }
 
 // Checks every sample of an augmentation call and lays out its workspace: fills (fill) or verifies each ws_offset.

@@ -443,7 +443,10 @@ class RAFT:
 
     def train_step(self, data):
         """model.py:126-144: forward with training=True under autograd, sequence loss, clip_by_global_norm,
-        optimizer.apply_gradients, metrics.  data = (image1, image2, flow_gt, valid) on the GPU.  Under an initialised
+        optimizer.apply_gradients, metrics.  data = (image1, image2, flow_gt, valid) on the GPU.  With
+        `compile(loss=UnsupervisedLoss())` the step is self-supervised: data = (image1, image2) or (image1, image2,
+        flow_gt, valid), the bidirectional graph and that loss, epe / u1 / u3 / u5 of the forward final prediction when
+        ground truth is given and not updated otherwise (tf_raft_b200/train.py).  Under an initialised
         torch.distributed process group the gradients are all-reduced (one flat NCCL call) and the context encoder's
         BatchNorm statistics are taken over the global batch (tf_raft_b200/train.py)."""
         from .train import AdamW
@@ -456,8 +459,9 @@ class RAFT:
         loss, info = self._trainer.step(data, self.optimizer, self.clip_norm, self.loss, self.epe)
         self._params_stale = True                      # the layers' own copies are refreshed on the next inference call
         self._metric_update('loss', loss)
-        for k in ('epe', 'u1', 'u3', 'u5'):
-            self._metric_update(k, info[k])
+        if info is not None:                           # UnsupervisedLoss on a batch without ground truth
+            for k in ('epe', 'u1', 'u3', 'u5'):
+                self._metric_update(k, info[k])
         return self._metric_results()
 
     def _sync_trained_params(self):

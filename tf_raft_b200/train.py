@@ -36,7 +36,7 @@ from .fit import Callback
 from .layers.corr import CorrBlock
 from .layers._params import _same_pads
 from .layers.extractor import force_ieee_fp32
-from .losses import end_point_error, sequence_loss
+from .losses import UnsupervisedLoss, end_point_error, sequence_loss
 from .preprocess import resize_with_crop_or_pad
 
 force_ieee_fp32()
@@ -369,6 +369,41 @@ class _CorrPyramid(torch.autograd.Function):
         return g1.reshape(fmap1.shape), g2, None, None, None
 
 
+class _UnsupLoss(torch.autograd.Function):
+    """UnsupervisedLoss on stacked predictions: forward = raft_b200_unsup_loss once per direction, which writes the loss
+    terms and, in the same pass, the gradient of each direction's share of the loss with respect to every prediction;
+    backward = that gradient scaled by grad_output.
+
+    flows (2n, B, H, W, 2): the n forward predictions, then the n backward ones; census (2B, H, W, 48) and images
+    (2B, H, W, 3): [image1; image2]; occ (2B, H, W) bool: [occ_fw; occ_bw]."""
+
+    NPARTIALS = 4 * 1024              # fp64 scratch of a call: 4 per CTA (fixed, so that every call reduces alike)
+
+    @staticmethod
+    def forward(ctx, flows, census, images, occ, census_weight, smoothness_weight, edge_weight, gamma):
+        flows = flows.contiguous()
+        n2, b, h, w, _ = flows.shape
+        n = n2 // 2
+        occ = occ.to(torch.uint8).contiguous()
+        grad = torch.empty_like(flows)
+        partials = torch.empty(_UnsupLoss.NPARTIALS, dtype=torch.float64, device=flows.device)
+        sums = torch.empty((2, 4), dtype=torch.float64, device=flows.device)
+        for d in range(2):                                     # d = 0: image1 -> image2, d = 1: image2 -> image1
+            t, s = slice(d * b, (d + 1) * b), slice((1 - d) * b, (2 - d) * b)
+            _lib.call('unsup_loss', flows.device, _lib.ptr(census[t]), _lib.ptr(census[s]), _lib.ptr(images[t]),
+                      _lib.ptr(occ[t]), _lib.ptr(flows[d * n:(d + 1) * n]), n, b, h, w, census_weight,
+                      smoothness_weight, edge_weight, gamma, _lib.ptr(partials), partials.numel(), _lib.ptr(sums[d]),
+                      _lib.ptr(grad[d * n:(d + 1) * n]))
+        ctx.save_for_backward(grad)
+        ctx.terms = sums                                       # [direction][L_c, L_s, mask count, share of the loss]
+        return (sums[0, 3] + sums[1, 3]).to(torch.float32)
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        (grad,) = ctx.saved_tensors
+        return grad * grad_out, None, None, None, None, None, None, None
+
+
 def _all_reduce_sum(x):
     """differentiable all-reduce (sum) over the default process group; identity without one."""
     if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
@@ -481,11 +516,36 @@ class TrainGraph:
         fmap1, fmap2 = fm[:bs].contiguous(), fm[bs:].contiguous()
         pyramid = _CorrPyramid.apply(fmap1, fmap2, cfg['levels'], cfg['radius'], self.precision)
         cnet = self.encoder(x1.permute(0, 3, 1, 2), 'cnet', cfg['cnorm'])
+        return self._iterate(pyramid, cnet, bs, H, W, iters, image1.device)
+
+    def forward_bidirectional(self, image1, image2, iters):
+        """Both directions of B pairs as one graph: fnet and cnet each run once on [x1; x2], and the loop runs at batch
+        2B with fmap1 = [f1; f2], fmap2 = [f2; f1], as `RAFT.predict_bidirectional` does.  Returns (preds_fw, preds_bw),
+        the n predictions image1 -> image2 and image2 -> image1, each (B, H, W, 2).
+
+        One consequence: cnet's BatchNorm (RAFT) normalises over, and updates its moving statistics from, the 2B images
+        -- the global 2B under torch.distributed (SyncBN) -- where the supervised step's sees image1 only."""
+        cfg = self.cfg
+        bs, H, W, _ = image1.shape
+        x1 = 2 * (image1 / 255.0) - 1.0
+        x2 = 2 * (image2 / 255.0) - 1.0
+        both = torch.cat([x1, x2], dim=0).permute(0, 3, 1, 2)
+        fm = self.encoder(both, 'fnet', cfg['fnorm']).permute(0, 2, 3, 1)
+        fmap1, fmap2 = fm.contiguous(), torch.cat([fm[bs:], fm[:bs]]).contiguous()
+        pyramid = _CorrPyramid.apply(fmap1, fmap2, cfg['levels'], cfg['radius'], self.precision)
+        cnet = self.encoder(both, 'cnet', cfg['cnorm'])
+        preds = self._iterate(pyramid, cnet, 2 * bs, H, W, iters, image1.device)
+        return [p[:bs] for p in preds], [p[bs:] for p in preds]
+
+    def _iterate(self, pyramid, cnet, bs, H, W, iters, device):
+        """model.py:86-106: the context split and `iters` update-block iterations from zero flow; the upsampled
+        predictions."""
+        cfg = self.cfg
         net = torch.tanh(cnet[:, :cfg['hidden']])
         inp = F.relu(cnet[:, cfg['hidden']:])
         h, w = H // 8, W // 8
-        gy, gx = torch.meshgrid(torch.arange(h, dtype=torch.float32, device=image1.device),
-                                torch.arange(w, dtype=torch.float32, device=image1.device), indexing='ij')
+        gy, gx = torch.meshgrid(torch.arange(h, dtype=torch.float32, device=device),
+                                torch.arange(w, dtype=torch.float32, device=device), indexing='ij')
         coords0 = torch.stack([gx, gy], dim=-1)[None].repeat(bs, 1, 1, 1)
         coords1 = coords0.clone()
         preds = []
@@ -520,6 +580,8 @@ class Trainer:
         return out
 
     def step(self, data, optimizer, clip_norm, loss_fn=sequence_loss, epe_fn=end_point_error):
+        if isinstance(loss_fn, UnsupervisedLoss):
+            return self._step_unsupervised(data, optimizer, clip_norm, loss_fn, epe_fn)
         image1, image2, flow_gt, valid = data
         image1 = image1.to(torch.float32)
         image2 = image2.to(torch.float32)
@@ -544,4 +606,31 @@ class Trainer:
         self.flat.apply(optimizer, clip_norm)                                  # :135-136
         with torch.no_grad():
             info = epe_fn([flow_gt, valid], preds[-1].detach())                # :138
+        return loss.detach(), info
+
+    def _step_unsupervised(self, data, optimizer, clip_norm, loss_fn, epe_fn):
+        """`step` with an UnsupervisedLoss: the bidirectional graph, the loss on both directions' predictions, then the
+        same all-reduce, clipping and AdamW.  data = (image1, image2) or (image1, image2, flow, valid); with ground truth
+        the metrics are taken on the forward final prediction, without it they are None."""
+        if len(data) not in (2, 4):
+            raise ValueError(f'unsupervised train_step takes (image1, image2[, flow, valid]); got {len(data)} items')
+        image1 = data[0].to(torch.float32)
+        image2 = data[1].to(torch.float32)
+        self.flat.zero_grad()
+        cudnn_enabled = torch.backends.cudnn.enabled                     # off, as in the supervised step
+        torch.backends.cudnn.enabled = False
+        try:
+            preds = self.graph.forward_bidirectional(image1, image2, self.model.iters)
+            loss = loss_fn((image1, image2), preds)
+            loss.backward()
+        finally:
+            torch.backends.cudnn.enabled = cudnn_enabled
+        if self.world > 1:
+            dist.all_reduce(self.flat.g, op=dist.ReduceOp.SUM)
+            self.flat.g.div_(self.world)
+        self.flat.apply(optimizer, clip_norm)
+        info = None
+        if len(data) == 4:
+            with torch.no_grad():
+                info = epe_fn([data[2], data[3]], preds[0][-1].detach())
         return loss.detach(), info
