@@ -168,6 +168,17 @@ int raft_b200_unsup_loss(const float* census_t, const float* census_s, const flo
                          float edge_weight, float gamma, double* partials, size_t npartials, double* sums, float* grad,
                          void* stream);
 
+/* raft_b200_unsup_loss_norm: raft_b200_unsup_loss with L_c = sum_i gamma_i sum_x m (D_i + 0.01)^0.4 / N.
+ * census_norm: NULL (N = max(sum_x m, 1): the same launches and bits as raft_b200_unsup_loss) or a device pointer to
+ * one double N > 0, 8-byte aligned (RAFT_ERR_BAD_ARG otherwise); sums[2] is still this call's own mask count.
+ * Under data parallelism over R equal shards, with C the mask count of the whole batch, a rank passes
+ * N = max(C, 1) / R: its census share is then R times its part of the whole batch's, and the gradients summed over
+ * the ranks and divided by R are the whole batch's.                                                                 */
+int raft_b200_unsup_loss_norm(const float* census_t, const float* census_s, const float* image_t, const uint8_t* occ,
+                              const float* flows, int n, int B, int H, int W, float census_weight,
+                              float smoothness_weight, float edge_weight, float gamma, double* partials,
+                              size_t npartials, double* sums, float* grad, const double* census_norm, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Training augmentation  (tf_raft/datasets/augmentor.py FlowAugmentor :9-129, SparseFlowAugmentor :132-267, given
  * their random draws; dataset.py:102's dense valid)

@@ -131,3 +131,15 @@ def test_call_checks_status_and_runs_on_the_tensors_device():
     coords = np.stack([rng.uniform(-2, 11, (8, 5, 5)), rng.uniform(-2, 13, (8, 5, 5))], axis=-1).astype(np.float32)
     got = bilinear_sampler(torch.from_numpy(image).cuda(), torch.from_numpy(coords).cuda()).cpu().numpy()
     np.testing.assert_array_equal(got, corr_np.bilinear_sampler(image, coords))
+
+
+def test_every_binding_takes_as_many_arguments_as_the_header_declares():
+    """ctypes calls with too few or too many arguments fail only when made; compare each signature with its declaration."""
+    import re
+    from tf_raft_b200 import _lib
+    header = open(os.path.join(ROOT, 'include', 'raft_b200.h')).read()
+    decls = {m.group(1): m.group(2).strip() for m in re.finditer(r'\b(raft_b200_\w+)\s*\(([^)]*)\)\s*;', header)}
+    assert set(decls) == set(_lib._SIGNATURES)
+    for name, params in decls.items():
+        n = 0 if params in ('', 'void') else params.count(',') + 1
+        assert len(_lib._SIGNATURES[name][1]) == n, f'{name}: {len(_lib._SIGNATURES[name][1])} bound, {n} declared'

@@ -177,3 +177,65 @@ def test_bidirectional_graph_and_loss_match_oracle_autograd_on_cpu(monkeypatch, 
     assert (num / den) ** 0.5 <= 1e-4
     if variant == 'raft':        # cnet's BatchNorm saw 2B images: its moving statistics moved
         assert any(float((moving[k] - P[k]).abs().max()) > 0 for k in moving if k.startswith('cnet.'))
+
+
+# --------------------------------------------------------------------------------------------- the closed form
+def _closed_vs_autograd(b, h, w, n, case='random', occ_p=0.3, seed=0, chunk=97, **kw):
+    """unsup_np.direction_closed_form against torch.autograd of direction_terms on the same direction: L_c, L_s and
+    every gradient element to 1e-12 relative (of the largest gradient entry).  chunk=97 makes the census chunks and the
+    smoothness row bands small, so their seams fall everywhere."""
+    from test_gpu_unsup import _flows, _texture
+    cw, sw = kw.get('census_weight', 1.0), kw.get('smoothness_weight', 0.5)
+    gamma, ew, norm = kw.get('gamma', GAMMA), kw.get('edge_weight', 150.0), kw.get('census_norm')
+    rng = np.random.default_rng(seed)
+    im_t, im_s = _texture(b, h, w, seed + 1), _texture(b, h, w, seed + 2)
+    ct, cs = unsup_np.census(im_t), unsup_np.census(im_s)
+    mask = unsup_np.border_mask(b, h, w) & (rng.random((b, h, w)) >= occ_p)
+    flows = _flows(case, n, b, h, w, rng)
+    leaves = [torch.from_numpy(f).double().requires_grad_(True) for f in flows]
+    lc, ls = unsup_np.direction_terms(ct, cs, im_t, mask, leaves, gamma, ew, norm)
+    want_g = [g.numpy() for g in torch.autograd.grad(cw / 2 * lc + sw / 2 * ls, leaves)]
+    got_lc, got_ls, count, got_g = unsup_np.direction_closed_form(ct, cs, im_t, mask, flows, cw, sw, ew, gamma, norm,
+                                                                  chunk=chunk)
+    assert count == int(mask.sum())
+    for got, want in ((got_lc, float(lc.detach())), (got_ls, float(ls.detach()))):
+        if np.isnan(want):
+            assert np.isnan(got)
+        else:
+            assert got == pytest.approx(want, rel=1e-12, abs=1e-300), (got, want)
+    finite = [np.isfinite(g) for g in want_g]
+    scale = max([float(np.abs(g[m]).max()) for g, m in zip(want_g, finite) if m.any()] + [0.0])
+    for i, (g, wg, m) in enumerate(zip(got_g, want_g, finite)):
+        np.testing.assert_array_equal(np.isfinite(g), m, err_msg=f'prediction {i}: non-finite pattern')
+        assert float(np.abs(g[m] - wg[m]).max(initial=0.0)) <= 1e-12 * scale, f'prediction {i}'
+    return count, got_lc, got_ls, got_g
+
+
+@pytest.mark.parametrize('case', ['random', 'integer', 'leaving', 'flat', 'nonfinite'])
+def test_closed_form_matches_autograd_on_every_flow_kind(case):
+    _closed_vs_autograd(2, 24, 40, 3, case, seed=len(case))
+
+
+@pytest.mark.parametrize('shape', [(3, 7, 7, 2), (2, 6, 40, 3), (2, 40, 6, 3), (1, 2, 2, 1), (5, 37, 53, 4)],
+                         ids=['7x7', 'H<7', 'W<7', '2x2', 'ragged'])
+def test_closed_form_matches_autograd_at_edge_shapes(shape):
+    b, h, w, n = shape
+    count = _closed_vs_autograd(b, h, w, n, occ_p=0.0 if h == 7 else 0.3)[0]
+    if h == w == 7:
+        assert count == b                                             # one masked pixel, (3, 3), per image
+    if min(h, w) < 7:
+        assert count == 0
+
+
+@pytest.mark.parametrize('kw', [dict(gamma=0.0), dict(gamma=1.0), dict(gamma=1.25), dict(edge_weight=0.0),
+                                dict(edge_weight=1e4), dict(census_weight=0.0), dict(smoothness_weight=0.0),
+                                dict(census_norm=777.5), dict(occ_p=1.0), dict(occ_p=0.0)],
+                         ids=lambda kw: '-'.join(f'{k}={v}' for k, v in kw.items()))
+def test_closed_form_matches_autograd_at_parameter_edges(kw):
+    kw = dict(kw)
+    occ_p = kw.pop('occ_p', 0.3)
+    count, lc, ls, grads = _closed_vs_autograd(2, 19, 31, 3, occ_p=occ_p, **kw)
+    if occ_p == 1.0:
+        assert count == 0 and lc == 0.0
+    if kw.get('gamma') == 0.0:                                          # only the last prediction carries weight
+        assert all(not g.any() for g in grads[:-1]) and grads[-1].any()

@@ -82,6 +82,8 @@ _SIGNATURES = {
     'raft_b200_census': (_i, [_vp, _i, _i, _i, _vp, _vp]),
     'raft_b200_unsup_loss': (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, ctypes.c_float, ctypes.c_float, ctypes.c_float,
                                   ctypes.c_float, _vp, _sz, _vp, _vp, _vp]),
+    'raft_b200_unsup_loss_norm': (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, ctypes.c_float, ctypes.c_float,
+                                       ctypes.c_float, ctypes.c_float, _vp, _sz, _vp, _vp, _vp, _vp]),
     'raft_b200_augment_workspace_bytes': (_i, [_vp, _i, _i, ctypes.POINTER(_sz)]),
     'raft_b200_augment_dense': (_i, [_vp, _vp, _i, _vp, _sz, _vp]),
     'raft_b200_augment_sparse': (_i, [_vp, _vp, _i, _vp, _sz, _vp]),

@@ -491,17 +491,18 @@ int raft_b200_census(const float* images, int B, int H, int W, float* out, void*
                 W, out);
 }
 
-int raft_b200_unsup_loss(const float* census_t, const float* census_s, const float* image_t, const uint8_t* occ,
-                         const float* flows, int n, int B, int H, int W, float census_weight, float smoothness_weight,
-                         float edge_weight, float gamma, double* partials, size_t npartials, double* sums, float* grad,
-                         void* stream) {
+int raft_b200_unsup_loss_norm(const float* census_t, const float* census_s, const float* image_t, const uint8_t* occ,
+                              const float* flows, int n, int B, int H, int W, float census_weight,
+                              float smoothness_weight, float edge_weight, float gamma, double* partials,
+                              size_t npartials, double* sums, float* grad, const double* census_norm, void* stream) {
   if (!census_t || !census_s || !image_t || !occ || !flows || !partials || !sums || !grad || npartials < 4)
     return RAFT_ERR_BAD_ARG;
   for (float v : {census_weight, smoothness_weight, edge_weight, gamma})
     if (!(v >= 0.0f && v <= FLT_MAX)) return RAFT_ERR_BAD_ARG;
   if ((reinterpret_cast<uintptr_t>(census_t) | reinterpret_cast<uintptr_t>(census_s)) % 16 ||
       (reinterpret_cast<uintptr_t>(flows) | reinterpret_cast<uintptr_t>(grad)) % sizeof(float2) ||
-      (reinterpret_cast<uintptr_t>(partials) | reinterpret_cast<uintptr_t>(sums)) % sizeof(double))
+      (reinterpret_cast<uintptr_t>(partials) | reinterpret_cast<uintptr_t>(sums) |
+       reinterpret_cast<uintptr_t>(census_norm)) % sizeof(double))
     return RAFT_ERR_BAD_ARG;
   RAFT_TRY(check_dims(B, H, W));
   if (n < 1 || H < 2 || W < 2) return RAFT_ERR_BAD_SHAPE;
@@ -511,7 +512,7 @@ int raft_b200_unsup_loss(const float* census_t, const float* census_s, const flo
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   RAFT_TRY(launch(unsup_mask_count_kernel, blocks, kUnsupThreads, 0, st, occ, B, H, W, partials));
   UnsupParams p;
-  p.ct = census_t; p.cs = census_s; p.img = image_t; p.occ = occ;
+  p.ct = census_t; p.cs = census_s; p.img = image_t; p.occ = occ; p.census_norm = census_norm;
   p.flows = reinterpret_cast<const float2*>(flows); p.grad = reinterpret_cast<float2*>(grad); p.partials = partials;
   p.n = n; p.B = B; p.H = H; p.W = W;
   p.gamma = gamma; p.edge = edge_weight; p.census_half = 0.5f * census_weight;
@@ -520,7 +521,16 @@ int raft_b200_unsup_loss(const float* census_t, const float* census_s, const flo
   p.sv_scale = (float)(0.25 * smoothness_weight / n_v);
   RAFT_TRY(launch(unsup_loss_partial_kernel, blocks, kUnsupThreads, 0, st, p));
   return launch(unsup_loss_final_kernel, 1, kUnsupThreads, 0, st, partials, blocks, n_h, n_v, 0.5 * census_weight,
-                0.5 * smoothness_weight, sums);
+                0.5 * smoothness_weight, census_norm, sums);
+}
+
+int raft_b200_unsup_loss(const float* census_t, const float* census_s, const float* image_t, const uint8_t* occ,
+                         const float* flows, int n, int B, int H, int W, float census_weight, float smoothness_weight,
+                         float edge_weight, float gamma, double* partials, size_t npartials, double* sums, float* grad,
+                         void* stream) {
+  return raft_b200_unsup_loss_norm(census_t, census_s, image_t, occ, flows, n, B, H, W, census_weight,
+                                   smoothness_weight, edge_weight, gamma, partials, npartials, sums, grad, nullptr,
+                                   stream);
 }
 
 // Checks every sample of an augmentation call and lays out its workspace: fills (fill) or verifies each ws_offset.

@@ -4,7 +4,8 @@
 //
 //   census_kernel              images (B, H, W, 3) in 0..255 -> (B, H, W, 48) census features, every operation an
 //                              explicitly rounded fp32 one (NumPy float32 reproduces each bit, oracle/unsup_np.py)
-//   unsup_mask_count_kernel    per CTA of the loss kernel's grid: its pixels' mask count (for the census normaliser)
+//   unsup_mask_count_kernel    per CTA of the loss kernel's grid: its pixels' mask count (the census normaliser unless
+//                              the caller supplies one)
 //   unsup_loss_partial_kernel  one thread per pixel, all n predictions: the gradient of the direction's share of the loss
 //                              and per-CTA fp64 partial sums in a fixed order
 //   unsup_loss_final_kernel    one CTA: the partials added in index order, the normalised terms
@@ -113,6 +114,7 @@ struct UnsupParams {
   float2* grad;            // (n, B, H, W) d(direction's loss share) / d flows
   double* partials;        // 3 per CTA: census, horizontal and vertical smoothness sums, gamma-weighted; then one mask
                            // count per CTA (unsup_mask_count_kernel)
+  const double* census_norm;  // NULL: max(mask count, 1); else the caller's normaliser (> 0), e.g. of a global batch
   int n, B, H, W;
   double gamma;
   float edge;              // lambda of the edge weight
@@ -135,7 +137,8 @@ __global__ void __launch_bounds__(kUnsupThreads) unsup_loss_partial_kernel(const
   const int H = P.H, W = P.W;
   const size_t hw = (size_t)H * W, npix = (size_t)P.B * hw;
   const float xmax = (float)(W - 1), ymax = (float)(H - 1);
-  const float census_scale = (float)(P.census_half / fmax(unsup_mask_total(P.partials, gridDim.x), 1.0));
+  const double norm = P.census_norm ? *P.census_norm : fmax(unsup_mask_total(P.partials, gridDim.x), 1.0);
+  const float census_scale = (float)(P.census_half / norm);
   double acc[3] = {0.0, 0.0, 0.0};
   for (size_t p = blockIdx.x * (size_t)kUnsupThreads + threadIdx.x; p < npix; p += (size_t)gridDim.x * kUnsupThreads) {
     const size_t bi = p / hw, q = p % hw;
@@ -229,11 +232,14 @@ __global__ void __launch_bounds__(kUnsupThreads) unsup_loss_partial_kernel(const
     for (int k = 0; k < 3; ++k) P.partials[(size_t)blockIdx.x * 3 + k] = acc[k];
 }
 
-// One CTA.  sums[2] = mask count, sums[0] = L_c = census sum / max(count, 1); sums[1] = L_s = (S_h + S_v) / 2 with S_h, S_v the smoothness
-// sums over the numbers of pairs; sums[3] = census_weight / 2 * L_c + smoothness_weight / 2 * L_s.
+// One CTA.  sums[2] = mask count, sums[0] = L_c = census sum / norm, norm = *census_norm or max(count, 1); sums[1] = L_s =
+// (S_h + S_v) / 2 with S_h, S_v the smoothness sums over the numbers of pairs; sums[3] = census_weight / 2 * L_c +
+// smoothness_weight / 2 * L_s.
 __global__ void __launch_bounds__(kUnsupThreads) unsup_loss_final_kernel(const double* __restrict__ partials, int nblocks,
                                                                          double n_h, double n_v, double census_half,
-                                                                         double smooth_half, double* __restrict__ sums) {
+                                                                         double smooth_half,
+                                                                         const double* __restrict__ census_norm,
+                                                                         double* __restrict__ sums) {
   const double count = unsup_mask_total(partials, nblocks);
   double v[3] = {0.0, 0.0, 0.0};
   for (int c = threadIdx.x; c < nblocks; c += kUnsupThreads)
@@ -241,7 +247,7 @@ __global__ void __launch_bounds__(kUnsupThreads) unsup_loss_final_kernel(const d
     for (int k = 0; k < 3; ++k) v[k] = __dadd_rn(v[k], partials[(size_t)c * 3 + k]);
   unsup_block_sum(v);
   if (threadIdx.x == 0) {
-    const double lc = v[0] / fmax(count, 1.0);
+    const double lc = v[0] / (census_norm ? *census_norm : fmax(count, 1.0));
     const double ls = (v[1] / n_h + v[2] / n_v) / 2.0;
     sums[0] = lc;
     sums[1] = ls;

@@ -1,6 +1,7 @@
 """Losses / metrics -- host-side mirror of tf_raft/losses/losses.py (torch elementwise ops; not on
 the hot path).  `y_true = (flow_gt, valid)`, predictions NHWC.  UnsupervisedLoss, an addition, runs in CUDA."""
 import torch
+import torch.distributed as dist
 
 from . import _lib
 from .layers.corr import fb_occlusion
@@ -94,6 +95,12 @@ class UnsupervisedLoss:
     loss and its gradient with respect to every prediction come from one CUDA pass per direction
     (raft_b200_unsup_loss, DESIGN.md section 9.1), deterministic: two calls on the same inputs give the same bits.
 
+    Under torch.distributed with R ranks, each holding an equal shard of the batch, the census sums of every rank are
+    normalised by the mask count C of the whole batch (one all-reduce of the two directions' counts): rank r's loss is
+    census_weight (sum_{x in r} m rho) R / max(C, 1) / 2 per direction plus its smoothness share, so the mean of the
+    ranks' losses is the whole batch's loss and the gradients summed over the ranks and divided by R are the whole
+    batch's gradient.
+
     The defaults are untuned starting values, not settings validated on any dataset.  `compile(loss=UnsupervisedLoss())`
     makes `train_step` run the bidirectional training graph on (image1, image2[, flow, valid]) batches."""
 
@@ -118,6 +125,12 @@ class UnsupervisedLoss:
             occ = torch.cat(fb_occlusion(preds_fw[-1].detach(), preds_bw[-1].detach(), self.alpha1, self.alpha2))
             images = torch.cat([image1, image2]).to(torch.float32).contiguous()
             census = census_transform(images)
+            census_norm = None
+            if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
+                h, w = occ.shape[1:]                                           # m: not occluded, 3 px inside the frame
+                counts = (~occ[:, 3:h - 3, 3:w - 3]).reshape(2, -1).sum(1).to(torch.float64)
+                dist.all_reduce(counts)                                          # the whole batch's (fw, bw) counts
+                census_norm = counts.clamp(min=1.0) / dist.get_world_size()
         flows = torch.stack(preds_fw + preds_bw)                                 # (2n, B, H, W, 2)
-        return train._UnsupLoss.apply(flows, census, images, occ, self.census_weight, self.smoothness_weight,
-                                      self.edge_weight, self.gamma)
+        args = (flows, census, images, occ, self.census_weight, self.smoothness_weight, self.edge_weight, self.gamma)
+        return train._UnsupLoss.apply(*args, *(() if census_norm is None else (census_norm,)))

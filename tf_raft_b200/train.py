@@ -375,12 +375,13 @@ class _UnsupLoss(torch.autograd.Function):
     backward = that gradient scaled by grad_output.
 
     flows (2n, B, H, W, 2): the n forward predictions, then the n backward ones; census (2B, H, W, 48) and images
-    (2B, H, W, 3): [image1; image2]; occ (2B, H, W) bool: [occ_fw; occ_bw]."""
+    (2B, H, W, 3): [image1; image2]; occ (2B, H, W) bool: [occ_fw; occ_bw]; census_norm: None (each direction divides
+    its census sum by max(its mask count, 1)) or a device float64 (2,) tensor of the two directions' normalisers."""
 
     NPARTIALS = 4 * 1024              # fp64 scratch of a call: 4 per CTA (fixed, so that every call reduces alike)
 
     @staticmethod
-    def forward(ctx, flows, census, images, occ, census_weight, smoothness_weight, edge_weight, gamma):
+    def forward(ctx, flows, census, images, occ, census_weight, smoothness_weight, edge_weight, gamma, census_norm=None):
         flows = flows.contiguous()
         n2, b, h, w, _ = flows.shape
         n = n2 // 2
@@ -390,10 +391,10 @@ class _UnsupLoss(torch.autograd.Function):
         sums = torch.empty((2, 4), dtype=torch.float64, device=flows.device)
         for d in range(2):                                     # d = 0: image1 -> image2, d = 1: image2 -> image1
             t, s = slice(d * b, (d + 1) * b), slice((1 - d) * b, (2 - d) * b)
-            _lib.call('unsup_loss', flows.device, _lib.ptr(census[t]), _lib.ptr(census[s]), _lib.ptr(images[t]),
+            _lib.call('unsup_loss_norm', flows.device, _lib.ptr(census[t]), _lib.ptr(census[s]), _lib.ptr(images[t]),
                       _lib.ptr(occ[t]), _lib.ptr(flows[d * n:(d + 1) * n]), n, b, h, w, census_weight,
                       smoothness_weight, edge_weight, gamma, _lib.ptr(partials), partials.numel(), _lib.ptr(sums[d]),
-                      _lib.ptr(grad[d * n:(d + 1) * n]))
+                      _lib.ptr(grad[d * n:(d + 1) * n]), _lib.ptr(None if census_norm is None else census_norm[d]))
         ctx.save_for_backward(grad)
         ctx.terms = sums                                       # [direction][L_c, L_s, mask count, share of the loss]
         return (sums[0, 3] + sums[1, 3]).to(torch.float32)
@@ -401,7 +402,7 @@ class _UnsupLoss(torch.autograd.Function):
     @staticmethod
     def backward(ctx, grad_out):
         (grad,) = ctx.saved_tensors
-        return grad * grad_out, None, None, None, None, None, None, None
+        return grad * grad_out, None, None, None, None, None, None, None, None
 
 
 def _all_reduce_sum(x):
