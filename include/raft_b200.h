@@ -464,6 +464,31 @@ int raft_b200_encode_pair(int variant, const void* fnet_prepared, int fnet_norm,
 int raft_b200_conv2d(const float* x, const float* kernel, const float* bias, int B, int H, int W, int cin, int kh,
                      int kw, int cout, int act, float* out, int out_stride, int out_c0, void* stream);
 
+/* Tensor-core convolutions of the training step (RAFT.compile(train_precision='f16x2')): a stride-1 Conv2D with odd
+ * kh, kw <= 7 and symmetric 'same' padding ((kh-1)/2, (kw-1)/2; a 1x1 'valid' convolution is the 1x1 case), 16 <= cin
+ * <= 1024, 1 <= cout <= 1024, B*H*W < 2^31 (RAFT_ERR_BAD_SHAPE otherwise).  NHWC fp32 activations, HWIO fp32 kernel, fp16
+ * hi/lo three-pass arithmetic with IEEE-fp32 promotion (DESIGN.md section 9).
+ *
+ * Workspace: with workspace == NULL either call writes the bytes the shape needs to *workspace_bytes and runs nothing;
+ * otherwise *workspace_bytes is the buffer's size (RAFT_ERR_WORKSPACE if smaller).  One buffer of that size serves the
+ * forward and the backward of a shape.  x_planes and workspace 256-byte aligned, out and grad_x 32-byte aligned
+ * (RAFT_ERR_BAD_ARG otherwise).
+ *
+ * forward: out (B,H,W,cout) = conv(x (B,H,W,cin)) + bias.  Writes x_planes, what the backward reads of x: the fp16
+ * hi/lo split of x * 2^k_x (hi plane, then lo plane, B*H*W * round_up(cin, 64) halves each; max finite |x| * 2^k_x in
+ * [2^12, 2^13), k_x in [-100, 100]) followed by 256 bytes holding the scale: 4 * B*H*W * round_up(cin, 64) + 256 bytes.
+ * backward: from x_planes and grad_out (B,H,W,cout): grad_kernel (kh,kw,cin,cout) and, unless grad_x is NULL, grad_x
+ * (B,H,W,cin).  grad_out is scaled by 2^k_g before its split, max finite |grad_out| * 2^k_g in [2^12, 2^13), k_g in
+ * [-100, 100]; a NaN or inf in grad_out or x makes every output whose sum includes it NaN, and no other (image
+ * edges included).  The weight gradient adds
+ * per-slice partial sums in a fixed order (slices depend on the shape only; no atomics): two calls give the same bits. */
+int raft_b200_conv_tc_forward(const float* x, const float* kernel, const float* bias, int B, int H, int W, int cin, int kh,
+                              int kw, int cout, float* out, void* x_planes, void* workspace, size_t* workspace_bytes,
+                              void* stream);
+int raft_b200_conv_tc_backward(const void* x_planes, const float* kernel, const float* grad_out, int B, int H, int W,
+                               int cin, int kh, int kw, int cout, float* grad_x, float* grad_kernel, void* workspace,
+                               size_t* workspace_bytes, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Model loop  (tf_raft/model.py)
  * ------------------------------------------------------------------------------------------- */

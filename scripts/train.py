@@ -62,7 +62,7 @@ def need(config, path):
     return node
 
 
-def train(name, config, logdir, small=False, workers=4, self_supervised=False):
+def train(name, config, logdir, small=False, workers=4, self_supervised=False, train_precision='fp32'):
     root = need(config, 'data.root')
     aug_params = need(config, 'augment')
     iters, iters_pred, resume = (need(config, 'model.' + k) for k in ('iters', 'iters_pred', 'resume'))
@@ -95,7 +95,8 @@ def train(name, config, logdir, small=False, workers=4, self_supervised=False):
     optimizer = T.AdamW(weight_decay=weight_decay, learning_rate=scheduler)
     raft = (T.SmallRAFT if small else T.RAFT)(drop_rate=0, iters=iters, iters_pred=iters_pred)
     loss = T.UnsupervisedLoss() if self_supervised else T.sequence_loss
-    raft.compile(optimizer=optimizer, clip_norm=clip_norm, loss=loss, epe=T.end_point_error)
+    raft.compile(optimizer=optimizer, clip_norm=clip_norm, loss=loss, epe=T.end_point_error,
+                 train_precision=train_precision)
     if resume:
         print(f'Restoring pretrained weights from {resume} ...', end=' ')
         raft.load_weights(resume)
@@ -121,6 +122,8 @@ def main():
     parser.add_argument('--small', action='store_true', help='SmallRAFT instead of RAFT')
     parser.add_argument('--seed', type=int, default=None, help='seed np.random and random before the first shuffle')
     parser.add_argument('--workers', type=int, default=4, help='loader threads')
+    parser.add_argument('--train-precision', choices=('fp32', 'f16x2'), default='fp32',
+                        help="convolutions of the step: IEEE-fp32 library (fp32) or tensor-core hi/lo (f16x2)")
     parser.add_argument('--self-supervised', action='store_true',
                         help='train with UnsupervisedLoss (census + smoothness, both directions) instead of ground truth')
     args = parser.parse_args()
@@ -138,7 +141,8 @@ def main():
     if args.seed is not None:
         np.random.seed(args.seed)
         random.seed(args.seed)
-    train(args.dataset, config, logdir, small=args.small, workers=args.workers, self_supervised=args.self_supervised)
+    train(args.dataset, config, logdir, small=args.small, workers=args.workers, self_supervised=args.self_supervised,
+          train_precision=args.train_precision)
 
 
 if __name__ == '__main__':

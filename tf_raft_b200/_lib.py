@@ -108,6 +108,10 @@ _SIGNATURES = {
     'raft_b200_encode_pair': (_i, [_i, _vp, _i, _i, _vp, _i, _i, _i, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _sz,
                                    _vp]),
     'raft_b200_conv2d': (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _vp]),
+    'raft_b200_conv_tc_forward': (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, ctypes.POINTER(_sz),
+                                       _vp]),
+    'raft_b200_conv_tc_backward': (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, ctypes.POINTER(_sz),
+                                        _vp]),
     'raft_b200_forward_loop': (_i, [_i, _vp, ctypes.POINTER(_vp), _i, _i, _vp, _vp, _vp, ctypes.POINTER(_vp), _i,
                                     _i, _i, _i, _vp, _sz, _i, _vp]),
 }

@@ -8,6 +8,7 @@
 #include <algorithm>
 
 #include "augment.cuh"
+#include "conv_train.cuh"
 #include "corr_tc.cuh"
 #include "dataset.cuh"
 #include "encoder.cuh"
@@ -936,6 +937,39 @@ int raft_b200_forward_loop(int variant, const void* prepared, const float* const
     }
   }
   return raft_launch_status();
+}
+
+// Training convolutions (conv_train.cuh).  workspace == null: *workspace_bytes = the size the shape needs, nothing runs.
+static int conv_train_prologue(int B, int H, int W, int cin, int kh, int kw, int cout, const void* planes, const void* ws,
+                               size_t* ws_bytes, ConvTrainLayout& L) {
+  if (!ws_bytes) return RAFT_ERR_BAD_ARG;
+  RAFT_TRY(conv_train_check(B, H, W, cin, kh, kw, cout));
+  RAFT_TRY(conv_train_layout(B, H, W, cin, kh, kw, cout, L));
+  if (!ws) return RAFT_OK;
+  if (!planes || (reinterpret_cast<uintptr_t>(planes) | reinterpret_cast<uintptr_t>(ws)) % 256) return RAFT_ERR_BAD_ARG;
+  return *ws_bytes < L.total ? RAFT_ERR_WORKSPACE : RAFT_OK;
+}
+
+int raft_b200_conv_tc_forward(const float* x, const float* kernel, const float* bias, int B, int H, int W, int cin, int kh,
+                              int kw, int cout, float* out, void* x_planes, void* workspace, size_t* workspace_bytes,
+                              void* stream) {
+  ConvTrainLayout L;
+  RAFT_TRY(conv_train_prologue(B, H, W, cin, kh, kw, cout, x_planes, workspace, workspace_bytes, L));
+  if (!workspace) { *workspace_bytes = L.total; return RAFT_OK; }
+  if (!x || !kernel || !bias || !out || reinterpret_cast<uintptr_t>(out) % 32) return RAFT_ERR_BAD_ARG;
+  return conv_train_forward(x, kernel, bias, B, H, W, cin, kh, kw, cout, out, static_cast<__half*>(x_planes),
+                            static_cast<uint8_t*>(workspace), L, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int raft_b200_conv_tc_backward(const void* x_planes, const float* kernel, const float* grad_out, int B, int H, int W,
+                               int cin, int kh, int kw, int cout, float* grad_x, float* grad_kernel, void* workspace,
+                               size_t* workspace_bytes, void* stream) {
+  ConvTrainLayout L;
+  RAFT_TRY(conv_train_prologue(B, H, W, cin, kh, kw, cout, x_planes, workspace, workspace_bytes, L));
+  if (!workspace) { *workspace_bytes = L.total; return RAFT_OK; }
+  if (!kernel || !grad_out || !grad_kernel || (grad_x && reinterpret_cast<uintptr_t>(grad_x) % 32)) return RAFT_ERR_BAD_ARG;
+  return conv_train_backward(static_cast<const __half*>(x_planes), kernel, grad_out, B, H, W, cin, kh, kw, cout, grad_x,
+                             grad_kernel, static_cast<uint8_t*>(workspace), L, reinterpret_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -646,9 +646,10 @@ struct TcCinMap { int nrange, src0[2], n[2], dst0[2]; };
 // Writes slot `s` of the zeroed blob at `base` from nsrc (1 or 2) HWIO convolutions, concatenated along cout.
 // cin_map == null keeps the channels where they are.  flatten: each source runs as a 1x1 convolution over its
 // kh * kw * cin window channels (HWIO is already [tap * cin + c][cout]), for layers fed by im2col planes.  The scale is
-// shared by the sources: it comes from the absmax over all of them.
+// shared by the sources: it comes from the absmax over all of them.  rot: the input-gradient form of one source (see
+// PackParams::rot; the slot's cout_pad covers the source cin, its cin_pad the source cout); a null bias is not copied.
 inline int tc_pack_weights(uint8_t* base, const TcWeightSlot& s, const raft_conv* const src[], int nsrc,
-                           const TcCinMap* cin_map, bool flatten, cudaStream_t st) {
+                           const TcCinMap* cin_map, bool flatten, cudaStream_t st, bool rot = false) {
   unsigned int* amax = reinterpret_cast<unsigned int*>(base + s.absmax);
   float* scale = reinterpret_cast<float*>(base + s.scale);
   for (int i = 0; i < nsrc; ++i) {
@@ -675,9 +676,11 @@ inline int tc_pack_weights(uint8_t* base, const TcWeightSlot& s, const raft_conv
       pp.r_dst0[r] = m.dst0[r];
     }
     pp.scale = scale;
+    pp.rot = rot ? 1 : 0;
     RAFT_TRY(launch(pack_weights_kernel, grid_for((size_t)cv.kh * cv.kw * cv.cin * cv.cout), 256, 0, st, pp));
-    RAFT_CUDA_TRY(cudaMemcpyAsync(base + s.bias + cout_off * sizeof(float), cv.bias, cv.cout * sizeof(float),
-                                  cudaMemcpyDeviceToDevice, st));
+    if (cv.bias)
+      RAFT_CUDA_TRY(cudaMemcpyAsync(base + s.bias + cout_off * sizeof(float), cv.bias, cv.cout * sizeof(float),
+                                    cudaMemcpyDeviceToDevice, st));
     cout_off += cv.cout;
   }
   return RAFT_OK;

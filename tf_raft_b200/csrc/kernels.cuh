@@ -500,6 +500,8 @@ struct PackParams {
   __half* hi; __half* lo; int cout_pad, cin_pad, cout_off;
   int r_src0[2], r_n[2], r_dst0[2], nrange;     // cin remap ranges
   const float* scale;                           // scale[0] = 2^k
+  int rot;                                      // 1: the input-gradient form -- taps rotated 180 deg, cin and cout
+                                                //    swapped (packed row = source cin, column = source cout); no remap
 };
 __global__ void pack_weights_kernel(const PackParams p) {
   const size_t total = (size_t)p.kh * p.kw * p.cin * p.cout;
@@ -510,6 +512,14 @@ __global__ void pack_weights_kernel(const PackParams p) {
     t /= p.cout;
     const int c = (int)(t % p.cin);
     const int tap = (int)(t / p.cin);
+    if (p.rot) {                                // rotating both kh and kw reverses the flat tap index
+      __half hh, ll;
+      split_f16(p.w[i] * s, hh, ll);
+      const size_t o = ((size_t)(p.kh * p.kw - 1 - tap) * p.cout_pad + c) * p.cin_pad + n;
+      p.hi[o] = hh;
+      p.lo[o] = ll;
+      continue;
+    }
     int cd = -1;
     for (int r = 0; r < p.nrange; ++r)
       if (c >= p.r_src0[r] && c < p.r_src0[r] + p.r_n[r]) cd = p.r_dst0[r] + (c - p.r_src0[r]);

@@ -40,6 +40,7 @@ class RAFT:
         self._pair_ws = _lib.WorkspaceCache()
         self.flow_metrics = None
         self.optimizer = None
+        self.train_precision = 'fp32'
         self._trainer = None
         self._params_stale = False
         self._pending_slots = None                         # optimiser state of load_weights awaiting the Trainer
@@ -417,7 +418,16 @@ class RAFT:
     call = __call__
 
     # -- keras-style steps (model.py:111-170) ---------------------------------------------------
-    def compile(self, optimizer=None, clip_norm=None, loss=sequence_loss, epe=end_point_error, **kwargs):
+    def compile(self, optimizer=None, clip_norm=None, loss=sequence_loss, epe=end_point_error, train_precision='fp32',
+                **kwargs):
+        """train_precision: 'fp32' (IEEE-fp32 library convolutions) or 'f16x2' (the training step's stride-1
+        convolutions with cin >= 64 forward and backward on the tensor cores, fp16 hi/lo three-pass; DESIGN.md section 9)."""
+        from .train import TRAIN_PRECISIONS
+        if train_precision not in TRAIN_PRECISIONS:
+            raise ValueError(f'unknown train_precision {train_precision!r}; expected one of {", ".join(TRAIN_PRECISIONS)}')
+        self.train_precision = train_precision
+        if self._trainer is not None:
+            self._trainer.graph.train_precision = train_precision
         self.optimizer = optimizer
         self.clip_norm = clip_norm
         self.loss = loss

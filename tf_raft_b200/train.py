@@ -13,9 +13,12 @@ What runs where (DESIGN.md "Training"):
   per-channel batch statistics of the context encoder's BatchNorm layers all-reduced in forward and backward (SyncBN:
   the single-device reference normalises over the global batch);
 * convolutions, norms, gates, convex upsampling and the loss in the backward-capable form: IEEE-fp32 PyTorch CUDA kernels
-  through torch.autograd, with cuDNN switched off for the step (see Trainer.step) -- library code, stated as such; the
-  hand-written tensor-core kernels are forward-only.
+  through torch.autograd, with cuDNN switched off for the step (see Trainer.step) -- library code, stated as such;
+* with `compile(train_precision='f16x2')`, every stride-1 convolution with cin >= 64 and 'same' (or 1x1 'valid') padding
+  runs forward, input gradient and weight gradient on hand-written tensor-core kernels instead (_ConvTC); the rest of
+  the list above is unchanged.
 """
+import ctypes
 import math
 import os
 import socket
@@ -405,6 +408,49 @@ class _UnsupLoss(torch.autograd.Function):
         return grad * grad_out, None, None, None, None, None, None, None, None
 
 
+TRAIN_PRECISIONS = ('fp32', 'f16x2')
+
+
+class _ConvTC(torch.autograd.Function):
+    """A stride-1 Conv2D with odd, symmetric 'same' padding on the tensor cores (raft_b200_conv_tc_forward / _backward):
+    x (B, cin, H, W) as a view of NHWC memory (torch.channels_last, read without a transpose), kernel HWIO, bias (cout,).
+    The forward keeps the fp16 hi/lo planes of x for the backward, not x; the backward writes the kernel gradient and,
+    when x needs one, the input gradient; the bias gradient is a torch reduction."""
+
+    @staticmethod
+    def forward(ctx, x, kernel, bias, workspaces):
+        b, cin, h, w = x.shape
+        kh, kw, _, cout = kernel.shape
+        dims = (b, h, w, cin, kh, kw, cout)
+        ws = workspaces.get(dims)
+        if ws is None:
+            need = ctypes.c_size_t()
+            _lib.call('conv_tc_forward', x.device, None, None, None, *dims, None, None, None, ctypes.byref(need))
+            ws = workspaces[dims] = _lib.workspace(need.value, x.device)
+        x_nhwc = x.permute(0, 2, 3, 1).contiguous()
+        kernel = kernel.detach().contiguous()
+        planes = torch.empty(2 * b * h * w * ((cin + 63) // 64 * 64) + 128, dtype=torch.float16, device=x.device)
+        out = torch.empty((b, h, w, cout), dtype=torch.float32, device=x.device)
+        _lib.call('conv_tc_forward', x.device, _lib.ptr(x_nhwc), _lib.ptr(kernel), _lib.ptr(bias.detach().contiguous()),
+                  *dims, _lib.ptr(out), _lib.ptr(planes), _lib.ptr(ws), ctypes.byref(ctypes.c_size_t(ws.numel())))
+        ctx.save_for_backward(kernel)
+        ctx.planes, ctx.ws, ctx.dims = planes, ws, dims
+        return out.permute(0, 3, 1, 2)
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        (kernel,) = ctx.saved_tensors
+        b, h, w, cin, kh, kw, cout = ctx.dims
+        g = grad_out.permute(0, 2, 3, 1).contiguous()
+        grad_x = torch.empty((b, h, w, cin), dtype=torch.float32, device=g.device) if ctx.needs_input_grad[0] else None
+        grad_kernel = torch.empty_like(kernel)
+        _lib.call('conv_tc_backward', g.device, _lib.ptr(ctx.planes), _lib.ptr(kernel), _lib.ptr(g), *ctx.dims,
+                  _lib.ptr(grad_x), _lib.ptr(grad_kernel), _lib.ptr(ctx.ws), ctypes.byref(ctypes.c_size_t(ctx.ws.numel())))
+        grad_bias = g.sum(dim=(0, 1, 2)) if ctx.needs_input_grad[2] else None
+        ctx.planes = None
+        return None if grad_x is None else grad_x.permute(0, 3, 1, 2), grad_kernel, grad_bias, None
+
+
 def _all_reduce_sum(x):
     """differentiable all-reduce (sum) over the default process group; identity without one."""
     if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
@@ -417,13 +463,20 @@ class TrainGraph:
     """The forward of model.py:68-109 / 190-226 with `training=True` in backward-capable form, on leaf parameters `P`
     (HWIO kernels, reference attribute paths).  NCHW inside, NHWC at the interface."""
 
-    def __init__(self, P, variant, precision, moving):
+    def __init__(self, P, variant, precision, moving, train_precision='fp32'):
         self.P, self.variant, self.precision, self.moving = P, variant, precision, moving
+        self.train_precision = train_precision
+        self._conv_ws = {}                              # _ConvTC workspaces by shape
         self.cfg = dict(raft=dict(hidden=128, context=128, levels=4, radius=4, fnorm='instance', cnorm='batch'),
                         small=dict(hidden=96, context=64, levels=4, radius=3, fnorm='instance', cnorm=None))[variant]
 
     # -- primitives --
     def conv(self, x, name, stride=1, padding='same'):
+        if self.train_precision == 'f16x2':
+            return self._conv_f16x2(x, name, stride, padding)
+        return self._conv_lib(x, name, stride, padding)
+
+    def _conv_lib(self, x, name, stride, padding):
         w = self.P[name + '.kernel'].permute(3, 2, 0, 1)
         if padding == 'same':
             pt, pb = _same_pads(x.shape[2], w.shape[2], stride)
@@ -431,6 +484,18 @@ class TrainGraph:
             if pt or pb or pl or pr:
                 x = F.pad(x, (pl, pr, pt, pb))
         return F.conv2d(x, w, self.P[name + '.bias'], stride=stride)
+
+    def _conv_f16x2(self, x, name, stride, padding):
+        """train_precision='f16x2': stride 1, 'same' (odd kernel) or 1x1 'valid', cin >= 64 on the tensor cores; convf1
+        (cin 2), SmallRAFT's 32-channel first stage, the stems and the stride-2 convolutions on the library, their outputs
+        put back into channels_last.  A 32-channel layer would fill half of the one 64-channel chunk it is padded to, and
+        its weight gradients, behind an instance norm at the full resolution of SmallRAFT's first stage, leave the
+        IEEE-fp32 gradient gates of the step on the three-pass split (DESIGN.md section 9.0)."""
+        kernel = self.P[name + '.kernel']
+        kh, kw, cin, _ = kernel.shape
+        if stride == 1 and cin >= 64 and kh % 2 == 1 and kw % 2 == 1 and (padding == 'same' or kh == kw == 1):
+            return _ConvTC.apply(x, kernel, self.P[name + '.bias'], self._conv_ws)
+        return self._conv_lib(x, name, stride, padding).contiguous(memory_format=torch.channels_last)
 
     def norm(self, x, name, norm_type):
         eps = 1e-3
@@ -572,7 +637,7 @@ class Trainer:
         sd = model.state_dict()
         self.flat = FlatState(sd, lambda k: not (k.endswith('.moving_mean') or k.endswith('.moving_variance')))
         self.moving = {k: v.clone() for k, v in sd.items() if k.endswith('.moving_mean') or k.endswith('.moving_variance')}
-        self.graph = TrainGraph(self.flat.views, self.variant, model.precision, self.moving)
+        self.graph = TrainGraph(self.flat.views, self.variant, model.precision, self.moving, model.train_precision)
         self.world = dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
 
     def params(self):
