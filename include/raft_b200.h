@@ -92,7 +92,15 @@ int raft_b200_corr_lookup(const float* const pyr[], const float* coords, int B, 
 /* Backward of CorrBlock.retrieve for the training step (tf_raft/model.py:133: tape.gradient through corr.py:116-152;
  * the reference does not detach coords1, model.py:102).  grad_out (B, h, w, levels*(2r+1)^2) -> grad_coords (B, h, w, 2)
  * and grad_pyr[l] (same shapes as pyr[l]); both outputs are ACCUMULATED into (zero them first).  TensorFlow gradient
- * rules: floor / ceil / indices carry no gradient, clip_by_value passes it inside [0, dim-1].                        */
+ * rules: floor / ceil / indices carry no gradient, clip_by_value passes it inside [0, dim-1]; terms with a zero
+ * grad_out, and pyramid terms with a zero bilinear weight, are skipped.
+ * Deterministic: no atomics, and every sum has a fixed order that depends on the shape and the data only, with each
+ * operation one rounded fp32 operation (no FMA).  With t = a*(2r+1) + b:
+ *   grad_pyr : a touched cell ends as in + term_1 + term_2 + ... left to right, terms fl(fl(wy*wx) * grad_out) in
+ *              ascending t (then corner 00, 01, 10, 11); cells no term reaches are not written;
+ *   grad_coords : per level l, 32 lane sums (lane j adds taps j, j+32, ... in order, from +0) combined by the xor
+ *              butterfly with strides 16, 8, 4, 2, 1 give G_l; grad_coords ends as in + fl(G_0 * 2^0) + fl(G_1 * 2^-1)
+ *              + ... in ascending level.  Two calls on the same inputs give the same bits (DESIGN.md section 9).  */
 int raft_b200_corr_lookup_backward(const float* const pyr[], const float* coords, const float* grad_out, int B, int h, int w,
                                    int levels, int radius, float* grad_coords, float* const grad_pyr[], void* stream);
 
@@ -500,6 +508,16 @@ int raft_b200_upsample_convex(const float* flow, const float* mask, int B, int h
 
 /* upflow8(flow): corr.py:93-96 = 8 * bilinear resize with half-pixel centres.                    */
 int raft_b200_upflow8(const float* flow, int B, int h, int w, float* out, void* stream);
+
+/* Backward of F.interpolate(scale_factor=8, mode='bilinear', align_corners=False), the upsampling of SmallRAFT's
+ * training graph (without upflow8's factor 8).  grad_up (B, 8h, 8w, 2) -> grad_flow (B, h, w, 2), WRITTEN (not
+ * accumulated); both 8-byte aligned (RAFT_ERR_BAD_ARG otherwise).  PyTorch's upsample_bilinear2d weights: per output
+ * coordinate X of an axis of n input cells, src = max(0.125 (X + 0.5) - 0.5, 0), i0 = (int)src, i1 = i0 + (i0 < n-1),
+ * l1 = src - i0, l0 = 1 - l1; y likewise.  Every output pixel contributes to all four of its corners, zero weights
+ * included (so NaN reaches the cells PyTorch's backward gives it), term fl(fl(ly * lx) * grad_up).  Deterministic, no
+ * atomics: a cell is +0 + its terms, added left to right in ascending output pixel (row-major), then corner 00, 01, 10,
+ * 11, each operation one rounded fp32 operation.                                                                      */
+int raft_b200_upflow8_backward(const float* grad_up, int B, int h, int w, float* grad_flow, void* stream);
 
 /* The iteration loop of RAFT.call / SmallRAFT.call: model.py:93-106 / :212-224.
  *   for i < iters:  corr = retrieve(coords1); flow = coords1 - coords0;

@@ -99,6 +99,7 @@ _SIGNATURES = {
     'raft_b200_update_small': (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _sz, _i, _vp]),
     'raft_b200_upsample_convex': (_i, [_vp, _vp, _i, _i, _i, _vp, _vp]),
     'raft_b200_upflow8': (_i, [_vp, _i, _i, _i, _vp, _vp]),
+    'raft_b200_upflow8_backward': (_i, [_vp, _i, _i, _i, _vp, _vp]),
     'raft_b200_encoder_prepared_bytes': (_i, [_i, _i, ctypes.POINTER(_sz)]),
     'raft_b200_encoder_prepare': (_i, [_i, _i, _i, _vp, _vp, _sz, _vp]),
     'raft_b200_encoder_workspace_bytes': (_i, [_i, _i, _i, _i, ctypes.POINTER(_sz)]),

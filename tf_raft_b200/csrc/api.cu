@@ -425,8 +425,9 @@ int raft_b200_corr_lookup_backward(const float* const pyr[], const float* coords
   const int side = 2 * radius + 1;
   p.coords = coords; p.gout = grad_out; p.gout_stride = levels * side * side; p.gcoords = grad_coords;
   p.nq = B * h * w; p.levels = levels; p.radius = radius;
-  const size_t nwork = (size_t)p.nq * levels;
-  return launch(corr_lookup_bwd_kernel, grid_for(nwork * 32, 256, kNumSMs * 32), 256, 0, reinterpret_cast<cudaStream_t>(stream), p);
+  const int qpb = lookup_bwd_queries_per_block(levels);
+  return launch(corr_lookup_bwd_kernel, grid_for((size_t)p.nq, qpb, kNumSMs * 32), 32 * levels * qpb, 0,
+                reinterpret_cast<cudaStream_t>(stream), p);
 }
 
 int raft_b200_sumsq(const float* g, size_t n, float* partials, size_t npartials, float* out, void* stream) {
@@ -773,6 +774,14 @@ int raft_b200_upflow8(const float* flow, int B, int h, int w, float* out, void* 
   RAFT_TRY(check_dims(B, h, w));
   return launch(upflow8_kernel, grid_for((size_t)B * h * w * 64), 256, 0, reinterpret_cast<cudaStream_t>(stream), flow, B, h,
                 w, out);
+}
+
+int raft_b200_upflow8_backward(const float* grad_up, int B, int h, int w, float* grad_flow, void* stream) {
+  if (!grad_up || !grad_flow || (reinterpret_cast<uintptr_t>(grad_up) & 7) || (reinterpret_cast<uintptr_t>(grad_flow) & 7))
+    return RAFT_ERR_BAD_ARG;
+  RAFT_TRY(check_dims(B, h, w));
+  return launch(upflow8_bwd_kernel, grid_for((size_t)B * h * w, 128), 128, 0, reinterpret_cast<cudaStream_t>(stream),
+                grad_up, B, h, w, grad_flow);
 }
 
 int raft_b200_encoder_prepared_bytes(int variant, int out_dim, size_t* bytes) {

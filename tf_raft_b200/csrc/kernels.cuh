@@ -467,6 +467,65 @@ __global__ void upflow8_kernel(const float* __restrict__ flow, int B, int h, int
   }
 }
 
+// Backward of the training graph's F.interpolate(scale_factor=8, mode='bilinear', align_corners=False) (SmallRAFT's
+// upsampling), with PyTorch upsample_bilinear2d's source indices and weights.  Per output coordinate X of an input axis
+// of n cells: src = max(0.125 * (X + 0.5) - 0.5, 0), i0 = (int)src, i1 = i0 + (i0 < n - 1), l1 = src - i0, l0 = 1 - l1
+// (all exact in fp32).  grad_flow[b, y, x, c] = +0 + term_1 + term_2 + ..., left to right, over the output pixels (Y, X)
+// in ascending row-major order and, within a pixel, its corners 00, 01, 10, 11 that land on (y, x) -- zero weights
+// included, so a NaN reaches every cell PyTorch's own backward gives it.  Each term is fl(fl(ly * lx) * grad_up); every
+// operation is one rounded fp32 operation.  A gather, one thread per input pixel and both channels: output pixels
+// within 4 of the cell's 8 x 8 block are the only ones that reach it, and for cell 1 of an axis also output 0..3, whose
+// clamped source gives cell 1 a zero weight.
+struct UpAxis {
+  int i0, i1;
+  float l0, l1;
+};
+
+__device__ __forceinline__ UpAxis upflow8_axis(int X, int n) {
+  const float src = fmaxf(__fsub_rn(__fmul_rn(0.125f, __fadd_rn((float)X, 0.5f)), 0.5f), 0.0f);
+  UpAxis a;
+  a.i0 = (int)src;
+  a.i1 = a.i0 + (a.i0 < n - 1 ? 1 : 0);
+  a.l1 = __fsub_rn(src, (float)a.i0);
+  a.l0 = __fsub_rn(1.0f, a.l1);
+  return a;
+}
+
+__global__ void __launch_bounds__(128) upflow8_bwd_kernel(const float* __restrict__ grad_up, int B, int h, int w,
+                                                          float* __restrict__ grad_flow) {
+  const int H = 8 * h, W = 8 * w;
+  const size_t total = (size_t)B * h * w;
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const int x = (int)(i % w), y = (int)((i / w) % h);
+    const size_t b = i / ((size_t)w * h);
+    const float2* g = reinterpret_cast<const float2*>(grad_up) + b * H * W;
+    float s0 = 0.0f, s1 = 0.0f;
+    const int Y0 = y == 1 ? 0 : max(8 * y - 4, 0), Y1 = min(8 * y + 12, H);
+    const int X0 = x == 1 ? 0 : max(8 * x - 4, 0), X1 = min(8 * x + 12, W);
+    for (int Y = Y0; Y < Y1; ++Y) {
+      const UpAxis ay = upflow8_axis(Y, h);
+      if (ay.i0 != y && ay.i1 != y) continue;
+      for (int X = X0; X < X1; ++X) {
+        const UpAxis ax = upflow8_axis(X, w);
+        if (ax.i0 != x && ax.i1 != x) continue;
+        const float2 gv = __ldg(g + (size_t)Y * W + X);
+#pragma unroll
+        for (int cy = 0; cy < 2; ++cy) {
+          if ((cy ? ay.i1 : ay.i0) != y) continue;
+#pragma unroll
+          for (int cx = 0; cx < 2; ++cx) {
+            if ((cx ? ax.i1 : ax.i0) != x) continue;
+            const float c = __fmul_rn(cy ? ay.l1 : ay.l0, cx ? ax.l1 : ax.l0);
+            s0 = __fadd_rn(s0, __fmul_rn(c, gv.x));
+            s1 = __fadd_rn(s1, __fmul_rn(c, gv.y));
+          }
+        }
+      }
+    }
+    reinterpret_cast<float2*>(grad_flow)[i] = make_float2(s0, s1);
+  }
+}
+
 // ------------------------------------------------------------------------------------------------
 // Weight re-layout for the tensor-core path.
 //   HWIO fp32 (kh,kw,cin,cout)  ->  [tap][cout_pad][cin_pad] fp16 hi / lo planes of w * 2^k,

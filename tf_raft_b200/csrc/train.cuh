@@ -13,8 +13,25 @@ namespace raft {
 //   d P_l[q, iy, ix] += wy * wx * go                                  (4 scatter-adds)
 //   d gx = go * ( wy1 * (P01 - P00) + wy0 * (P11 - P10) ),  d cx += d gx / 2^l  when 0 <= cx/2^l + (a-r) <= W-1
 //   d gy = go * ( wx1 * (P10 - P00) + wx0 * (P11 - P01) ),  d cy likewise.
-// One warp per (query, level); lanes stride over the taps; coordinate gradients are reduced in the warp and added with
-// one atomic per (query, level); pyramid gradients are scatter-added with atomics (floating-point order not fixed).
+// Terms are skipped where go == 0 and, for the pyramid, where c = wy * wx == 0; the coordinate terms are gated by the
+// clip as above.
+//
+// Fixed order, no atomics: every result depends on the shape and the data only, so two calls give the same bits.  Each
+// operation is one rounded fp32 operation (__fmul_rn / __fadd_rn / __fsub_rn, never contracted into an FMA), so
+// oracle/determinism_np.py reproduces every bit in NumPy float32.  With t = a*(2r+1) + b the tap index:
+//   d P_l[q] : a touched cell ends as v_in + term_1 + term_2 + ..., added left to right, its terms fl(fl(wy*wx) * go) in
+//              ascending t and, within a tap, in corner order 00, 01, 10, 11 (a tap reaches a cell through one corner at
+//              most).  Untouched cells are neither read nor written.
+//   d coords : per level, lane j (0..31) sums, left to right from +0, the gated d gx of taps j, j+32, j+64, ...; the 32
+//              lane sums are combined by the butterfly s_j <- s_j + s_{j xor o}, o = 16, 8, 4, 2, 1, giving G_l (lane 0's
+//              value; d gy likewise).  grad_coords[q] ends as in + fl(G_0 * inv_0) + fl(G_1 * inv_1) + ..., added in
+//              ascending level l, inv_l = 2^-l.
+// One warp per (query, level) owns grad_pyr[l]'s private h_l x w_l slice of that query: first its lanes stride over the
+// taps for G_l, then over the (2r+2)^2 cells of the window, each lane gathering a cell's terms in order.  A tap with a
+// non-zero x weight has x0 = floor(fl(cx + a - r)) = floor(cx) + a - r exactly (rounding cannot move a non-integer sum
+// past an integer), so window column s (0..2r+1) is reached by tap a = s-1 through its x1 corner and by a = s through its
+// x0 corner, and by no other tap; rows likewise.  The warps of one query share a block, and one thread per query adds
+// their G_l to grad_coords after a barrier.
 // ------------------------------------------------------------------------------------------------
 struct LookupBwdParams {
   const float* pyr[RAFT_MAX_LEVELS];
@@ -26,50 +43,118 @@ struct LookupBwdParams {
   int nq, levels, radius;
 };
 
+// One axis of one tap: u = c + offset before the clip, g = clip(u, 0, n-1); corner 0 = floor(g) with weight w1 =
+// ceil(g) - g, corner 1 = ceil(g) with weight w0 = g - floor(g); `in` is the clip's gradient gate.
+struct LookupAxis {
+  int i0, i1;
+  float w0, w1;
+  bool in;
+};
+
+__device__ __forceinline__ LookupAxis lookup_axis(float c, int offset, int n) {
+  const float u = __fadd_rn(c, (float)offset);
+  const float g = fminf(fmaxf(u, 0.0f), (float)(n - 1));
+  const float f0 = floorf(g), f1 = ceilf(g);
+  LookupAxis ax;
+  ax.i0 = (int)f0;
+  ax.i1 = (int)f1;
+  ax.w1 = __fsub_rn(f1, g);
+  ax.w0 = __fsub_rn(g, f0);
+  ax.in = u >= 0.0f && u <= (float)(n - 1);
+  return ax;
+}
+
+// Queries per block for `levels` levels: one warp per (query, level), at most 8 warps.
+inline int lookup_bwd_queries_per_block(int levels) { return levels >= 8 ? 1 : 8 / levels; }
+
 __global__ void __launch_bounds__(256) corr_lookup_bwd_kernel(const LookupBwdParams p) {
-  const int warps_per_block = blockDim.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int side = 2 * p.radius + 1, ntap = side * side;
-  const size_t nwork = (size_t)p.nq * p.levels;
-  for (size_t wi = (size_t)blockIdx.x * warps_per_block + (threadIdx.x >> 5); wi < nwork;
-       wi += (size_t)gridDim.x * warps_per_block) {
-    const int q = (int)(wi / p.levels), l = (int)(wi % p.levels);
-    const int H = p.lh[l], W = p.lw[l];
-    const float* img = p.pyr[l] + (size_t)q * H * W;
-    float* gimg = p.gpyr[l] + (size_t)q * H * W;
-    const float inv = 1.0f / (float)(1 << l);
-    const float cx = __ldg(p.coords + 2 * (size_t)q) * inv, cy = __ldg(p.coords + 2 * (size_t)q + 1) * inv;
-    float gcx = 0.0f, gcy = 0.0f;
-    for (int t = lane; t < ntap; t += 32) {
-      const int a = t / side, b = t - a * side;
-      const float go = __ldg(p.gout + (size_t)q * p.gout_stride + l * ntap + t);
-      const float ux = cx + (float)(a - p.radius), uy = cy + (float)(b - p.radius);      // before the clip
-      const float gx = fminf(fmaxf(ux, 0.0f), (float)(W - 1)), gy = fminf(fmaxf(uy, 0.0f), (float)(H - 1));
-      const float x0 = floorf(gx), x1 = ceilf(gx), y0 = floorf(gy), y1 = ceilf(gy);
-      const float wx1 = x1 - gx, wx0 = gx - x0, wy1 = y1 - gy, wy0 = gy - y0;
-      const int o00 = (int)y0 * W + (int)x0, o01 = (int)y0 * W + (int)x1, o10 = (int)y1 * W + (int)x0, o11 = (int)y1 * W + (int)x1;
-      const float p00 = __ldg(img + o00), p01 = __ldg(img + o01), p10 = __ldg(img + o10), p11 = __ldg(img + o11);
-      if (go != 0.0f) {
-        const float c00 = wy1 * wx1, c01 = wy1 * wx0, c10 = wy0 * wx1, c11 = wy0 * wx0;
-        if (c00 != 0.0f) atomicAdd(gimg + o00, c00 * go);
-        if (c01 != 0.0f) atomicAdd(gimg + o01, c01 * go);
-        if (c10 != 0.0f) atomicAdd(gimg + o10, c10 * go);
-        if (c11 != 0.0f) atomicAdd(gimg + o11, c11 * go);
-        const float dgx = go * (wy1 * (p01 - p00) + wy0 * (p11 - p10));
-        const float dgy = go * (wx1 * (p10 - p00) + wx0 * (p11 - p01));
-        if (ux >= 0.0f && ux <= (float)(W - 1)) gcx += dgx;
-        if (uy >= 0.0f && uy <= (float)(H - 1)) gcy += dgy;
+  __shared__ float level_sum[8][2];                              // G_l of each warp of the block
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int qpb = blockDim.x / (32 * p.levels);
+  const int l = warp % p.levels;
+  const int side = 2 * p.radius + 1, ntap = side * side, ncell = (side + 1) * (side + 1);
+  for (size_t q0 = (size_t)blockIdx.x * qpb; q0 < (size_t)p.nq; q0 += (size_t)gridDim.x * qpb) {
+    const size_t q = q0 + warp / p.levels;
+    if (q < (size_t)p.nq) {
+      const int H = p.lh[l], W = p.lw[l];
+      const float* img = p.pyr[l] + q * H * W;
+      float* gimg = p.gpyr[l] + q * H * W;
+      const float* go_row = p.gout + q * p.gout_stride + (size_t)l * ntap;
+      const float inv = 1.0f / (float)(1 << l);
+      const float cx = __fmul_rn(__ldg(p.coords + 2 * q), inv), cy = __fmul_rn(__ldg(p.coords + 2 * q + 1), inv);
+      // coordinate gradient: lanes stride over the taps
+      float gcx = 0.0f, gcy = 0.0f;
+      for (int t = lane; t < ntap; t += 32) {
+        const float go = __ldg(go_row + t);
+        if (go == 0.0f) continue;
+        const int a = t / side, b = t - a * side;
+        const LookupAxis X = lookup_axis(cx, a - p.radius, W), Y = lookup_axis(cy, b - p.radius, H);
+        const float p00 = __ldg(img + (size_t)Y.i0 * W + X.i0), p01 = __ldg(img + (size_t)Y.i0 * W + X.i1);
+        const float p10 = __ldg(img + (size_t)Y.i1 * W + X.i0), p11 = __ldg(img + (size_t)Y.i1 * W + X.i1);
+        const float dgx = __fmul_rn(go, __fadd_rn(__fmul_rn(Y.w1, __fsub_rn(p01, p00)), __fmul_rn(Y.w0, __fsub_rn(p11, p10))));
+        const float dgy = __fmul_rn(go, __fadd_rn(__fmul_rn(X.w1, __fsub_rn(p10, p00)), __fmul_rn(X.w0, __fsub_rn(p11, p01))));
+        if (X.in) gcx = __fadd_rn(gcx, dgx);
+        if (Y.in) gcy = __fadd_rn(gcy, dgy);
+      }
+#pragma unroll
+      for (int off = 16; off > 0; off >>= 1) {
+        gcx = __fadd_rn(gcx, __shfl_xor_sync(0xffffffffu, gcx, off));
+        gcy = __fadd_rn(gcy, __shfl_xor_sync(0xffffffffu, gcy, off));
+      }
+      if (lane == 0) {
+        level_sum[warp][0] = gcx;
+        level_sum[warp][1] = gcy;
+      }
+      // pyramid gradient: lanes stride over the window's cells, x fastest; cell (sx, sy) gathers taps a = sx-1 (x1
+      // corner), a = sx (x0 corner) and b = sy-1 (y1 corner), b = sy (y0 corner), in ascending t
+      for (int k = lane; k < ncell; k += 32) {
+        const int sy = k / (side + 1), sx = k - sy * (side + 1);
+        LookupAxis Ys[2];
+#pragma unroll
+        for (int ib = 0; ib < 2; ++ib) Ys[ib] = lookup_axis(cy, sy - 1 + ib - p.radius, H);
+        float v = 0.0f;
+        size_t off = 0;
+        bool touched = false;
+#pragma unroll
+        for (int ia = 0; ia < 2; ++ia) {
+          const int a = sx - 1 + ia;
+          if (a < 0 || a >= side) continue;
+          const LookupAxis X = lookup_axis(cx, a - p.radius, W);
+          const float wx = ia == 0 ? X.w0 : X.w1;
+          const int xi = ia == 0 ? X.i1 : X.i0;
+#pragma unroll
+          for (int ib = 0; ib < 2; ++ib) {
+            const int b = sy - 1 + ib;
+            if (b < 0 || b >= side) continue;
+            const float go = __ldg(go_row + a * side + b);
+            if (go == 0.0f) continue;
+            const float wy = ib == 0 ? Ys[0].w0 : Ys[1].w1;
+            const float c = __fmul_rn(wy, wx);
+            if (c == 0.0f) continue;
+            if (!touched) {
+              off = (size_t)(ib == 0 ? Ys[0].i1 : Ys[1].i0) * W + xi;
+              v = gimg[off];
+              touched = true;
+            }
+            v = __fadd_rn(v, __fmul_rn(c, go));
+          }
+        }
+        if (touched) gimg[off] = v;
       }
     }
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) {
-      gcx += __shfl_xor_sync(0xffffffffu, gcx, off);
-      gcy += __shfl_xor_sync(0xffffffffu, gcy, off);
+    __syncthreads();
+    if (threadIdx.x < qpb && q0 + threadIdx.x < (size_t)p.nq) {       // one owner per query: levels in ascending order
+      const size_t qq = q0 + threadIdx.x;
+      float gx = p.gcoords[2 * qq], gy = p.gcoords[2 * qq + 1];
+      for (int k = 0; k < p.levels; ++k) {
+        const float inv = 1.0f / (float)(1 << k);
+        gx = __fadd_rn(gx, __fmul_rn(level_sum[threadIdx.x * p.levels + k][0], inv));
+        gy = __fadd_rn(gy, __fmul_rn(level_sum[threadIdx.x * p.levels + k][1], inv));
+      }
+      p.gcoords[2 * qq] = gx;
+      p.gcoords[2 * qq + 1] = gy;
     }
-    if (lane == 0) {
-      atomicAdd(p.gcoords + 2 * (size_t)q, gcx * inv);
-      atomicAdd(p.gcoords + 2 * (size_t)q + 1, gcy * inv);
-    }
+    __syncthreads();
   }
 }
 

@@ -334,6 +334,25 @@ class _Lookup(torch.autograd.Function):
         return (g_coords, None) + tuple(g_pyr)
 
 
+class _Upsample8(torch.autograd.Function):
+    """SmallRAFT's training upsampling of an NHWC flow: forward = the graph's F.interpolate(scale_factor=8, 'bilinear')
+    on its NCHW view, unchanged; backward = raft_b200_upflow8_backward, a gather in a fixed order.  PyTorch's own CUDA
+    backward of that op scatters with atomics, and torch.use_deterministic_algorithms(True) refuses it."""
+
+    @staticmethod
+    def forward(ctx, flow):
+        ctx.shape = flow.shape
+        return F.interpolate(flow.permute(0, 3, 1, 2), scale_factor=8, mode='bilinear', align_corners=False)
+
+    @staticmethod
+    def backward(ctx, grad_up):
+        b, h, w, _ = ctx.shape
+        grad_up = grad_up.permute(0, 2, 3, 1).contiguous()
+        grad_flow = torch.empty((b, h, w, 2), dtype=torch.float32, device=grad_up.device)
+        _lib.call('upflow8_backward', grad_up.device, _lib.ptr(grad_up), b, h, w, _lib.ptr(grad_flow))
+        return grad_flow
+
+
 class _CorrPyramid(torch.autograd.Function):
     """CorrBlock.__init__: forward = the wgmma correlation kernels; backward = fp32 GEMMs on the pooled features
     (level l = fmap1 . avgpool^l(fmap2)^T / sqrt(C), so d fmap1 = sum_l dP_l . pool^l(fmap2) / sqrt(C) and
@@ -622,6 +641,8 @@ class TrainGraph:
             coords1 = coords1 + delta.permute(0, 2, 3, 1)
             if self.variant == 'raft':
                 preds.append(self.upsample_flow(coords1 - coords0, mask.permute(0, 2, 3, 1)))
+            elif coords1.is_cuda:
+                preds.append(8 * _Upsample8.apply(coords1 - coords0).permute(0, 2, 3, 1))
             else:
                 up = F.interpolate((coords1 - coords0).permute(0, 3, 1, 2), scale_factor=8, mode='bilinear', align_corners=False)
                 preds.append(8 * up.permute(0, 2, 3, 1))
