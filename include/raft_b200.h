@@ -57,6 +57,25 @@ typedef enum raft_precision { RAFT_PREC_FP32 = 0, RAFT_PREC_F16X2 = 1 } raft_pre
 /* model.py:10-30 (RAFT, BasicUpdateBlock) / model.py:173-188 (SmallRAFT, SmallUpdateBlock). */
 typedef enum raft_variant { RAFT_VARIANT_BASIC = 0, RAFT_VARIANT_SMALL = 1 } raft_variant;
 
+/* Lookup sampler (raft_b200_corr_lookup_ex, raft_b200_forward_loop_ex).
+ *   TF    tf-raft's bilinear_sampler (corr.py:28-69): clamp to [0, S-1], floor / ceil corners.
+ *   GRID  the original PyTorch RAFT's: F.grid_sample(align_corners=True, padding_mode='zeros') after RAFT's
+ *         normalisation 2*x/(S-1) - 1.  Per axis of size S, level coordinate v = fl(fl(c * 2^-l) + d), op by op in
+ *         fp32 with no FMA: g = fl(fl(fl(2v) * fl(1 / (S-1))) - 1) (the division as ATen's CUDA kernel does it for
+ *         a scalar divisor, a product with the reciprocal); ix = fl(fl(fl(g + 1) / 2) * (S-1)); ix = -100 unless
+ *         -2^31 <= ix <= 2^31 (NaN included); corners x0 = floor(ix), x1 = x0 + 1 with weights fl(x1 - ix),
+ *         fl(ix - x0).  A corner outside [0, S-1] is never read and adds nothing, so a level with S = 1 gives 0 for
+ *         every tap.  Sum order of a tap: acc = +0, then for (y0,x0), (y0,x1), (y1,x0), (y1,x1) in that order, if the
+ *         corner is in the level, acc = fl(acc + fl(fl(wy * wx) * texel)) -- weight 0 included.                    */
+typedef enum raft_sampler { RAFT_SAMPLER_TF = 0, RAFT_SAMPLER_GRID = 1 } raft_sampler;
+
+/* Arithmetic conventions of the encoders (raft_b200_encoder_prepare_ex).
+ *   TF       tf-raft: Keras 'same' padding, asymmetric at stride 2 on even inputs (7x7/s2 pads 2 before, 3 after;
+ *            3x3/s2 0 / 1), norm epsilon 1e-3.
+ *   PYTORCH  the original PyTorch RAFT: symmetric padding (7x7/s2 p=3, 3x3/s2 p=1, 1x1/s2 p=0), epsilon 1e-5.
+ * Both give ceil(H/2) outputs at stride 2, so workspaces do not depend on the convention.                        */
+typedef enum raft_conventions { RAFT_CONVENTIONS_TF = 0, RAFT_CONVENTIONS_PYTORCH = 1 } raft_conventions;
+
 const char* raft_b200_strerror(int status);
 int raft_b200_abi_version(void);
 /* 0 if device `device` can run the kernels (compute capability 9.0), else RAFT_ERR_NO_DEVICE.  */
@@ -88,6 +107,9 @@ int raft_b200_corr_pyramid_build(const float* fmap1, const float* fmap2, int B, 
  *   an integer is exactly 0 (floor/ceil corners, corr.py:45-60) -- reproduced bit for bit.      */
 int raft_b200_corr_lookup(const float* const pyr[], const float* coords, int B, int h, int w, int levels,
                           int radius, float* out, int out_stride, void* stream);
+/* raft_b200_corr_lookup with the sampler chosen (raft_sampler); RAFT_SAMPLER_TF is raft_b200_corr_lookup.        */
+int raft_b200_corr_lookup_ex(const float* const pyr[], const float* coords, int B, int h, int w, int levels,
+                             int radius, float* out, int out_stride, int sampler, void* stream);
 
 /* Backward of CorrBlock.retrieve for the training step (tf_raft/model.py:133: tape.gradient through corr.py:116-152;
  * the reference does not detach coords1, model.py:102).  grad_out (B, h, w, levels*(2r+1)^2) -> grad_coords (B, h, w, 2)
@@ -430,6 +452,15 @@ typedef enum raft_norm_type { RAFT_NORM_NONE = 0, RAFT_NORM_INSTANCE = 1, RAFT_N
 int raft_b200_encoder_prepared_bytes(int variant, int out_dim, size_t* bytes);
 int raft_b200_encoder_prepare(int variant, int norm_type, int out_dim, const raft_encoder_weights* weights,
                               void* prepared, size_t prepared_bytes, void* stream);
+/* raft_b200_encoder_prepare under the given conventions (raft_conventions), which the blob records: the BatchNorm
+ * fold uses its epsilon now, and raft_b200_encoder_forward / raft_b200_encode_pair take its padding and epsilon from
+ * the blob.  raft_b200_encoder_prepare is this call with RAFT_CONVENTIONS_TF.  The convention is bound to the blob's
+ * device address by the last prepare call at that address, and forward calls look it up there without touching the
+ * device.  A blob copied to an address no prepare call has used has its convention read back from the device once
+ * (never under CUDA-graph capture: RAFT_ERR_UNSUPPORTED).  A blob copied onto an address a prepare call used is taken
+ * to have that call's convention: prepare a blob where it is used instead of copying one there.                  */
+int raft_b200_encoder_prepare_ex(int variant, int norm_type, int out_dim, const raft_encoder_weights* weights,
+                                 int conventions, void* prepared, size_t prepared_bytes, void* stream);
 int raft_b200_encoder_workspace_bytes(int variant, int N, int H, int W, size_t* bytes);
 
 /* BasicEncoder.call / SmallEncoder.call (extractor.py:113-130 / 158-175) on N images.
@@ -536,6 +567,11 @@ int raft_b200_forward_loop(int variant, const void* prepared, const float* const
                            float* net, const float* inp, float* coords1, float* const flow_up[], int iters,
                            int B, int h, int w, void* workspace, size_t workspace_bytes, int precision,
                            void* stream);
+/* raft_b200_forward_loop with the lookup's sampler chosen (raft_sampler); RAFT_SAMPLER_TF is raft_b200_forward_loop. */
+int raft_b200_forward_loop_ex(int variant, const void* prepared, const float* const pyr[], int levels, int radius,
+                              float* net, const float* inp, float* coords1, float* const flow_up[], int iters,
+                              int B, int h, int w, void* workspace, size_t workspace_bytes, int precision,
+                              int sampler, void* stream);
 
 /* Number of kernels launched on this host thread since the last raft_b200_launch_count_reset (bench.py's gpu_launches). */
 long long raft_b200_launch_count(void);

@@ -13,6 +13,12 @@ started from the previous pair's forward-interpolated flow, as RAFT produced its
 
     python scripts/evaluate.py sintel --root ... --checkpoint ... --padding replicate --warm-start --iters 32
     python scripts/evaluate.py kitti --root ... --checkpoint ... --padding replicate --pad-mode kitti
+
+A checkpoint of the original PyTorch RAFT (raft-things.pth, ...) is scored with `--pytorch-checkpoint PATH` instead of
+`--checkpoint`: RAFT(conventions='pytorch') with RAFT's validation protocol -- replicate padding (bottom-only for
+KITTI), 32 iterations on Sintel and 24 on KITTI, each unless --padding, --pad-mode or --iters says otherwise:
+
+    python scripts/evaluate.py sintel --root datasets/MPI-Sintel-complete --pytorch-checkpoint models/raft-things.pth
 """
 import argparse
 import json
@@ -44,17 +50,20 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('dataset', choices=sorted(DEFAULTS))
     ap.add_argument('--root', required=True)
-    ap.add_argument('--checkpoint', required=True, help='TF checkpoint prefix (the path before .index)')
+    src = ap.add_mutually_exclusive_group(required=True)
+    src.add_argument('--checkpoint', help='TF checkpoint prefix (the path before .index)')
+    src.add_argument('--pytorch-checkpoint', help="the original PyTorch RAFT's .pth (basic model)")
     ap.add_argument('--small', action='store_true', help='SmallRAFT instead of RAFT')
     ap.add_argument('--dstype', default=None, help="Sintel 'clean' / 'final'; Things 'frames_cleanpass' / ...")
     ap.add_argument('--split-txt', default='FlyingChairs_train_val.txt')
-    ap.add_argument('--iters', type=int, default=24)
+    ap.add_argument('--iters', type=int, default=None, help='default 24; with --pytorch-checkpoint 32 on Sintel')
     ap.add_argument('--batch-size', type=int, default=4)
     ap.add_argument('--workers', type=int, default=8)
     ap.add_argument('--protocol', choices=T.evaluation.PROTOCOLS, default=None)
     ap.add_argument('--max-flow', type=float, default=-1, help='ground-truth magnitude cut; 0 turns it off')
-    ap.add_argument('--padding', choices=('zero', 'replicate'), default='zero',
-                    help="'replicate' is RAFT's InputPadder; 'zero' the reference's CropOrPadder")
+    ap.add_argument('--padding', choices=('zero', 'replicate'), default=None,
+                    help="'replicate' is RAFT's InputPadder; 'zero' the reference's CropOrPadder (the default, "
+                         "'replicate' with --pytorch-checkpoint)")
     ap.add_argument('--pad-mode', choices=('sintel', 'kitti'), default=None,
                     help="'kitti' puts all vertical padding at the bottom (default 'sintel': centred)")
     ap.add_argument('--warm-start', action='store_true',
@@ -66,13 +75,26 @@ def main():
     protocol = args.protocol or protocol
     if args.max_flow >= 0:
         max_flow = args.max_flow or None
-    model = (T.SmallRAFT if args.small else T.RAFT)(iters_pred=args.iters)
-    model.load_params(T.load_tf_checkpoint(args.checkpoint, expect=model.state_dict()))
+    if args.pytorch_checkpoint:
+        if args.small:
+            ap.error('--pytorch-checkpoint loads the basic RAFT model only')
+        args.padding = args.padding or 'replicate'                      # RAFT's InputPadder
+        args.pad_mode = args.pad_mode or ('kitti' if args.dataset == 'kitti' else 'sintel')
+        if args.iters is None:
+            args.iters = 32 if args.dataset == 'sintel' else 24
+        model = T.RAFT(iters_pred=args.iters, conventions='pytorch')
+        model.load_pytorch_weights(args.pytorch_checkpoint)
+    else:
+        args.iters = 24 if args.iters is None else args.iters
+        args.padding = args.padding or 'zero'
+        model = (T.SmallRAFT if args.small else T.RAFT)(iters_pred=args.iters)
+        model.load_params(T.load_tf_checkpoint(args.checkpoint, expect=model.state_dict()))
     ds = dataset(args.dataset, args)
     res = T.evaluate(model, ds, batch_size=1 if args.warm_start else args.batch_size, max_flow=max_flow,
                      protocol=protocol, workers=args.workers, padding=args.padding, pad_mode=args.pad_mode,
                      warm_start=args.warm_start)
     print(json.dumps({'dataset': args.dataset, 'pairs': len(ds), 'protocol': protocol, 'max_flow': max_flow,
+                      'conventions': model.conventions,
                       'iters': args.iters, 'padding': args.padding, 'pad_mode': args.pad_mode or 'sintel',
                       'warm_start': args.warm_start, **res}))
 

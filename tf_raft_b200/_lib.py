@@ -56,6 +56,9 @@ class RaftEncoderWeights(ctypes.Structure):
 
 
 NORM_TYPES = {None: 0, 'instance': 1, 'batch': 2}
+# raft_conventions / raft_sampler (include/raft_b200.h): tf-raft's arithmetic, or the original PyTorch RAFT's
+CONVENTIONS = {'tf-raft': 0, 'pytorch': 1}
+SAMPLERS = {'tf-raft': 0, 'grid_sample': 1}
 
 _vp, _i, _sz = ctypes.c_void_p, ctypes.c_int, ctypes.c_size_t
 _SIGNATURES = {
@@ -70,6 +73,7 @@ _SIGNATURES = {
     'raft_b200_corr_workspace_bytes': (_i, [_i, _i, _i, _i, _i, _i, ctypes.POINTER(_sz)]),
     'raft_b200_corr_pyramid_build': (_i, [_vp, _vp, _i, _i, _i, _i, _i, ctypes.POINTER(_vp), _vp, _sz, _i, _vp]),
     'raft_b200_corr_lookup': (_i, [ctypes.POINTER(_vp), _vp, _i, _i, _i, _i, _i, _vp, _i, _vp]),
+    'raft_b200_corr_lookup_ex': (_i, [ctypes.POINTER(_vp), _vp, _i, _i, _i, _i, _i, _vp, _i, _i, _vp]),
     'raft_b200_corr_lookup_backward': (_i, [ctypes.POINTER(_vp), _vp, _vp, _i, _i, _i, _i, _i, _vp, ctypes.POINTER(_vp), _vp]),
     'raft_b200_sumsq': (_i, [_vp, _sz, _vp, _sz, _vp, _vp]),
     'raft_b200_adamw_step': (_i, [_vp, _vp, _vp, _vp, _sz, _vp, ctypes.c_float, ctypes.c_float, ctypes.c_float,
@@ -102,6 +106,7 @@ _SIGNATURES = {
     'raft_b200_upflow8_backward': (_i, [_vp, _i, _i, _i, _vp, _vp]),
     'raft_b200_encoder_prepared_bytes': (_i, [_i, _i, ctypes.POINTER(_sz)]),
     'raft_b200_encoder_prepare': (_i, [_i, _i, _i, _vp, _vp, _sz, _vp]),
+    'raft_b200_encoder_prepare_ex': (_i, [_i, _i, _i, _vp, _i, _vp, _sz, _vp]),
     'raft_b200_encoder_workspace_bytes': (_i, [_i, _i, _i, _i, ctypes.POINTER(_sz)]),
     'raft_b200_encoder_forward': (_i, [_i, _i, _i, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _sz, _vp]),
     'raft_b200_context_split': (_i, [_vp, _i, _i, _i, _vp, _vp, _vp]),
@@ -115,6 +120,8 @@ _SIGNATURES = {
                                         _vp]),
     'raft_b200_forward_loop': (_i, [_i, _vp, ctypes.POINTER(_vp), _i, _i, _vp, _vp, _vp, ctypes.POINTER(_vp), _i,
                                     _i, _i, _i, _vp, _sz, _i, _vp]),
+    'raft_b200_forward_loop_ex': (_i, [_i, _vp, ctypes.POINTER(_vp), _i, _i, _vp, _vp, _vp, ctypes.POINTER(_vp), _i,
+                                       _i, _i, _i, _vp, _sz, _i, _i, _vp]),
 }
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)
 

@@ -17,6 +17,7 @@ writer below produces exactly such bytes, round-trips files through both, and ch
 attribute tree.
 """
 import os
+import re
 import struct
 
 import numpy as np
@@ -364,4 +365,106 @@ def load_tf_checkpoint(prefix, verify=False, expect=None):
         if missing or extra or shapes:
             raise ValueError(f'{prefix}: does not match the model -- missing {missing[:8]}{"..." if len(missing) > 8 else ""}, '
                              f'unexpected {extra[:8]}{"..." if len(extra) > 8 else ""}, shapes {shapes[:8]}')
+    return params
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# The original PyTorch RAFT's checkpoints (raft-chairs.pth, raft-things.pth, raft-sintel.pth, raft-kitti.pth)
+# ------------------------------------------------------------------------------------------------------------------
+_PT_NORM = {'weight': 'gamma', 'bias': 'beta', 'running_mean': 'moving_mean', 'running_var': 'moving_variance'}
+
+
+def mask_head_permutation():
+    """Output channel c of this project's mask head (update_block.mask.2) is channel perm[c] of the PyTorch RAFT's:
+    here c = (8a + b) * 9 + k, there k * 64 + 8a + b (RAFT's `mask.view(N, 1, 9, 8, 8, H, W)`), for the 8x8 sub-pixel
+    (a, b) and the 3x3 tap k."""
+    c = np.arange(576)
+    return (c % 9) * 64 + c // 9
+
+
+def load_pytorch_checkpoint(path_or_state_dict, expect=None):
+    """A checkpoint of the original PyTorch RAFT (basic model) -> `{param name: ndarray}` for `RAFT.load_params` of a
+    model built with `conventions='pytorch'`.
+
+    Read with `torch.load(map_location='cpu', weights_only=True)` (or given as a state dict).  The mapping: the
+    `module.` prefix of nn.DataParallel is stripped; OIHW weights become HWIO kernels; BatchNorm's weight / bias /
+    running_mean / running_var become gamma / beta / moving_mean / moving_variance and `num_batches_tracked` is dropped;
+    each ResidualBlock's `norm3`, which PyTorch also stores as `downsample.1`, must equal that twin and is dropped;
+    fnet's instance norms (affine=False, no parameters) get gamma = 1 and beta = 0; the mask head's output channels are
+    permuted (`mask_head_permutation`).  Missing, unexpected and mis-shaped keys are reported in ONE ValueError (with
+    `expect` = the model's `state_dict()`, against its names and shapes)."""
+    import torch
+    label = 'state dict'
+    sd = path_or_state_dict
+    if not isinstance(sd, dict):
+        label = str(sd)
+        sd = torch.load(sd, map_location='cpu', weights_only=True)
+        if isinstance(sd, dict) and isinstance(sd.get('state_dict'), dict):
+            sd = sd['state_dict']
+    if not isinstance(sd, dict):
+        raise ValueError(f'{label}: not a state dict ({type(sd).__name__})')
+    src = {}
+    for k, v in sd.items():
+        k = k[len('module.'):] if k.startswith('module.') else k
+        src[k] = v.detach().cpu().numpy() if isinstance(v, torch.Tensor) else np.asarray(v)
+    small = sorted(k for k in src if re.search(r'\.(conv3|norm4)\.', k))
+    if small:
+        raise ValueError(f'{label}: bottleneck-block keys {small[:4]} -- a RAFT-small checkpoint; only the basic RAFT '
+                         'model loads (this SmallRAFT is built from residual blocks)')
+    params, extra, twins = {}, [], []
+    for k, v in src.items():
+        if k.endswith('.num_batches_tracked'):
+            continue
+        m = re.fullmatch(r'(.*\.layer\d\.\d)\.norm3\.(weight|bias|running_mean|running_var)', k)
+        if m:                                  # ResidualBlock.norm3 is also downsample.1: keep one copy
+            twin = f'{m.group(1)}.downsample.1.{m.group(2)}'
+            if twin not in src or np.shape(src[twin]) != np.shape(v) or not np.array_equal(src[twin], v):
+                twins.append(k)
+            continue
+        stem, _, leaf = k.rpartition('.')
+        if v.ndim == 4 and leaf == 'weight':
+            params[stem + '.kernel'] = np.ascontiguousarray(v.transpose(2, 3, 1, 0), dtype=np.float32)   # OIHW -> HWIO
+        elif v.ndim == 1 and leaf == 'bias' and stem + '.weight' in src and src[stem + '.weight'].ndim == 4:
+            params[stem + '.bias'] = v.astype(np.float32)
+        elif v.ndim == 1 and leaf in _PT_NORM:
+            params[f'{stem}.{_PT_NORM[leaf]}'] = v.astype(np.float32)
+        else:
+            extra.append(k)
+    if 'update_block.mask.2.kernel' in params and params['update_block.mask.2.kernel'].shape[-1] == 576:
+        perm = mask_head_permutation()
+        params['update_block.mask.2.kernel'] = np.ascontiguousarray(params['update_block.mask.2.kernel'][..., perm])
+        if 'update_block.mask.2.bias' in params and params['update_block.mask.2.bias'].shape == (576,):
+            params['update_block.mask.2.bias'] = params['update_block.mask.2.bias'][perm]
+    # fnet's nn.InstanceNorm2d(affine=False): the identity affine of tfa InstanceNormalization
+    fnorms = [('fnet.norm1', 64)]
+    for li, (c, stride) in enumerate(((64, 1), (96, 2), (128, 2)), start=1):
+        for bi in (0, 1):
+            fnorms += [(f'fnet.layer{li}.{bi}.norm1', c), (f'fnet.layer{li}.{bi}.norm2', c)]
+            if bi == 0 and stride != 1:
+                fnorms.append((f'fnet.layer{li}.{bi}.downsample.1', c))
+    if any(k.startswith('fnet.') for k in params):
+        for name, c in fnorms:
+            if f'{name}.gamma' not in params:
+                params[f'{name}.gamma'] = np.ones(c, np.float32)
+                params[f'{name}.beta'] = np.zeros(c, np.float32)
+    if not any(k.startswith(('fnet.', 'cnet.', 'update_block.')) for k in params):
+        raise ValueError(f'{label}: no fnet / cnet / update_block parameters found')
+    problems = []
+    if twins:
+        problems.append(f'norm3 differing from its downsample.1 twin {twins[:4]}')
+    if expect is not None:
+        want = {k: tuple(np.shape(v)) for k, v in dict(expect).items()}
+        missing = sorted(set(want) - set(params))
+        extra += sorted(set(params) - set(want))
+        shapes = sorted(f'{k}: checkpoint {tuple(params[k].shape)} vs model {want[k]}' for k in set(want) & set(params)
+                        if tuple(params[k].shape) != want[k])
+        if missing:
+            problems.append(f'missing {missing[:8]}{"..." if len(missing) > 8 else ""}')
+        if shapes:
+            problems.append(f'shapes {shapes[:8]}')
+    if extra:
+        extra = sorted(extra)
+        problems.append(f'unexpected {extra[:8]}{"..." if len(extra) > 8 else ""}')
+    if problems:
+        raise ValueError(f'{label}: does not match the model -- ' + '; '.join(problems))
     return params

@@ -24,6 +24,10 @@ thread_local long long g_launches = 0;
 static int check_dims(int B, int h, int w) { return (B > 0 && h > 0 && w > 0) ? 0 : RAFT_ERR_BAD_SHAPE; }
 static int check_variant(int v) { return (v == RAFT_VARIANT_BASIC || v == RAFT_VARIANT_SMALL) ? 0 : RAFT_ERR_BAD_ARG; }
 static int check_precision(int p) { return (p == RAFT_PREC_FP32 || p == RAFT_PREC_F16X2) ? 0 : RAFT_ERR_BAD_ARG; }
+static int check_sampler(int s) { return (s == RAFT_SAMPLER_TF || s == RAFT_SAMPLER_GRID) ? 0 : RAFT_ERR_BAD_ARG; }
+static int check_conventions(int c) {
+  return (c == RAFT_CONVENTIONS_TF || c == RAFT_CONVENTIONS_PYTORCH) ? 0 : RAFT_ERR_BAD_ARG;
+}
 
 // Per-kernel timing of raft_b200_forward_loop for bench.py's roofline objects: CUDA events on the launching stream around
 // the lookup and around the update-block kernel(s) of every iteration (raft_b200_profile_loop / _read).  Off by default;
@@ -280,7 +284,7 @@ static int update_once(int variant, const void* prepared, const float* net, cons
 // im_flow != null (iteration loop, tensor-core path): the convf1 im2col planes im_hi / im_lo are produced too -- by the
 // window kernel itself when it runs, else by flow_im2col_kernel.
 static int lookup_launch(const float* const pyr[], const float* coords, int B, int h, int w, int levels, int radius,
-                         float* out, int out_stride, __half* out_hi, __half* out_lo, int h_stride, int h_pad,
+                         float* out, int out_stride, __half* out_hi, __half* out_lo, int h_stride, int h_pad, int sampler,
                          cudaStream_t st, const float* im_flow = nullptr, __half* im_hi = nullptr, __half* im_lo = nullptr) {
   LookupParams p;
   memset(&p, 0, sizeof(p));
@@ -300,9 +304,10 @@ static int lookup_launch(const float* const pyr[], const float* coords, int B, i
   p.im_flow = im_flow; p.im_hi = im_hi; p.im_lo = im_lo; p.im_B = B; p.im_h = h; p.im_w = w;
   const size_t nwork = (size_t)p.nq * levels;
   static const int gather = [] { const char* e = getenv("RAFT_B200_LOOKUP_GATHER"); return e ? atoi(e) : 0; }();   // A/B: force the generic kernel
-  const LookupKernel win = gather ? nullptr : lookup_win_kernel(p, levels, radius);   // the model's (radius, levels)
+  const LookupKernel win = gather ? nullptr : lookup_win_kernel(p, levels, radius, sampler);   // the model's (radius, levels)
   if (win) return launch(win, grid_for(nwork * 32, 256, kNumSMs * 4), 256, 0, st, p);   // 4 resident blocks per SM: one wave
-  RAFT_TRY(launch(corr_lookup_kernel, grid_for(nwork * 32, 256, kNumSMs * 32), 256, 0, st, p));
+  RAFT_TRY(launch(sampler == RAFT_SAMPLER_GRID ? corr_lookup_grid_kernel : corr_lookup_kernel,
+                  grid_for(nwork * 32, 256, kNumSMs * 32), 256, 0, st, p));
   if (!im_flow) return RAFT_OK;
   return launch(flow_im2col_kernel, grid_for((size_t)p.nq * 128), 256, 0, st, im_flow, B, h, w, im_hi, im_lo);
 }
@@ -397,14 +402,20 @@ int raft_b200_corr_pyramid_build(const float* fmap1, const float* fmap2, int B, 
   return corr_build_tc(fmap1, fmap2, B, h, w, C, levels, pyr, workspace, st);
 }
 
-int raft_b200_corr_lookup(const float* const pyr[], const float* coords, int B, int h, int w, int levels, int radius,
-                          float* out, int out_stride, void* stream) {
+int raft_b200_corr_lookup_ex(const float* const pyr[], const float* coords, int B, int h, int w, int levels, int radius,
+                             float* out, int out_stride, int sampler, void* stream) {
   if (!pyr || !coords || !out || levels < 1 || levels > RAFT_MAX_LEVELS || radius < 0) return RAFT_ERR_BAD_ARG;
+  RAFT_TRY(check_sampler(sampler));
   RAFT_TRY(check_dims(B, h, w));
   const int side = 2 * radius + 1;
   if (out_stride < levels * side * side) return RAFT_ERR_BAD_SHAPE;
-  return lookup_launch(pyr, coords, B, h, w, levels, radius, out, out_stride, nullptr, nullptr, 0, 0,
+  return lookup_launch(pyr, coords, B, h, w, levels, radius, out, out_stride, nullptr, nullptr, 0, 0, sampler,
                        reinterpret_cast<cudaStream_t>(stream));
+}
+
+int raft_b200_corr_lookup(const float* const pyr[], const float* coords, int B, int h, int w, int levels, int radius,
+                          float* out, int out_stride, void* stream) {
+  return raft_b200_corr_lookup_ex(pyr, coords, B, h, w, levels, radius, out, out_stride, RAFT_SAMPLER_TF, stream);
 }
 
 int raft_b200_corr_lookup_backward(const float* const pyr[], const float* coords, const float* grad_out, int B, int h, int w,
@@ -792,13 +803,21 @@ int raft_b200_encoder_prepared_bytes(int variant, int out_dim, size_t* bytes) {
   return RAFT_OK;
 }
 
-int raft_b200_encoder_prepare(int variant, int norm_type, int out_dim, const raft_encoder_weights* weights,
-                              void* prepared, size_t prepared_bytes, void* stream) {
+int raft_b200_encoder_prepare_ex(int variant, int norm_type, int out_dim, const raft_encoder_weights* weights,
+                                 int conventions, void* prepared, size_t prepared_bytes, void* stream) {
   if (!weights || !prepared) return RAFT_ERR_BAD_ARG;
   RAFT_TRY(check_variant(variant));
+  RAFT_TRY(check_conventions(conventions));
   if (norm_type < 0 || norm_type > 2) return RAFT_ERR_BAD_ARG;
   if (out_dim < 32 || out_dim > 256 || out_dim % 32) return RAFT_ERR_BAD_SHAPE;
-  return encoder_prepare(variant, norm_type, out_dim, weights, prepared, prepared_bytes, reinterpret_cast<cudaStream_t>(stream));
+  return encoder_prepare(variant, norm_type, out_dim, weights, conventions, prepared, prepared_bytes,
+                         reinterpret_cast<cudaStream_t>(stream));
+}
+
+int raft_b200_encoder_prepare(int variant, int norm_type, int out_dim, const raft_encoder_weights* weights,
+                              void* prepared, size_t prepared_bytes, void* stream) {
+  return raft_b200_encoder_prepare_ex(variant, norm_type, out_dim, weights, RAFT_CONVENTIONS_TF, prepared, prepared_bytes,
+                                      stream);
 }
 
 int raft_b200_encoder_workspace_bytes(int variant, int N, int H, int W, size_t* bytes) {
@@ -855,6 +874,11 @@ int raft_b200_encode_pair(int variant, const void* fnet_prepared, int fnet_norm,
   const PairWs P = pair_ws_layout(workspace, variant, N, H, W, cnet_dim);
   if (P.total > workspace_bytes) return RAFT_ERR_WORKSPACE;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  // image1's stem planes serve fnet and cnet, so both blobs must share one convention
+  int fconv = 0, cconv = 0;
+  RAFT_TRY(enc_conventions(fnet_prepared, enc_layout(variant, fnet_dim), st, &fconv));
+  RAFT_TRY(enc_conventions(cnet_prepared, enc_layout(variant, cnet_dim), st, &cconv));
+  if (fconv != cconv) return RAFT_ERR_BAD_ARG;
   PairStreams* ps = nullptr;
   RAFT_TRY(pair_streams(st, &ps));
   cudaStream_t sa = ps->s[0], sb = ps->s[1], sc = ps->s[2];
@@ -864,7 +888,7 @@ int raft_b200_encode_pair(int variant, const void* fnet_prepared, int fnet_norm,
   // first and C reads them from A's workspace.
   RAFT_CUDA_TRY(cudaEventRecord(ps->fork, st));
   for (cudaStream_t s : {sa, sb, sc}) RAFT_CUDA_TRY(cudaStreamWaitEvent(s, ps->fork, 0));
-  int status = encoder_stem_im2col(variant, image1, N, H, W, 1, P.enc[0], sa);
+  int status = encoder_stem_im2col(variant, image1, N, H, W, 1, fconv, P.enc[0], sa);
   if (!status) status = (int)cudaEventRecord(ps->stem, sa);
   if (!status) status = encoder_forward(variant, fnet_norm, fnet_dim, fnet_prepared, image2, N, H, W, 0, 1, fmap2, P.enc[1],
                                         enc_bytes, sb);
@@ -901,11 +925,13 @@ int raft_b200_conv2d(const float* x, const float* kernel, const float* bias, int
   return launch(conv_simt_kernel, grid, 256, 0, reinterpret_cast<cudaStream_t>(stream), p);
 }
 
-int raft_b200_forward_loop(int variant, const void* prepared, const float* const pyr[], int levels, int radius,
-                           float* net, const float* inp, float* coords1, float* const flow_up[], int iters, int B,
-                           int h, int w, void* workspace, size_t workspace_bytes, int precision, void* stream) {
+int raft_b200_forward_loop_ex(int variant, const void* prepared, const float* const pyr[], int levels, int radius,
+                              float* net, const float* inp, float* coords1, float* const flow_up[], int iters, int B,
+                              int h, int w, void* workspace, size_t workspace_bytes, int precision, int sampler,
+                              void* stream) {
   if (!pyr || !net || !inp || !coords1 || !flow_up || iters < 0) return RAFT_ERR_BAD_ARG;
   if (levels < 1 || levels > RAFT_MAX_LEVELS || radius < 0) return RAFT_ERR_BAD_ARG;
+  RAFT_TRY(check_sampler(sampler));
   UpdateCtx c;
   RAFT_TRY(make_ctx(c, variant, prepared, B, h, w, workspace, workspace_bytes, precision, stream));
   const VariantDims d = variant_dims(variant);
@@ -927,14 +953,15 @@ int raft_b200_forward_loop(int variant, const void* prepared, const float* const
     if (precision == RAFT_PREC_F16X2) {
       if (prof) RAFT_CUDA_TRY(cudaEventRecord(g_prof.ev[i][0], c.stream));
       RAFT_TRY(lookup_launch(pyr, coords1, B, h, w, levels, radius, nullptr, 0, W.corr_hi, W.corr_lo, d.s_corr, d.s_corr,
-                             c.stream, W.flow, W.fim_hi, W.fim_lo));                                // model.py:95 (+ convf1's im2col)
+                             sampler, c.stream, W.flow, W.fim_hi, W.fim_lo));                                // model.py:95 (+ convf1's im2col)
       if (prof) RAFT_CUDA_TRY(cudaEventRecord(g_prof.ev[i][1], c.stream));
       c.fim_ready = true;
       RAFT_TRY(update_block_tc(c, net, W.delta, mask, coords1));                                    // :99, :102 (fused advance)
       c.fim_ready = false;
       if (prof) RAFT_CUDA_TRY(cudaEventRecord(g_prof.ev[i][2], c.stream));
     } else {
-      RAFT_TRY(lookup_launch(pyr, coords1, B, h, w, levels, radius, W.corr, d.corr_ch, nullptr, nullptr, 0, 0, c.stream));
+      RAFT_TRY(lookup_launch(pyr, coords1, B, h, w, levels, radius, W.corr, d.corr_ch, nullptr, nullptr, 0, 0, sampler,
+                             c.stream));
       RAFT_TRY(update_core_fp32(c, net, W.delta, mask));
       RAFT_TRY(launch(flow_advance_kernel, grid_for(npix), 256, 0, c.stream, coords1, W.delta, W.flow, B, h, w));  // :102
     }
@@ -946,6 +973,13 @@ int raft_b200_forward_loop(int variant, const void* prepared, const float* const
     }
   }
   return raft_launch_status();
+}
+
+int raft_b200_forward_loop(int variant, const void* prepared, const float* const pyr[], int levels, int radius,
+                           float* net, const float* inp, float* coords1, float* const flow_up[], int iters, int B,
+                           int h, int w, void* workspace, size_t workspace_bytes, int precision, void* stream) {
+  return raft_b200_forward_loop_ex(variant, prepared, pyr, levels, radius, net, inp, coords1, flow_up, iters, B, h, w,
+                                   workspace, workspace_bytes, precision, RAFT_SAMPLER_TF, stream);
 }
 
 // Training convolutions (conv_train.cuh).  workspace == null: *workspace_bytes = the size the shape needs, nothing runs.

@@ -2,12 +2,16 @@
 //   conv1 7x7 s2 (Cin = 3, K = 147: CUDA cores, image normalisation 2*(x/255)-1 fused into the load)
 //   6 ResBlocks (extractor.py:19-49): 3x3 convs on conv_tc_kernel; stride-2 convs fetch their A operand with
 //   TMA elementStrides = 2 (Keras 'same' is asymmetric there: pad 0 before / 1 after); 1x1 s2 downsample.
+// Conventions (recorded in the prepared blob): RAFT_CONVENTIONS_TF as above with norm epsilon 1e-3, or
+// RAFT_CONVENTIONS_PYTORCH -- the original RAFT's symmetric padding ((k-1)/2 at every stride) and epsilon 1e-5.
 //   conv2 1x1.
 // Norms: 'batch' in inference is a per-channel affine folded into the conv epilogue (everything fuses);
 // 'instance' (and 'batch' in training) need statistics of the raw conv output: two deterministic reduction
 // passes + one apply kernel that also does ReLU, the residual add and the fp16 hi/lo re-split.
 #pragma once
 #include <algorithm>
+#include <mutex>
+#include <unordered_map>
 
 #include "lookup.cuh"
 #include "update.cuh"
@@ -31,6 +35,7 @@ struct EncLayout {
   EncNormSlot bn1[6], bn2[6], bnd[6];
   int has_ds[6], bc[6], bstride[6];
   TcWeightSlot conv2;
+  size_t conventions;                         // one byte: RAFT_CONVENTIONS_*
   size_t total;
 };
 
@@ -63,6 +68,7 @@ inline EncLayout enc_layout(int variant, int out_dim) {
     cin = c;
   }
   L.conv2 = conv_slot(1, 1, cin, out_dim);
+  L.conventions = take(1);
   L.total = off;
   return L;
 }
@@ -115,7 +121,39 @@ inline int enc_pack_conv(const raft_conv& cv, int kh, int kw, int cin, int cout,
   return tc_pack_weights(base, s, src, 1, nullptr, flatten, st);
 }
 
-inline int enc_pack_norm(const raft_norm& nm, const EncNormSlot& s, int norm_type, uint8_t* base, cudaStream_t st) {
+inline float enc_norm_eps(int conventions) { return conventions == RAFT_CONVENTIONS_PYTORCH ? 1e-5f : 1e-3f; }
+
+// The convention of every blob prepared in this process, by its address, as the last prepare at that address set it:
+// encoder_forward reads it on the host without a device round trip (and so under graph capture).  Entries are never
+// dropped, so a raw copy of another blob onto a prepared address reads as that address's last prepare
+// (include/raft_b200.h).
+inline std::mutex& enc_conv_mutex() { static std::mutex m; return m; }
+inline std::unordered_map<const void*, int>& enc_conv_table() { static std::unordered_map<const void*, int> t; return t; }
+inline void enc_conventions_record(const void* prepared, int conventions) {
+  std::lock_guard<std::mutex> g(enc_conv_mutex());
+  enc_conv_table()[prepared] = conventions;
+}
+// The blob's convention: from the table, or (a blob this process did not prepare at this address) read back from the
+// blob's own field once -- a synchronisation, refused under capture.
+inline int enc_conventions(const void* prepared, const EncLayout& L, cudaStream_t st, int* conventions) {
+  {
+    std::lock_guard<std::mutex> g(enc_conv_mutex());
+    const auto it = enc_conv_table().find(prepared);
+    if (it != enc_conv_table().end()) { *conventions = it->second; return RAFT_OK; }
+  }
+  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+  RAFT_CUDA_TRY(cudaStreamIsCapturing(st, &cs));
+  if (cs != cudaStreamCaptureStatusNone) return RAFT_ERR_UNSUPPORTED;
+  uint8_t v = 0;
+  RAFT_CUDA_TRY(cudaMemcpyAsync(&v, reinterpret_cast<const uint8_t*>(prepared) + L.conventions, 1, cudaMemcpyDeviceToHost, st));
+  RAFT_CUDA_TRY(cudaStreamSynchronize(st));
+  if (v != RAFT_CONVENTIONS_TF && v != RAFT_CONVENTIONS_PYTORCH) return RAFT_ERR_BAD_ARG;
+  enc_conventions_record(prepared, v);
+  *conventions = v;
+  return RAFT_OK;
+}
+
+inline int enc_pack_norm(const raft_norm& nm, const EncNormSlot& s, int norm_type, float eps, uint8_t* base, cudaStream_t st) {
   if (norm_type == NORM_NONE) return 0;
   if (!nm.gamma || !nm.beta) return RAFT_ERR_BAD_ARG;
   float* g = reinterpret_cast<float*>(base + s.gamma);
@@ -125,30 +163,33 @@ inline int enc_pack_norm(const raft_norm& nm, const EncNormSlot& s, int norm_typ
   if (norm_type == NORM_BATCH) {
     if (!nm.moving_mean || !nm.moving_variance) return RAFT_ERR_BAD_ARG;
     return launch(bn_fold_kernel, ceil_div(s.C, 128), 128, 0, st, nm.gamma, nm.beta, nm.moving_mean, nm.moving_variance,
-                  1e-3f, s.C, reinterpret_cast<float*>(base + s.fscale), reinterpret_cast<float*>(base + s.fshift));
+                  eps, s.C, reinterpret_cast<float*>(base + s.fscale), reinterpret_cast<float*>(base + s.fshift));
   }
   return raft_launch_status();
 }
 
-inline int encoder_prepare(int variant, int norm_type, int out_dim, const raft_encoder_weights* w, void* prepared,
-                           size_t bytes, cudaStream_t st) {
+inline int encoder_prepare(int variant, int norm_type, int out_dim, const raft_encoder_weights* w, int conventions,
+                           void* prepared, size_t bytes, cudaStream_t st) {
   const EncLayout L = enc_layout(variant, out_dim);
   if (L.total > bytes) return RAFT_ERR_WORKSPACE;
   const EncSpec S = enc_spec(variant);
+  const float eps = enc_norm_eps(conventions);
   uint8_t* base = reinterpret_cast<uint8_t*>(prepared);
   RAFT_CUDA_TRY(cudaMemsetAsync(base, 0, L.total, st));
+  RAFT_CUDA_TRY(cudaMemsetAsync(base + L.conventions, conventions, 1, st));
+  enc_conventions_record(prepared, conventions);
   RAFT_TRY(enc_pack_conv(w->conv1, 7, 7, 3, S.c0, L.conv1, true, base, st));
-  RAFT_TRY(enc_pack_norm(w->norm1, L.norm1, norm_type, base, st));
+  RAFT_TRY(enc_pack_norm(w->norm1, L.norm1, norm_type, eps, base, st));
   int cin = S.c0;
   for (int k = 0; k < 6; ++k) {
     const int c = L.bc[k];
     RAFT_TRY(enc_pack_conv(w->block[k].conv1, 3, 3, cin, c, L.bc1[k], false, base, st));
     RAFT_TRY(enc_pack_conv(w->block[k].conv2, 3, 3, c, c, L.bc2[k], false, base, st));
-    RAFT_TRY(enc_pack_norm(w->block[k].norm1, L.bn1[k], norm_type, base, st));
-    RAFT_TRY(enc_pack_norm(w->block[k].norm2, L.bn2[k], norm_type, base, st));
+    RAFT_TRY(enc_pack_norm(w->block[k].norm1, L.bn1[k], norm_type, eps, base, st));
+    RAFT_TRY(enc_pack_norm(w->block[k].norm2, L.bn2[k], norm_type, eps, base, st));
     if (L.has_ds[k]) {
       RAFT_TRY(enc_pack_conv(w->block[k].downsample, 1, 1, cin, c, L.bds[k], false, base, st));
-      RAFT_TRY(enc_pack_norm(w->block[k].downsample_norm, L.bnd[k], norm_type, base, st));
+      RAFT_TRY(enc_pack_norm(w->block[k].downsample_norm, L.bnd[k], norm_type, eps, base, st));
     }
     cin = c;
   }
@@ -161,6 +202,7 @@ struct EncCtx {
   const uint8_t* prep; EncLayout L; EncWs W; cudaStream_t st;
   int N, norm_type, stats;    // stats: 1 = statistics from the data (instance, or batch in training)
   int per_image;              // instance: one group per image; batch-training: one group
+  int conventions;            // RAFT_CONVENTIONS_*: padding of the stride-2 convolutions, norm epsilon
 };
 
 // y (npix, C) raw conv output -> normalised, activated, (+skip), re-split.
@@ -174,7 +216,7 @@ inline int enc_norm_apply(const EncCtx& c, const EncNormSlot& ns, const float* y
   // (Finalisation is a separate launch: inside norm_stats_kernel the merge of C channels by the last block of a group would
   //  be serial, where norm_final_kernel spreads it over G*C warps.)
   RAFT_TRY(launch(norm_stats_kernel, dim3((unsigned)G, kNormSplit), 256, 0, c.st, y, Pg, C, kNormSplit, c.W.part));
-  RAFT_TRY(launch(norm_final_kernel, ceil_div(G * C * 32, 256), 256, 0, c.st, c.W.part, G, C, kNormSplit, gamma, 1e-3f,
+  RAFT_TRY(launch(norm_final_kernel, ceil_div(G * C * 32, 256), 256, 0, c.st, c.W.part, G, C, kNormSplit, gamma, enc_norm_eps(c.conventions),
                   c.W.mean, c.W.mult));
   return launch(norm_apply_kernel, grid_for(npix * (pad64(C) / 8)), 256, 0, c.st, y, npix, P, C, c.per_image, c.W.mean,
                 c.W.mult, beta, relu, skip32, skip_hi, skip_lo, out32, hi, lo, pad64(C));
@@ -197,8 +239,9 @@ inline int enc_conv_tc(const EncCtx& c, const TcWeightSlot& cs, int cout, const 
   p.nseg = 1; p.seg_chunks[0] = cs.cin_pad / kChunkK; p.seg_c0[0] = 0;
   p.stride = stride;
   // Keras 'same': stride 1 -> (k-1)/2 before; stride 2 on even input -> total k-2, before = (k-2)/2 (0 for 3x3);
-  // 1x1 convs are 'valid' (no padding).
-  if (stride == 1) { p.ph = (cs.kh - 1) / 2; p.pw = (cs.kw - 1) / 2; }
+  // 1x1 convs are 'valid' (no padding).  PyTorch: (k-1)/2 before at every stride -- at stride 2 an odd, negative
+  // first tap coordinate, which TMA fills with zeros like any other out-of-bounds element.
+  if (stride == 1 || c.conventions == RAFT_CONVENTIONS_PYTORCH) { p.ph = (cs.kh - 1) / 2; p.pw = (cs.kw - 1) / 2; }
   else {
     const int tot_h = (Hout - 1) * stride + cs.kh - Hin, tot_w = (Wout - 1) * stride + cs.kw - Win;
     p.ph = (tot_h > 0 ? tot_h : 0) / 2; p.pw = (tot_w > 0 ? tot_w : 0) / 2;
@@ -228,12 +271,14 @@ inline int enc_conv_tc(const EncCtx& c, const TcWeightSlot& cs, int cout, const 
 
 // The stem's operand: the 7x7 s2 input window of every output pixel as 192-channel fp16 planes (E.Ih / E.Il of `ws`).
 // It depends on the images alone, so encoders of the same images can share it (raft_b200_encode_pair).
-inline int encoder_stem_im2col(int variant, const float* images, int N, int H, int W, int image_norm, void* ws,
-                               cudaStream_t st) {
+inline int encoder_stem_im2col(int variant, const float* images, int N, int H, int W, int image_norm, int conventions,
+                               void* ws, cudaStream_t st) {
   const EncWs E = enc_ws_layout(ws, variant, N, H, W);
   const int h = (H + 1) / 2, w = (W + 1) / 2;
   const size_t npix = (size_t)N * h * w;
-  const int tot_h = (h - 1) * 2 + 7 - H, tot_w = (w - 1) * 2 + 7 - W;
+  // twice the pad before: Keras 'same' total (asymmetric on even sizes), or PyTorch's 3 on each side
+  const bool pt = conventions == RAFT_CONVENTIONS_PYTORCH;
+  const int tot_h = pt ? 6 : (h - 1) * 2 + 7 - H, tot_w = pt ? 6 : (w - 1) * 2 + 7 - W;
   const float* src = images;
   if (image_norm) {                                 // normalise once (O32 is free until the first ResBlock finishes)
     const size_t nimg = (size_t)N * H * W * 3;
@@ -255,6 +300,7 @@ inline int encoder_forward(int variant, int norm_type, int out_dim, const void* 
   c.W = enc_ws_layout(ws, variant, N, H, W);
   if (c.W.total > ws_bytes) return RAFT_ERR_WORKSPACE;
   c.st = st; c.N = N; c.norm_type = norm_type;
+  RAFT_TRY(enc_conventions(prepared, c.L, st, &c.conventions));
   c.stats = (norm_type == NORM_INSTANCE) || (norm_type == NORM_BATCH && training);
   c.per_image = norm_type == NORM_INSTANCE;
   const EncSpec S = enc_spec(variant);
@@ -268,7 +314,7 @@ inline int encoder_forward(int variant, int norm_type, int out_dim, const void* 
   {
     const size_t npix = (size_t)N * h * w;
     if (!stem_hi) {
-      RAFT_TRY(encoder_stem_im2col(variant, images, N, H, W, image_norm, ws, st));
+      RAFT_TRY(encoder_stem_im2col(variant, images, N, H, W, image_norm, c.conventions, ws, st));
       stem_hi = E.Ih; stem_lo = E.Il;
     }
     if (!c.stats && pad64(S.c0) != S.c0) {

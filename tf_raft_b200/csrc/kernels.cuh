@@ -115,7 +115,63 @@ struct LookupParams {
   const float* im_flow; __half* im_hi; __half* im_lo; int im_B, im_h, im_w;
 };
 
-__global__ void __launch_bounds__(256) corr_lookup_kernel(const LookupParams p) {
+// ------------------------------------------------------------------------------------------------
+// The grid_sample sampler (RAFT_SAMPLER_GRID): what the original PyTorch RAFT's lookup computes,
+// F.grid_sample(align_corners=True, padding_mode='zeros') after RAFT's own normalisation.  Per axis of
+// size n, for the level coordinate v = fl(fl(c * 2^-l) + d), op by op in fp32 with no FMA:
+//   g  = fl(fl(fl(2 * v) * fl(1 / (n - 1))) - 1)         RAFT's 2 * xgrid / (W - 1) - 1 as ATen's CUDA true divide
+//                                                        computes it: by a CPU scalar as a product with its reciprocal
+//   ix = fl(fl(fl(g + 1) / 2) * (n - 1))                 ATen grid_sampler_unnormalize (align_corners)
+//   ix = -100 unless -2^31 <= ix <= 2^31 (NaN included)  ATen safe_downgrade_to_int_range
+//   x0 = floor(ix), x1 = x0 + 1; weights w(x0) = fl(x1 - ix), w(x1) = fl(ix - x0)
+// A corner outside [0, n-1] is never read and adds nothing (n = 1: 2v/0 is +-inf or NaN, so every tap is 0).
+// Sum order of a tap: acc = +0, then for the corners (y0,x0), (y0,x1), (y1,x0), (y1,x1) in that order, if the
+// corner is in the frame, acc = fl(acc + fl(fl(wy * wx) * texel)) -- an in-frame corner adds even at weight 0.
+// ------------------------------------------------------------------------------------------------
+struct GridAxis { float wf, wc; int i0, i1; };   // weights of x0 / x1; indices, -1 when outside the frame
+__device__ __forceinline__ float grid_unnormalize(float v, float nm1) {
+  const float g = __fsub_rn(__fmul_rn(__fmul_rn(2.0f, v), __fdiv_rn(1.0f, nm1)), 1.0f);
+  const float ix = __fmul_rn(__fdiv_rn(__fadd_rn(g, 1.0f), 2.0f), nm1);
+  return (ix >= -2147483648.0f && ix <= 2147483648.0f) ? ix : -100.0f;
+}
+__device__ __forceinline__ GridAxis grid_axis(float v, int n) {
+  const float nm1 = (float)(n - 1);
+  const float ix = grid_unnormalize(v, nm1);
+  const float x0 = floorf(ix), x1 = __fadd_rn(x0, 1.0f);
+  GridAxis a;
+  a.wf = __fsub_rn(x1, ix);
+  a.wc = __fsub_rn(ix, x0);
+  a.i0 = (x0 >= 0.0f && x0 <= nm1) ? (int)x0 : -1;
+  a.i1 = (x1 >= 0.0f && x1 <= nm1) ? (int)x1 : -1;
+  return a;
+}
+// One tap from its two axis set-ups and the four texels (read only where in frame), in the order stated above.
+__device__ __forceinline__ float grid_combine(const GridAxis& ax, const GridAxis& ay, float x00, float x01, float x10,
+                                              float x11) {
+  float acc = 0.0f;
+  if (ay.i0 >= 0 && ax.i0 >= 0) acc = __fadd_rn(acc, __fmul_rn(__fmul_rn(ay.wf, ax.wf), x00));
+  if (ay.i0 >= 0 && ax.i1 >= 0) acc = __fadd_rn(acc, __fmul_rn(__fmul_rn(ay.wf, ax.wc), x01));
+  if (ay.i1 >= 0 && ax.i0 >= 0) acc = __fadd_rn(acc, __fmul_rn(__fmul_rn(ay.wc, ax.wf), x10));
+  if (ay.i1 >= 0 && ax.i1 >= 0) acc = __fadd_rn(acc, __fmul_rn(__fmul_rn(ay.wc, ax.wc), x11));
+  return acc;
+}
+__device__ __forceinline__ float sample_grid(const float* __restrict__ img, int H, int W, float px, float py) {
+  const GridAxis ax = grid_axis(px, W), ay = grid_axis(py, H);
+  const float x00 = (ay.i0 >= 0 && ax.i0 >= 0) ? __ldg(img + ay.i0 * W + ax.i0) : 0.0f;
+  const float x01 = (ay.i0 >= 0 && ax.i1 >= 0) ? __ldg(img + ay.i0 * W + ax.i1) : 0.0f;
+  const float x10 = (ay.i1 >= 0 && ax.i0 >= 0) ? __ldg(img + ay.i1 * W + ax.i0) : 0.0f;
+  const float x11 = (ay.i1 >= 0 && ax.i1 >= 0) ? __ldg(img + ay.i1 * W + ax.i1) : 0.0f;
+  return grid_combine(ax, ay, x00, x01, x10, x11);
+}
+// The sampler of one lookup: kGrid = false is tf-raft's floor/ceil sampler, true the grid_sample one.
+template <bool kGrid>
+__device__ __forceinline__ float sample_tap(const float* __restrict__ img, int H, int W, float px, float py) {
+  if constexpr (kGrid) return sample_grid(img, H, W, px, py);
+  else return sample_floor_ceil(img, H, W, px, py);
+}
+
+template <bool kGrid>
+__device__ __forceinline__ void corr_lookup_body(const LookupParams& p) {
   __shared__ float4 axis_smem[8 * 32];                          // per warp: 16 x-axis + 16 y-axis tap set-ups
   const int warps_per_block = blockDim.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -143,12 +199,18 @@ __global__ void __launch_bounds__(256) corr_lookup_kernel(const LookupParams p) 
         const int i = isy ? lane - side : lane;
         const float cc = isy ? cy : cx;
         const int dim = isy ? H : W;
-        const float g = fminf(fmaxf(__fadd_rn(cc, (float)(i - p.radius)), 0.0f), (float)(dim - 1));   // centroid + delta, clamp
-        const float g0 = floorf(g), g1 = ceilf(g);
-        ax[(isy ? 16 : 0) + i] = make_float4(__fsub_rn(g1, g), __fsub_rn(g, g0), __int_as_float((int)g0), __int_as_float((int)g1));
+        if constexpr (kGrid) {
+          const GridAxis ga = grid_axis(__fadd_rn(cc, (float)(i - p.radius)), dim);
+          ax[(isy ? 16 : 0) + i] = make_float4(ga.wf, ga.wc, __int_as_float(ga.i0), __int_as_float(ga.i1));
+        } else {
+          const float g = fminf(fmaxf(__fadd_rn(cc, (float)(i - p.radius)), 0.0f), (float)(dim - 1));   // centroid + delta, clamp
+          const float g0 = floorf(g), g1 = ceilf(g);
+          ax[(isy ? 16 : 0) + i] = make_float4(__fsub_rn(g1, g), __fsub_rn(g, g0), __int_as_float((int)g0), __int_as_float((int)g1));
+        }
       }
       __syncwarp();
-      TapGather tg[kMaxIter];
+      TapGather tg[kGrid ? 1 : kMaxIter];
+      GridAxis gx[kGrid ? kMaxIter : 1], gy[kGrid ? kMaxIter : 1];
       float x00[kMaxIter], x01[kMaxIter], x10[kMaxIter], x11[kMaxIter];
 #pragma unroll
       for (int i = 0; i < kMaxIter; ++i) {
@@ -156,16 +218,26 @@ __global__ void __launch_bounds__(256) corr_lookup_kernel(const LookupParams p) 
         const int a = t / side, b2 = t - a * side;
         const float4 sx = ax[a], sy = ax[16 + b2];               // (w1, w0, i0, i1) per axis
         const int ix0 = __float_as_int(sx.z), ix1 = __float_as_int(sx.w), iy0 = __float_as_int(sy.z), iy1 = __float_as_int(sy.w);
-        tg[i].c00 = __fmul_rn(sy.x, sx.x); tg[i].c01 = __fmul_rn(sy.x, sx.y);
-        tg[i].c10 = __fmul_rn(sy.y, sx.x); tg[i].c11 = __fmul_rn(sy.y, sx.y);
-        x00[i] = __ldg(img + iy0 * W + ix0); x01[i] = __ldg(img + iy0 * W + ix1);
-        x10[i] = __ldg(img + iy1 * W + ix0); x11[i] = __ldg(img + iy1 * W + ix1);
+        if constexpr (kGrid) {                                   // corners outside the frame are not read
+          gx[i] = GridAxis{sx.x, sx.y, ix0, ix1};
+          gy[i] = GridAxis{sy.x, sy.y, iy0, iy1};
+          x00[i] = (iy0 >= 0 && ix0 >= 0) ? __ldg(img + iy0 * W + ix0) : 0.0f;
+          x01[i] = (iy0 >= 0 && ix1 >= 0) ? __ldg(img + iy0 * W + ix1) : 0.0f;
+          x10[i] = (iy1 >= 0 && ix0 >= 0) ? __ldg(img + iy1 * W + ix0) : 0.0f;
+          x11[i] = (iy1 >= 0 && ix1 >= 0) ? __ldg(img + iy1 * W + ix1) : 0.0f;
+        } else {
+          tg[i].c00 = __fmul_rn(sy.x, sx.x); tg[i].c01 = __fmul_rn(sy.x, sx.y);
+          tg[i].c10 = __fmul_rn(sy.y, sx.x); tg[i].c11 = __fmul_rn(sy.y, sx.y);
+          x00[i] = __ldg(img + iy0 * W + ix0); x01[i] = __ldg(img + iy0 * W + ix1);
+          x10[i] = __ldg(img + iy1 * W + ix0); x11[i] = __ldg(img + iy1 * W + ix1);
+        }
       }
 #pragma unroll
       for (int i = 0; i < kMaxIter; ++i) {
         const int t = lane + 32 * i;
         if (t < ntap) {
-          const float v = tap_combine(tg[i], x00[i], x01[i], x10[i], x11[i]);
+          const float v = kGrid ? grid_combine(gx[i], gy[i], x00[i], x01[i], x10[i], x11[i])
+                                : tap_combine(tg[kGrid ? 0 : i], x00[i], x01[i], x10[i], x11[i]);
           const int ch = l * ntap + t;
           if (p.out) p.out[(size_t)q * p.out_stride + ch] = v;
           if (p.out_hi) {
@@ -181,7 +253,7 @@ __global__ void __launch_bounds__(256) corr_lookup_kernel(const LookupParams p) 
         const int a = t / side, b2 = t - a * side;
         const float px = __fadd_rn(cx, (float)(a - p.radius));   // centroid + delta (corr.py:143)
         const float py = __fadd_rn(cy, (float)(b2 - p.radius));
-        const float v = sample_floor_ceil(img, H, W, px, py);
+        const float v = sample_tap<kGrid>(img, H, W, px, py);
         const int ch = l * ntap + t;
         if (p.out) p.out[(size_t)q * p.out_stride + ch] = v;
         if (p.out_hi) {
@@ -201,6 +273,8 @@ __global__ void __launch_bounds__(256) corr_lookup_kernel(const LookupParams p) 
     }
   }
 }
+__global__ void __launch_bounds__(256) corr_lookup_kernel(const LookupParams p) { corr_lookup_body<false>(p); }
+__global__ void __launch_bounds__(256) corr_lookup_grid_kernel(const LookupParams p) { corr_lookup_body<true>(p); }
 
 // ------------------------------------------------------------------------------------------------
 // fp32 correlation (RAFT_PREC_FP32): out[b, q, n] = <f1[b,q,:], f2[b,n,:]> / sqrt(C)  (corr.py:154-162)

@@ -12,6 +12,13 @@
 //      coordinate => 0, x-major tap order, fl(fl(c / 2^l) + d)).
 // About 140 warp instructions per item instead of the 469 of the gather-per-tap kernel (kernels.cuh, kept for other
 // radii / level counts and as the per-item escape when a footprint does not fit the window).
+//
+// corr_lookup_win_grid_kernel is the same kernel with the grid_sample sampler (RAFT_SAMPLER_GRID, kernels.cuh): the
+// set-up lanes compute RAFT's normalisation and ATen's unnormalisation op by op, a corner outside the level is marked
+// (offset -1) and never read, and the footprint is the intersection of the taps' corners with the level -- it may be
+// empty.  Its corners still span at most 2r+2 texels per axis, so the window bound holds.  Sum order of one tap: acc =
+// +0, then (y0,x0), (y0,x1), (y1,x0), (y1,x1), each in-frame corner adding fl(fl(wy * wx) * texel) (weight 0 included,
+// so a NaN texel there reaches the tap as in ATen).
 #pragma once
 #include "kernels.cuh"
 
@@ -28,8 +35,8 @@ struct LookupItem {
   float cx, cy;          // level coordinates (escape path only)
 };
 
-template <int R, int L, bool kVec, bool kHalf>
-__global__ void __launch_bounds__(256, 4) corr_lookup_win_kernel(const LookupParams p) {
+template <int R, int L, bool kVec, bool kHalf, bool kGrid>
+__device__ __forceinline__ void corr_lookup_win_body(const LookupParams& p) {
   constexpr int S = 2 * R + 1, NT = S * S;
   constexpr int NJ = (S + 2) / 3;                                   // taps per lane
   constexpr int NV = kVec ? 2 : 6;                                  // window registers per lane (float4 / float)
@@ -82,16 +89,37 @@ __global__ void __launch_bounds__(256, 4) corr_lookup_win_kernel(const LookupPar
 
   auto stage = [&](float2 c, const float* img_q) {                  // set-up + loads of one item
     const float cx = __fmul_rn(c.x, inv), cy = __fmul_rn(c.y, inv); // coords / 2**i  (corr.py:141)
-    const float g = fminf(fmaxf(__fadd_rn(isy ? cy : cx, fi), 0.0f), fmax_dim);   // centroid + delta, clamp
-    const float g0 = floorf(g), g1 = ceilf(g);
-    const int i0 = (int)g0, i1 = (int)g1;
-    const int bx = __shfl_sync(0xffffffffu, i0, 0), by = __shfl_sync(0xffffffffu, i0, S);
-    const int ex = __shfl_sync(0xffffffffu, i1, S - 1), ey = __shfl_sync(0xffffffffu, i1, 2 * S - 1);
+    int i0, i1, lo, hi;                                             // corners; this lane's share of the footprint
+    float g, g0, g1;                                                // coordinate and its floor / ceil corners
+    if constexpr (kGrid) {
+      // the taps' ix are non-decreasing in the tap index wherever a corner can lie in the level (-100 only stands for
+      // values far outside or NaN, which are so for every tap): tap 0's x0 and tap S-1's x0 + 1, clipped to the level,
+      // bound every in-frame corner.  lo > hi: no corner of this axis is in the frame.
+      g = grid_unnormalize(__fadd_rn(isy ? cy : cx, fi), fmax_dim);
+      g0 = floorf(g);
+      g1 = __fadd_rn(g0, 1.0f);
+      i0 = (g0 >= 0.0f && g0 <= fmax_dim) ? (int)g0 : -1;
+      i1 = (g1 >= 0.0f && g1 <= fmax_dim) ? (int)g1 : -1;
+      lo = (int)fminf(fmaxf(g0, 0.0f), __fadd_rn(fmax_dim, 1.0f));
+      hi = (int)fmaxf(fminf(g1, fmax_dim), -1.0f);
+    } else {
+      g = fminf(fmaxf(__fadd_rn(isy ? cy : cx, fi), 0.0f), fmax_dim);   // centroid + delta, clamp
+      g0 = floorf(g);
+      g1 = ceilf(g);
+      i0 = (int)g0; i1 = (int)g1;
+      lo = i0; hi = i1;
+    }
+    const int bx = __shfl_sync(0xffffffffu, lo, 0), by = __shfl_sync(0xffffffffu, lo, S);
+    const int ex = __shfl_sync(0xffffffffu, hi, S - 1), ey = __shfl_sync(0xffffffffu, hi, 2 * S - 1);
     const int bxa = kVec ? (bx & ~3) : bx;                          // first window column (16-byte aligned when vectorised)
-    it.w1 = __fsub_rn(g1, g);
+    it.w1 = __fsub_rn(g1, g);                                       // weights of the floor / ceil corner
     it.w0 = __fsub_rn(g, g0);
     it.off0 = (isy ? (i0 - by) * kWinPitch : i0 - bxa) * 4;           // BYTE offsets inside the window
     it.off1 = (isy ? (i1 - by) * kWinPitch : i1 - bxa) * 4;
+    if constexpr (kGrid) {                                          // -1: the corner lies outside the level
+      if (i0 < 0) it.off0 = -1;
+      if (i1 < 0) it.off1 = -1;
+    }
     it.ok = (ex - bxa < 16 && ey - by < kWinRows) ? 1 : 0;
     it.cx = cx;
     it.cy = cy;
@@ -149,10 +177,20 @@ __global__ void __launch_bounds__(256, 4) corr_lookup_win_kernel(const LookupPar
           if (S % 3 == 0 || bq + 3 * j < S) {
             const float4 sy = ax[16 + bq + 3 * j];
             const int oy0 = __float_as_int(sy.z), oy1 = __float_as_int(sy.w);
-            float v = __fmul_rn(__fmul_rn(sy.x, sx.x), *reinterpret_cast<const float*>(w0p + oy0));   // corr.py:68, left to right
-            v = __fadd_rn(v, __fmul_rn(__fmul_rn(sy.x, sx.y), *reinterpret_cast<const float*>(w1p + oy0)));
-            v = __fadd_rn(v, __fmul_rn(__fmul_rn(sy.y, sx.x), *reinterpret_cast<const float*>(w0p + oy1)));
-            v = __fadd_rn(v, __fmul_rn(__fmul_rn(sy.y, sx.y), *reinterpret_cast<const float*>(w1p + oy1)));
+            float v;
+            if constexpr (kGrid) {
+              const int ox0 = __float_as_int(sx.z), ox1 = __float_as_int(sx.w);
+              v = 0.0f;
+              if (oy0 >= 0 && ox0 >= 0) v = __fadd_rn(v, __fmul_rn(__fmul_rn(sy.x, sx.x), *reinterpret_cast<const float*>(w0p + oy0)));
+              if (oy0 >= 0 && ox1 >= 0) v = __fadd_rn(v, __fmul_rn(__fmul_rn(sy.x, sx.y), *reinterpret_cast<const float*>(w1p + oy0)));
+              if (oy1 >= 0 && ox0 >= 0) v = __fadd_rn(v, __fmul_rn(__fmul_rn(sy.y, sx.x), *reinterpret_cast<const float*>(w0p + oy1)));
+              if (oy1 >= 0 && ox1 >= 0) v = __fadd_rn(v, __fmul_rn(__fmul_rn(sy.y, sx.y), *reinterpret_cast<const float*>(w1p + oy1)));
+            } else {
+              v = __fmul_rn(__fmul_rn(sy.x, sx.x), *reinterpret_cast<const float*>(w0p + oy0));   // corr.py:68, left to right
+              v = __fadd_rn(v, __fmul_rn(__fmul_rn(sy.x, sx.y), *reinterpret_cast<const float*>(w1p + oy0)));
+              v = __fadd_rn(v, __fmul_rn(__fmul_rn(sy.y, sx.x), *reinterpret_cast<const float*>(w0p + oy1)));
+              v = __fadd_rn(v, __fmul_rn(__fmul_rn(sy.y, sx.y), *reinterpret_cast<const float*>(w1p + oy1)));
+            }
             if constexpr (kHalf) {
               __half hh, ll;
               split_f16(v, hh, ll);
@@ -167,7 +205,7 @@ __global__ void __launch_bounds__(256, 4) corr_lookup_win_kernel(const LookupPar
     } else {                                                        // escape: gather per tap (never taken in practice)
       for (int t = lane; t < NT; t += 32) {
         const int ta = t / S, tb = t - ta * S;
-        const float v = sample_floor_ceil(img_base + img_cur, H, W, __fadd_rn(ecx, (float)(ta - R)), __fadd_rn(ecy, (float)(tb - R)));
+        const float v = sample_tap<kGrid>(img_base + img_cur, H, W, __fadd_rn(ecx, (float)(ta - R)), __fadd_rn(ecy, (float)(tb - R)));
         if constexpr (kHalf) {
           __half hh, ll;
           split_f16(v, hh, ll);
@@ -191,10 +229,32 @@ __global__ void __launch_bounds__(256, 4) corr_lookup_win_kernel(const LookupPar
     flow_im2col_rider(p.im_flow, p.im_B, p.im_h, p.im_w, p.im_hi, p.im_lo, (size_t)blockIdx.x * blockDim.x + threadIdx.x,
                       (size_t)gridDim.x * blockDim.x);
 }
+template <int R, int L, bool kVec, bool kHalf>
+__global__ void __launch_bounds__(256, 4) corr_lookup_win_kernel(const LookupParams p) {
+  corr_lookup_win_body<R, L, kVec, kHalf, false>(p);
+}
+template <int R, int L, bool kVec, bool kHalf>
+__global__ void __launch_bounds__(256, 4) corr_lookup_win_grid_kernel(const LookupParams p) {
+  corr_lookup_win_body<R, L, kVec, kHalf, true>(p);
+}
 
-// The window kernel instantiation for (radius, levels) in {(4,4), (3,4)}; null when the configuration has none.
+// The window kernel instantiation for (radius, levels) in {(4,4), (3,4)} and the sampler (RAFT_SAMPLER_*); null when
+// the configuration has none.
 using LookupKernel = void (*)(LookupParams);
-inline LookupKernel lookup_win_kernel(const LookupParams& p, int levels, int radius) {
+template <template <int, int, bool, bool> class K>
+struct WinKernels {
+  static LookupKernel pick(int radius, bool vec, bool half) {
+    if (radius == 4) {
+      if (vec) return half ? K<4, 4, true, true>::fn : K<4, 4, true, false>::fn;
+      return half ? K<4, 4, false, true>::fn : K<4, 4, false, false>::fn;
+    }
+    if (vec) return half ? K<3, 4, true, true>::fn : K<3, 4, true, false>::fn;
+    return half ? K<3, 4, false, true>::fn : K<3, 4, false, false>::fn;
+  }
+};
+template <int R, int L, bool V, bool H> struct WinTf { static constexpr LookupKernel fn = corr_lookup_win_kernel<R, L, V, H>; };
+template <int R, int L, bool V, bool H> struct WinGrid { static constexpr LookupKernel fn = corr_lookup_win_grid_kernel<R, L, V, H>; };
+inline LookupKernel lookup_win_kernel(const LookupParams& p, int levels, int radius, int sampler) {
   const size_t nwork = (size_t)p.nq * levels;
   if (levels != 4 || (radius != 4 && radius != 3) || nwork >= (1u << 31)) return nullptr;
   if ((size_t)p.nq * p.lh[0] * p.lw[0] >= (1u << 31) || (size_t)p.nq * (size_t)(p.out_hi ? p.h_stride : p.out_stride) >= (1u << 31))
@@ -204,12 +264,7 @@ inline LookupKernel lookup_win_kernel(const LookupParams& p, int levels, int rad
     vec = vec && (p.lw[l] % 4 == 0) && ((reinterpret_cast<uintptr_t>(p.pyr[l]) & 15) == 0);
   const bool half = p.out_hi != nullptr;
   if (half == (p.out != nullptr)) return nullptr;                    // exactly one of the two output forms
-  if (radius == 4) {
-    if (vec) return half ? corr_lookup_win_kernel<4, 4, true, true> : corr_lookup_win_kernel<4, 4, true, false>;
-    return half ? corr_lookup_win_kernel<4, 4, false, true> : corr_lookup_win_kernel<4, 4, false, false>;
-  }
-  if (vec) return half ? corr_lookup_win_kernel<3, 4, true, true> : corr_lookup_win_kernel<3, 4, true, false>;
-  return half ? corr_lookup_win_kernel<3, 4, false, true> : corr_lookup_win_kernel<3, 4, false, false>;
+  return sampler == RAFT_SAMPLER_GRID ? WinKernels<WinGrid>::pick(radius, vec, half) : WinKernels<WinTf>::pick(radius, vec, half);
 }
 
 }  // namespace raft

@@ -2,6 +2,8 @@
 
 Parameter names are the reference's Keras attribute paths, kernels HWIO as Keras stores them.  The seeded default
 values are drawn on the CPU in the order of the `add_conv` calls, so they depend on the seed and the layer alone.
+`conventions` selects the torch backend's arithmetic: 'tf-raft' (Keras 'same' padding, eps 1e-3) or 'pytorch' (the
+original RAFT's symmetric padding, eps 1e-5).
 """
 import math
 
@@ -16,8 +18,9 @@ def _same_pads(n_in, k, s):
 
 
 class _Params:
-    def __init__(self, device, seed):
+    def __init__(self, device, seed, conventions='tf-raft'):
         self.device = torch.device(device)
+        self.conventions = conventions
         self.params = {}
         self._gen = torch.Generator(device='cpu')
         self._gen.manual_seed(0 if seed is None else seed)
@@ -58,6 +61,9 @@ class _Params:
         if w is None:
             w = self.params[name + '.kernel'].permute(3, 2, 0, 1).contiguous()
             self._nchw_cache[name] = w
+        if padding == 'same' and self.conventions == 'pytorch':         # nn.Conv2d(padding=(k-1)//2)
+            return F.conv2d(x, w, self.params[name + '.bias'], stride=stride,
+                            padding=((w.shape[2] - 1) // 2, (w.shape[3] - 1) // 2))
         if padding == 'same':
             pt, pb = _same_pads(x.shape[2], w.shape[2], stride)
             pl, pr = _same_pads(x.shape[3], w.shape[3], stride)
@@ -66,7 +72,8 @@ class _Params:
         return F.conv2d(x, w, self.params[name + '.bias'], stride=stride)
 
     def norm(self, x, name, norm_type, training):
-        eps = 1e-3        # tfa InstanceNormalization and keras BatchNormalization both default to 1e-3
+        # tfa InstanceNormalization and keras BatchNormalization both default to 1e-3, nn.InstanceNorm2d / BatchNorm2d to 1e-5
+        eps = 1e-5 if self.conventions == 'pytorch' else 1e-3
         if norm_type is None:
             return x
         g = self.params[name + '.gamma'].view(1, -1, 1, 1)

@@ -127,10 +127,16 @@ class CorrBlock:
 
     Attributes as in the reference: fmap1, fmap2, num_levels, radius, corr_pyramid (list of
     `num_levels` tensors (B*h*w, h>>l, w>>l, 1)).  `precision` ('f16x2' tensor-core path, or 'fp32'
-    CUDA-core path) is a keyword-only extra.
+    CUDA-core path) is a keyword-only extra, and so is `sampler`: 'tf-raft' (the reference's floor / ceil
+    bilinear_sampler) or 'grid_sample' (the original PyTorch RAFT's lookup, F.grid_sample with align_corners=True and
+    zero padding; include/raft_b200.h, raft_sampler).
     """
+    sampler = 'tf-raft'
 
-    def __init__(self, fmap1, fmap2, num_levels=4, radius=4, *, precision=None):
+    def __init__(self, fmap1, fmap2, num_levels=4, radius=4, *, precision=None, sampler='tf-raft'):
+        if sampler not in _lib.SAMPLERS:
+            raise ValueError(f'unknown sampler {sampler!r}; expected one of {", ".join(_lib.SAMPLERS)}')
+        self.sampler = sampler
         self.fmap1 = fmap1
         self.fmap2 = fmap2
         self.num_levels = num_levels
@@ -158,12 +164,12 @@ class CorrBlock:
             raise ValueError(f'coords shape {tuple(coords.shape)} does not match the correlation volume {self._shape}')
         nch = self.num_levels * (2 * self.radius + 1) ** 2
         out = torch.empty((b, h, w, nch), dtype=torch.float32, device=coords.device)
-        _lib.call('corr_lookup', coords.device, _lib.ptr_array(self.corr_pyramid), _lib.ptr(coords), b, h, w,
-                  self.num_levels, self.radius, _lib.ptr(out), nch)
+        _lib.call('corr_lookup_ex', coords.device, _lib.ptr_array(self.corr_pyramid), _lib.ptr(coords), b, h, w,
+                  self.num_levels, self.radius, _lib.ptr(out), nch, _lib.SAMPLERS[self.sampler])
         return out
 
     def correlation(self, fmap1, fmap2):
         """Reference corr.py:154-162 -> (B, h, w, 1, h, w) = fmap1 . fmap2^T / sqrt(C)."""
-        block = CorrBlock(fmap1, fmap2, num_levels=1, radius=self.radius, precision=self.precision)
+        block = CorrBlock(fmap1, fmap2, num_levels=1, radius=self.radius, precision=self.precision, sampler=self.sampler)
         b, h, w = block._shape
         return block.corr_pyramid[0].reshape(b, h, w, 1, h, w)

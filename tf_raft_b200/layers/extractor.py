@@ -7,6 +7,8 @@ backend='torch': IEEE-fp32 cuDNN convolutions through PyTorch with the reference
 restated (Keras 'same' padding incl. the asymmetric stride-2 case, eps = 1e-3 norms) -- kept as an
 independent GPU cross-check of the native path, never selected implicitly.
 Parameter names are the reference's Keras attribute paths, kernels HWIO, NHWC tensors at the interface.
+`conventions='pytorch'` (keyword-only) computes what the original PyTorch RAFT's encoders compute on both backends:
+symmetric padding at stride 2 and eps = 1e-5 (include/raft_b200.h, raft_conventions).
 """
 import ctypes
 import os
@@ -48,16 +50,20 @@ class _Encoder:
     _stages = ()
     _variant = None
 
-    def __init__(self, output_dim=128, norm_type='batch', drop_rate=0.0, *, device='cuda', seed=None, backend=None):
+    def __init__(self, output_dim=128, norm_type='batch', drop_rate=0.0, *, device='cuda', seed=None, backend=None,
+                 conventions='tf-raft'):
         self.backend = backend or os.environ.get('RAFT_B200_ENCODER', 'native')
         if self.backend not in ('native', 'torch'):
             raise ValueError(f'unknown encoder backend {self.backend!r}')
+        if conventions not in _lib.CONVENTIONS:
+            raise ValueError(f'unknown conventions {conventions!r}; expected one of {", ".join(_lib.CONVENTIONS)}')
+        self.conventions = conventions
         self._prepared = None
         self.workspaces = _lib.WorkspaceCache()
         self.output_dim = output_dim
         self.norm_type = Normalization(norm_type)
         self.drop_rate = drop_rate
-        self.store = _Params(device, seed)
+        self.store = _Params(device, seed, conventions)
         s = self.store
         s.add_conv('conv1', 7, 7, 3, self._c0)
         s.add_norm('norm1', norm_type, self._c0)
@@ -119,8 +125,9 @@ class _Encoder:
             w.conv2 = self._conv_struct('conv2')
             blob = _lib.workspace(_lib.query_bytes('encoder_prepared_bytes', self._variant, self.output_dim),
                                   self.store.device)
-            _lib.call('encoder_prepare', blob.device, self._variant, _lib.NORM_TYPES[self.norm_type], self.output_dim,
-                      ctypes.cast(ctypes.pointer(w), ctypes.c_void_p), _lib.ptr(blob), blob.numel())
+            _lib.call('encoder_prepare_ex', blob.device, self._variant, _lib.NORM_TYPES[self.norm_type], self.output_dim,
+                      ctypes.cast(ctypes.pointer(w), ctypes.c_void_p), _lib.CONVENTIONS[self.conventions], _lib.ptr(blob),
+                      blob.numel())
             self._prepared = blob
         return self._prepared
 

@@ -6,6 +6,10 @@
 upsample) is ONE call into libraft_b200.so (raft_b200_forward_loop); the correlation pyramid is
 another (raft_b200_corr_pyramid_build); in inference on the native encoders, so are the encoders, run as concurrent
 stream branches (raft_b200_encode_pair).  Optionally the whole forward is replayed from a CUDA graph.
+
+`RAFT(conventions='pytorch')` computes what the original PyTorch RAFT computes, so that its published checkpoints
+(`load_pytorch_weights`) give their numbers: symmetric stride-2 padding and eps = 1e-5 in the encoders, and the
+F.grid_sample lookup (DESIGN.md section 11).
 """
 from collections import OrderedDict
 
@@ -23,7 +27,13 @@ class RAFT:
     _variant = _lib.VARIANT_BASIC
 
     def __init__(self, drop_rate=0, iters=12, iters_pred=24, *, precision=None, device='cuda', seed=None,
-                 use_graph=False, encoder_backend=None, **kwargs):
+                 use_graph=False, encoder_backend=None, conventions='tf-raft', **kwargs):
+        if conventions not in _lib.CONVENTIONS:
+            raise ValueError(f'unknown conventions {conventions!r}; expected one of {", ".join(_lib.CONVENTIONS)}')
+        if conventions == 'pytorch' and self._variant != _lib.VARIANT_BASIC:
+            raise ValueError("conventions='pytorch' is RAFT's only: the original RAFT-small's encoder is built from "
+                             'bottleneck blocks, this SmallRAFT from residual blocks')
+        self.conventions = conventions
         self.hidden_dim = 128
         self.context_dim = 128
         self.corr_levels = 4
@@ -52,9 +62,10 @@ class RAFT:
     def _build_layers(self, seed):
         s = 0 if seed is None else seed
         self.fnet = BasicEncoder(output_dim=256, norm_type='instance', drop_rate=self.drop_rate, device=self.device,
-                                 seed=s, backend=self._encoder_backend())
+                                 seed=s, backend=self._encoder_backend(), conventions=self.conventions)
         self.cnet = BasicEncoder(output_dim=self.hidden_dim + self.context_dim, norm_type='batch',
-                                 drop_rate=self.drop_rate, device=self.device, seed=s + 1, backend=self._encoder_backend())
+                                 drop_rate=self.drop_rate, device=self.device, seed=s + 1, backend=self._encoder_backend(),
+                                 conventions=self.conventions)
         self.update_block = BasicUpdateBlock(filters=self.hidden_dim, precision=self.precision, device=self.device,
                                              seed=s + 2)
 
@@ -121,6 +132,19 @@ class RAFT:
                                'v': {k: tensors[keys[k, 'v']] for k in shapes}}
         if self.optimizer is not None:
             self._build_trainer()
+
+    def load_pytorch_weights(self, path):
+        """Loads a checkpoint of the original PyTorch RAFT (`raft-things.pth`, ...; a path or a state dict) through
+        `load_pytorch_checkpoint`.  Only a model built with `conventions='pytorch'` computes what those weights were
+        trained for; any other raises ValueError."""
+        from .checkpoint import load_pytorch_checkpoint
+        if self.conventions != 'pytorch':
+            raise ValueError("PyTorch RAFT weights need RAFT(conventions='pytorch'); under 'tf-raft' the encoders pad "
+                             'and sample differently and every feature would be shifted')
+        self.load_params(load_pytorch_checkpoint(path, expect=self.state_dict()))
+
+    def _sampler(self):
+        return 'grid_sample' if self.conventions == 'pytorch' else 'tf-raft'
 
     def _build_trainer(self):
         """The training state of `train_step`, with the optimiser state `load_weights` left pending applied to it."""
@@ -204,10 +228,10 @@ class RAFT:
     def _loop(self, corr_block, net, inp, coords1, flow_ups, b, h, w):
         ub = self.update_block
         ws = ub.workspace(b, h, w)
-        _lib.call('forward_loop', net.device, self._variant, _lib.ptr(ub.prepared()),
+        _lib.call('forward_loop_ex', net.device, self._variant, _lib.ptr(ub.prepared()),
                   _lib.ptr_array(corr_block.corr_pyramid), self.corr_levels, self.corr_radius, _lib.ptr(net), _lib.ptr(inp),
                   _lib.ptr(coords1), _lib.ptr_array(flow_ups), len(flow_ups), b, h, w, _lib.ptr(ws), ws.numel(),
-                  self.precision)
+                  self.precision, _lib.SAMPLERS[corr_block.sampler])
 
     def __call__(self, inputs, training, *, last_only=False, flow_init=None):
         """inputs = [image1, image2], each (B, H, W, 3) float in 0..255 on the GPU.
@@ -292,7 +316,7 @@ class RAFT:
         h, w = H // 8, W // 8
         iters = self.iters if training else self.iters_pred                  # model.py:92
         corr_block = CorrBlock(fmap1, fmap2, num_levels=self.corr_levels, radius=self.corr_radius,
-                               precision=self.precision)                      # :77-79
+                               precision=self.precision, sampler=self._sampler())   # :77-79
         if flow_init is None:
             coords1 = coords_grid(bs, h, w, self.device)                      # :89
         else:
@@ -423,6 +447,7 @@ class RAFT:
         """train_precision: 'fp32' (IEEE-fp32 library convolutions) or 'f16x2' (the training step's stride-1
         convolutions with cin >= 64 forward and backward on the tensor cores, fp16 hi/lo three-pass; DESIGN.md section 9)."""
         from .train import TRAIN_PRECISIONS
+        self._check_trainable()
         if train_precision not in TRAIN_PRECISIONS:
             raise ValueError(f'unknown train_precision {train_precision!r}; expected one of {", ".join(TRAIN_PRECISIONS)}')
         self.train_precision = train_precision
@@ -431,8 +456,7 @@ class RAFT:
         self.optimizer = optimizer
         self.clip_norm = clip_norm
         self.loss = loss
-        self.epe = epe
-        self.flow_metrics = OrderedDict((k, [0.0, 0]) for k in ('loss', 'epe', 'u1', 'u3', 'u5'))
+        self._init_metrics(epe)
         if self._pending_slots is not None and optimizer is not None:
             self._build_trainer()
 
@@ -442,6 +466,15 @@ class RAFT:
         from .fit import fit
         return fit(self, x, epochs=epochs, callbacks=callbacks, steps_per_epoch=steps_per_epoch,
                    validation_data=validation_data, validation_steps=validation_steps, verbose=verbose)
+
+    def _init_metrics(self, epe):
+        self.epe = epe
+        self.flow_metrics = OrderedDict((k, [0.0, 0]) for k in ('loss', 'epe', 'u1', 'u3', 'u5'))
+
+    def _check_trainable(self):
+        if self.conventions != 'tf-raft':
+            raise NotImplementedError("training runs in the tf-raft conventions only; conventions='pytorch' is for "
+                                      'inference with the original RAFT checkpoints')
 
     def _metric_update(self, key, value):
         m = self.flow_metrics[key]
@@ -460,6 +493,7 @@ class RAFT:
         torch.distributed process group the gradients are all-reduced (one flat NCCL call) and the context encoder's
         BatchNorm statistics are taken over the global batch (tf_raft_b200/train.py)."""
         from .train import AdamW
+        self._check_trainable()
         if self.flow_metrics is None or getattr(self, 'optimizer', None) is None:
             raise RuntimeError('compile(optimizer=..., clip_norm=...) before train_step, as in train_chairs.py:92-98')
         if not isinstance(self.optimizer, AdamW):
@@ -484,7 +518,10 @@ class RAFT:
     def test_step(self, data):
         """model.py:146-159."""
         if self.flow_metrics is None:
-            self.compile()
+            if self.conventions == 'tf-raft':
+                self.compile()
+            else:                                      # evaluation needs the metrics only, not a training set-up
+                self._init_metrics(end_point_error)
         image1, image2, flow, valid = data
         preds = self([image1, image2], training=False, last_only=True)
         info = self.epe([flow, valid], preds[-1])
