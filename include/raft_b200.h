@@ -125,6 +125,18 @@ int raft_b200_corr_lookup_ex(const float* const pyr[], const float* coords, int 
  *              + ... in ascending level.  Two calls on the same inputs give the same bits (DESIGN.md section 9).  */
 int raft_b200_corr_lookup_backward(const float* const pyr[], const float* coords, const float* grad_out, int B, int h, int w,
                                    int levels, int radius, float* grad_coords, float* const grad_pyr[], void* stream);
+/* raft_b200_corr_lookup_backward with the sampler chosen (raft_sampler); RAFT_SAMPLER_TF is
+ * raft_b200_corr_lookup_backward.  RAFT_SAMPLER_GRID is the backward of the grid_sample lookup with respect to the
+ * pyramid only, as the original RAFT, which detaches the sampling position, computes it: grad_coords must be NULL
+ * (RAFT_ERR_BAD_ARG otherwise) and pyr is not read.  ATen's grid_sampler_2d_backward with the forward's per-axis
+ * set-up: every in-frame corner of a tap adds fl(fl(wy*wx) * grad_out) to its cell, a zero weight or a zero grad_out
+ * included (so a non-finite grad_out reaches the cells ATen's backward reaches); corners outside the level add nothing.
+ * grad_pyr is ACCUMULATED, in the same order as above: a touched cell ends as in + term_1 + term_2 + ... left to right,
+ * in ascending t, then corner 00, 01, 10, 11; cells no in-frame corner reaches are not written (a level with S = 1
+ * receives nothing).  No atomics; two calls on the same inputs give the same bits.                                 */
+int raft_b200_corr_lookup_backward_ex(const float* const pyr[], const float* coords, const float* grad_out, int B, int h,
+                                      int w, int levels, int radius, float* grad_coords, float* const grad_pyr[],
+                                      int sampler, void* stream);
 
 /* tf.linalg.global_norm over a flat gradient buffer (model.py:135): out[0] = sum g^2 (deterministic two-stage
  * reduction; `partials` holds one float per block, at most npartials blocks are used).                               */
@@ -135,6 +147,19 @@ int raft_b200_sumsq(const float* g, size_t n, float* partials, size_t npartials,
  * m = b1 m + (1-b1) g'; v = b2 v + (1-b2) g'^2; var -= lr_t * m / (sqrt(v) + eps), lr_t already bias-corrected.        */
 int raft_b200_adamw_step(float* param, const float* grad, float* m, float* v, size_t n, const float* sumsq, float clip_norm,
                          float lr_t, float beta1, float beta2, float epsilon, float weight_decay, void* stream);
+
+/* Optimiser rule of raft_b200_adamw_step_ex.
+ *   TFA    tf.clip_by_global_norm + tfa AdamW: raft_b200_adamw_step (lr = the bias-corrected lr_t; bias_correction1/2
+ *          are not read).
+ *   TORCH  the original PyTorch RAFT's: torch.nn.utils.clip_grad_norm_ then torch.optim.AdamW,
+ *          g' = g * min(1, clip / (sqrt(*sumsq) + 1e-6)) (clip_norm <= 0: no clipping); var *= 1 - lr*wd;
+ *          m = b1 m + (1-b1) g'; v = b2 v + (1-b2) g'^2; var -= (lr / bias_correction1) * m / (sqrt(v) /
+ *          sqrt(bias_correction2) + eps), with the scheduled lr and bias_correction1 = 1 - b1^t, bias_correction2 =
+ *          1 - b2^t of step t from the caller.                                                                     */
+typedef enum raft_adamw_rule { RAFT_ADAMW_TFA = 0, RAFT_ADAMW_TORCH = 1 } raft_adamw_rule;
+int raft_b200_adamw_step_ex(float* param, const float* grad, float* m, float* v, size_t n, const float* sumsq,
+                            float clip_norm, float lr, float beta1, float beta2, float epsilon, float weight_decay,
+                            float bias_correction1, float bias_correction2, int rule, void* stream);
 
 /* bilinear_sampler(image, coords): corr.py:28-69.  image (M, H, W, 1), coords (M, P, 2),
  * out (M, P).  Same floor/ceil semantics as above.                                             */

@@ -18,11 +18,20 @@ config saved beside them as config.yml.  The timestamp has seconds (the referenc
 started in the same minute do not share a directory.  `model.resume` names a checkpoint prefix written by a previous
 run; its weights, Adam moments and step count are restored, so the learning-rate schedule continues.
 
+`--pytorch-checkpoint PATH` fine-tunes a checkpoint of the original PyTorch RAFT (`raft-things.pth`, ...) with RAFT's
+own training step (DESIGN.md section 11, "Training"): `RAFT(conventions='pytorch')` loads the file, the optimiser is
+`TorchAdamW(weight_decay, OneCycleLR(learning_rate, epochs * steps_per_epoch + 100))` with the config's clip_norm,
+`--freeze-bn` freezes cnet's BatchNorm (RAFT's `freeze_bn()`, which its recipe uses after FlyingChairs), `--gamma G` sets
+the sequence loss's weight decay over the iterations (RAFT's later stages use 0.85), and the trained weights are
+written as a `.pth` the original code reads, `<logdir>/<timestamp>/checkpoints/model.pth`, at the end.  Refused with
+`--small` and `--self-supervised`.
+
 `--self-supervised` compiles with `UnsupervisedLoss()` (DESIGN.md section 9.1): the training batches' ground truth is not
 used by the loss (the epe metrics of the forward prediction are still logged); the config, datasets, validation (val_epe
 against ground truth) and callbacks are the same.
 """
 import argparse
+import functools
 import os
 import random
 import sys
@@ -62,7 +71,8 @@ def need(config, path):
     return node
 
 
-def train(name, config, logdir, small=False, workers=4, self_supervised=False, train_precision='fp32'):
+def train(name, config, logdir, small=False, workers=4, self_supervised=False, train_precision='fp32',
+          pytorch_checkpoint=None, freeze_bn=False, gamma=None):
     root = need(config, 'data.root')
     aug_params = need(config, 'augment')
     iters, iters_pred, resume = (need(config, 'model.' + k) for k in ('iters', 'iters_pred', 'resume'))
@@ -90,11 +100,22 @@ def train(name, config, logdir, small=False, workers=4, self_supervised=False, t
     print(f'Found {train_size} samples for training')
     print(f'Found {val_size} samples for validation')
 
-    scheduler = T.CyclicalLearningRate(initial_learning_rate=learning_rate, maximal_learning_rate=2 * learning_rate,
-                                       step_size=1000, scale_fn=T.first_cycle_scaler, scale_mode='cycle')
-    optimizer = T.AdamW(weight_decay=weight_decay, learning_rate=scheduler)
-    raft = (T.SmallRAFT if small else T.RAFT)(drop_rate=0, iters=iters, iters_pred=iters_pred)
+    steps_per_epoch = train_size // batch_size
+    if pytorch_checkpoint:
+        optimizer = T.TorchAdamW(weight_decay=weight_decay,
+                                 learning_rate=T.OneCycleLR(learning_rate, epochs * steps_per_epoch + 100))
+        raft = T.RAFT(drop_rate=0, iters=iters, iters_pred=iters_pred, conventions='pytorch')
+        raft.load_pytorch_weights(pytorch_checkpoint)
+        if freeze_bn:
+            raft.freeze_bn()
+    else:
+        scheduler = T.CyclicalLearningRate(initial_learning_rate=learning_rate, maximal_learning_rate=2 * learning_rate,
+                                           step_size=1000, scale_fn=T.first_cycle_scaler, scale_mode='cycle')
+        optimizer = T.AdamW(weight_decay=weight_decay, learning_rate=scheduler)
+        raft = (T.SmallRAFT if small else T.RAFT)(drop_rate=0, iters=iters, iters_pred=iters_pred)
     loss = T.UnsupervisedLoss() if self_supervised else T.sequence_loss
+    if gamma is not None:
+        loss = functools.partial(T.sequence_loss, gamma=gamma)
     raft.compile(optimizer=optimizer, clip_norm=clip_norm, loss=loss, epe=T.end_point_error,
                  train_precision=train_precision)
     if resume:
@@ -109,10 +130,16 @@ def train(name, config, logdir, small=False, workers=4, self_supervised=False, t
         T.ModelCheckpoint(filepath=os.path.join(logdir, 'checkpoints', 'model'), save_weights_only=True,
                           monitor='val_epe', mode='min', save_best_only=True),
     ]
-    return raft.fit(ds_train.batches(batch_size, workers=workers, repeat=True), epochs=epochs, callbacks=callbacks,
-                    steps_per_epoch=train_size // batch_size,
-                    validation_data=Batches(ds_val, 1, target_size=VAL_SIZE[name], workers=workers),
-                    validation_steps=val_size)
+    history = raft.fit(ds_train.batches(batch_size, workers=workers, repeat=True), epochs=epochs, callbacks=callbacks,
+                       steps_per_epoch=steps_per_epoch,
+                       validation_data=Batches(ds_val, 1, target_size=VAL_SIZE[name], workers=workers),
+                       validation_steps=val_size)
+    if pytorch_checkpoint:
+        path = os.path.join(logdir, 'checkpoints', 'model.pth')
+        os.makedirs(os.path.dirname(path), exist_ok=True)
+        raft.save_pytorch_weights(path)
+        print(f'wrote {path}', flush=True)
+    return history
 
 
 def main():
@@ -126,7 +153,20 @@ def main():
                         help="convolutions of the step: IEEE-fp32 library (fp32) or tensor-core hi/lo (f16x2)")
     parser.add_argument('--self-supervised', action='store_true',
                         help='train with UnsupervisedLoss (census + smoothness, both directions) instead of ground truth')
+    parser.add_argument('--pytorch-checkpoint', metavar='PATH', default=None,
+                        help="fine-tune a checkpoint of the original PyTorch RAFT with its own training step "
+                             "(conventions='pytorch') and write <logdir>/checkpoints/model.pth at the end")
+    parser.add_argument('--freeze-bn', action='store_true',
+                        help="with --pytorch-checkpoint: RAFT's freeze_bn(), cnet's BatchNorm in eval mode")
+    parser.add_argument('--gamma', type=float, default=None,
+                        help='weight decay of the sequence loss over the iterations (default 0.8)')
     args = parser.parse_args()
+    if args.pytorch_checkpoint and (args.small or args.self_supervised):
+        parser.error('--pytorch-checkpoint trains the basic RAFT with ground truth: not with --small or --self-supervised')
+    if args.freeze_bn and not args.pytorch_checkpoint:
+        parser.error("--freeze-bn is the original RAFT's and needs --pytorch-checkpoint")
+    if args.gamma is not None and args.self_supervised:
+        parser.error('--gamma weights the supervised sequence loss; UnsupervisedLoss takes its own')
 
     with open(args.config) as f:
         config = yaml.load(f, Loader=yaml.SafeLoader)
@@ -142,7 +182,8 @@ def main():
         np.random.seed(args.seed)
         random.seed(args.seed)
     train(args.dataset, config, logdir, small=args.small, workers=args.workers, self_supervised=args.self_supervised,
-          train_precision=args.train_precision)
+          train_precision=args.train_precision, pytorch_checkpoint=args.pytorch_checkpoint, freeze_bn=args.freeze_bn,
+          gamma=args.gamma)
 
 
 if __name__ == '__main__':

@@ -12,11 +12,11 @@ from .layers.update import BasicUpdateBlock, SmallUpdateBlock
 from .losses import EndPointError, UnsupervisedLoss, end_point_error, sequence_loss
 from .model import RAFT, SmallRAFT
 from .checkpoint import (load_pytorch_checkpoint, load_tf_checkpoint, param_to_tf_key, read_tf_checkpoint, tf_key_to_param,
-                         write_tf_checkpoint)
+                         to_pytorch_state_dict, write_tf_checkpoint)
 from .preprocess import CropOrPadder, InputPadder, pad_to_multiple, resize_with_crop_or_pad
 from .fit import Callback, History
-from .train import (AdamW, CyclicalLearningRate, ModelCheckpoint, TensorBoard, VisFlowCallback, first_cycle_scaler,
-                    inverse_scaler)
+from .train import (AdamW, CyclicalLearningRate, ModelCheckpoint, OneCycleLR, TensorBoard, TorchAdamW, VisFlowCallback,
+                    first_cycle_scaler, inverse_scaler)
 from .evaluation import FlowMetrics, evaluate, flow_metrics
 from . import datasets
 from .submission import create_kitti_submission, create_sintel_submission
@@ -25,7 +25,7 @@ __all__ = ['CorrBlock', 'bilinear_sampler', 'coords_grid', 'fb_occlusion', 'forw
            'BasicEncoder', 'SmallEncoder',
            'BasicUpdateBlock', 'SmallUpdateBlock', 'RAFT', 'SmallRAFT', 'sequence_loss', 'end_point_error', 'UnsupervisedLoss',
            'resize_with_crop_or_pad', 'CropOrPadder', 'InputPadder', 'pad_to_multiple',
-           'load_pytorch_checkpoint', 'load_tf_checkpoint',
+           'load_pytorch_checkpoint', 'load_tf_checkpoint', 'to_pytorch_state_dict', 'TorchAdamW', 'OneCycleLR',
            'read_tf_checkpoint', 'write_tf_checkpoint', 'param_to_tf_key', 'tf_key_to_param', 'FlowMetrics', 'evaluate', 'flow_metrics',
            'Callback', 'History', 'ModelCheckpoint', 'TensorBoard', 'create_sintel_submission',
            'create_kitti_submission']

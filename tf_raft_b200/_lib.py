@@ -59,6 +59,8 @@ NORM_TYPES = {None: 0, 'instance': 1, 'batch': 2}
 # raft_conventions / raft_sampler (include/raft_b200.h): tf-raft's arithmetic, or the original PyTorch RAFT's
 CONVENTIONS = {'tf-raft': 0, 'pytorch': 1}
 SAMPLERS = {'tf-raft': 0, 'grid_sample': 1}
+# raft_adamw_rule: tfa AdamW after tf.clip_by_global_norm, or torch.optim.AdamW after clip_grad_norm_
+ADAMW_RULES = {'tfa': 0, 'torch': 1}
 
 _vp, _i, _sz = ctypes.c_void_p, ctypes.c_int, ctypes.c_size_t
 _SIGNATURES = {
@@ -75,9 +77,12 @@ _SIGNATURES = {
     'raft_b200_corr_lookup': (_i, [ctypes.POINTER(_vp), _vp, _i, _i, _i, _i, _i, _vp, _i, _vp]),
     'raft_b200_corr_lookup_ex': (_i, [ctypes.POINTER(_vp), _vp, _i, _i, _i, _i, _i, _vp, _i, _i, _vp]),
     'raft_b200_corr_lookup_backward': (_i, [ctypes.POINTER(_vp), _vp, _vp, _i, _i, _i, _i, _i, _vp, ctypes.POINTER(_vp), _vp]),
+    'raft_b200_corr_lookup_backward_ex': (_i, [ctypes.POINTER(_vp), _vp, _vp, _i, _i, _i, _i, _i, _vp, ctypes.POINTER(_vp),
+                                              _i, _vp]),
     'raft_b200_sumsq': (_i, [_vp, _sz, _vp, _sz, _vp, _vp]),
     'raft_b200_adamw_step': (_i, [_vp, _vp, _vp, _vp, _sz, _vp, ctypes.c_float, ctypes.c_float, ctypes.c_float,
                                   ctypes.c_float, ctypes.c_float, ctypes.c_float, _vp]),
+    'raft_b200_adamw_step_ex': (_i, [_vp, _vp, _vp, _vp, _sz, _vp] + [ctypes.c_float] * 8 + [_i, _vp]),
     'raft_b200_bilinear_sampler': (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp]),
     'raft_b200_coords_grid': (_i, [_i, _i, _i, _vp, _vp]),
     'raft_b200_forward_interpolate': (_i, [_vp, _i, _i, _i, _vp, _vp]),

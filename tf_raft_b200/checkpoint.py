@@ -19,6 +19,7 @@ attribute tree.
 import os
 import re
 import struct
+from collections import OrderedDict
 
 import numpy as np
 
@@ -468,3 +469,39 @@ def load_pytorch_checkpoint(path_or_state_dict, expect=None):
     if problems:
         raise ValueError(f'{label}: does not match the model -- ' + '; '.join(problems))
     return params
+
+
+def to_pytorch_state_dict(params, num_batches_tracked=0):
+    """The inverse of `load_pytorch_checkpoint`: `{param name: array}` of a conventions='pytorch' RAFT -> an ordered
+    state dict the original PyTorch RAFT loads (float32 CPU tensors): `module.` prefix, HWIO kernels as OIHW weights,
+    gamma / beta / moving_mean / moving_variance as weight / bias / running_mean / running_var plus an int64
+    `num_batches_tracked`, each ResidualBlock's `norm3` written again as its `downsample.1` twin, the mask head back in
+    RAFT's channel order, and no entries for fnet's norms (nn.InstanceNorm2d(affine=False) has none)."""
+    import torch
+    inv_norm = {v: k for k, v in _PT_NORM.items()}
+    out = OrderedDict()
+    perm = mask_head_permutation()
+
+    def put(key, value):
+        out['module.' + key] = torch.from_numpy(np.ascontiguousarray(value, dtype=np.float32))
+
+    for name, v in params.items():
+        v = np.asarray(v.detach().cpu().numpy() if hasattr(v, 'detach') else v, dtype=np.float32)
+        stem, _, leaf = name.rpartition('.')
+        if leaf == 'kernel':
+            if name == 'update_block.mask.2.kernel' and v.shape[-1] == 576:
+                v = v[..., np.argsort(perm)]
+            put(stem + '.weight', v.transpose(3, 2, 0, 1))                              # HWIO -> OIHW
+        elif leaf == 'bias' and stem + '.kernel' in params:
+            put(name, v[np.argsort(perm)] if name == 'update_block.mask.2.bias' and v.shape == (576,) else v)
+        elif leaf in inv_norm:
+            if stem.startswith('fnet.'):
+                continue
+            twin = re.fullmatch(r'(.*\.layer\d\.\d)\.downsample\.1', stem)
+            for s in ((stem, f'{twin.group(1)}.norm3') if twin else (stem,)):
+                put(f'{s}.{inv_norm[leaf]}', v)
+                if leaf == 'moving_variance':
+                    out[f'module.{s}.num_batches_tracked'] = torch.tensor(int(num_batches_tracked), dtype=torch.int64)
+        else:
+            raise ValueError(f'{name}: not a parameter of the PyTorch RAFT layout')
+    return out

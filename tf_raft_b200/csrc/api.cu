@@ -418,27 +418,42 @@ int raft_b200_corr_lookup(const float* const pyr[], const float* coords, int B, 
   return raft_b200_corr_lookup_ex(pyr, coords, B, h, w, levels, radius, out, out_stride, RAFT_SAMPLER_TF, stream);
 }
 
-int raft_b200_corr_lookup_backward(const float* const pyr[], const float* coords, const float* grad_out, int B, int h, int w,
-                                   int levels, int radius, float* grad_coords, float* const grad_pyr[], void* stream) {
-  if (!pyr || !coords || !grad_out || !grad_coords || !grad_pyr || levels < 1 || levels > RAFT_MAX_LEVELS || radius < 0)
-    return RAFT_ERR_BAD_ARG;
+int raft_b200_corr_lookup_backward_ex(const float* const pyr[], const float* coords, const float* grad_out, int B, int h,
+                                      int w, int levels, int radius, float* grad_coords, float* const grad_pyr[],
+                                      int sampler, void* stream) {
+  RAFT_TRY(check_sampler(sampler));
+  const bool grid = sampler == RAFT_SAMPLER_GRID;
+  // the grid_sample backward reads neither the pyramid nor a coordinate gradient: the original RAFT detaches coords
+  if (!coords || !grad_out || !grad_pyr || levels < 1 || levels > RAFT_MAX_LEVELS || radius < 0) return RAFT_ERR_BAD_ARG;
+  if (grid ? grad_coords != nullptr : (!pyr || !grad_coords)) return RAFT_ERR_BAD_ARG;
   RAFT_TRY(check_dims(B, h, w));
   LookupBwdParams p;
   memset(&p, 0, sizeof(p));
   int lh = h, lw = w;
   for (int l = 0; l < levels; ++l) {
     if (lh < 1 || lw < 1) return RAFT_ERR_BAD_SHAPE;
-    if (!pyr[l] || !grad_pyr[l]) return RAFT_ERR_BAD_ARG;
-    p.pyr[l] = pyr[l]; p.gpyr[l] = grad_pyr[l]; p.lh[l] = lh; p.lw[l] = lw;
+    if ((!grid && !pyr[l]) || !grad_pyr[l]) return RAFT_ERR_BAD_ARG;
+    p.pyr[l] = grid ? nullptr : pyr[l]; p.gpyr[l] = grad_pyr[l]; p.lh[l] = lh; p.lw[l] = lw;
     lh /= 2;
     lw /= 2;
   }
   const int side = 2 * radius + 1;
   p.coords = coords; p.gout = grad_out; p.gout_stride = levels * side * side; p.gcoords = grad_coords;
   p.nq = B * h * w; p.levels = levels; p.radius = radius;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (grid) {                                             // one warp per (query, level), 8 warps per block
+    const size_t smem = 8 * 2 * (size_t)side * sizeof(GridAxis);
+    if (smem > 48 * 1024) return RAFT_ERR_UNSUPPORTED;
+    return launch(corr_lookup_grid_bwd_kernel, grid_for((size_t)p.nq * levels, 8, kNumSMs * 32), 256, smem, st, p);
+  }
   const int qpb = lookup_bwd_queries_per_block(levels);
-  return launch(corr_lookup_bwd_kernel, grid_for((size_t)p.nq, qpb, kNumSMs * 32), 32 * levels * qpb, 0,
-                reinterpret_cast<cudaStream_t>(stream), p);
+  return launch(corr_lookup_bwd_kernel, grid_for((size_t)p.nq, qpb, kNumSMs * 32), 32 * levels * qpb, 0, st, p);
+}
+
+int raft_b200_corr_lookup_backward(const float* const pyr[], const float* coords, const float* grad_out, int B, int h, int w,
+                                   int levels, int radius, float* grad_coords, float* const grad_pyr[], void* stream) {
+  return raft_b200_corr_lookup_backward_ex(pyr, coords, grad_out, B, h, w, levels, radius, grad_coords, grad_pyr,
+                                           RAFT_SAMPLER_TF, stream);
 }
 
 int raft_b200_sumsq(const float* g, size_t n, float* partials, size_t npartials, float* out, void* stream) {
@@ -450,11 +465,23 @@ int raft_b200_sumsq(const float* g, size_t n, float* partials, size_t npartials,
   return launch(sumsq_final_kernel, 1, 256, 0, st, partials, blocks, out);
 }
 
+int raft_b200_adamw_step_ex(float* param, const float* grad, float* m, float* v, size_t n, const float* sumsq,
+                            float clip_norm, float lr, float beta1, float beta2, float epsilon, float weight_decay,
+                            float bias_correction1, float bias_correction2, int rule, void* stream) {
+  if (!param || !grad || !m || !v || (clip_norm > 0.0f && !sumsq)) return RAFT_ERR_BAD_ARG;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (rule == RAFT_ADAMW_TFA)
+    return launch(adamw_kernel, grid_for(n), 256, 0, st, param, grad, m, v, n, sumsq, clip_norm, lr, beta1, beta2, epsilon,
+                  weight_decay);
+  if (rule != RAFT_ADAMW_TORCH) return RAFT_ERR_BAD_ARG;
+  return launch(adamw_torch_kernel, grid_for(n), 256, 0, st, param, grad, m, v, n, sumsq, clip_norm, lr, beta1, beta2,
+                epsilon, weight_decay, bias_correction1, bias_correction2);
+}
+
 int raft_b200_adamw_step(float* param, const float* grad, float* m, float* v, size_t n, const float* sumsq, float clip_norm,
                          float lr_t, float beta1, float beta2, float epsilon, float weight_decay, void* stream) {
-  if (!param || !grad || !m || !v || (clip_norm > 0.0f && !sumsq)) return RAFT_ERR_BAD_ARG;
-  return launch(adamw_kernel, grid_for(n), 256, 0, reinterpret_cast<cudaStream_t>(stream), param, grad, m, v, n, sumsq,
-                clip_norm, lr_t, beta1, beta2, epsilon, weight_decay);
+  return raft_b200_adamw_step_ex(param, grad, m, v, n, sumsq, clip_norm, lr_t, beta1, beta2, epsilon, weight_decay, 1.0f,
+                                 1.0f, RAFT_ADAMW_TFA, stream);
 }
 
 int raft_b200_bilinear_sampler(const float* image, const float* coords, int M, int H, int W, int P, float* out,

@@ -159,6 +159,82 @@ __global__ void __launch_bounds__(256) corr_lookup_bwd_kernel(const LookupBwdPar
 }
 
 // ------------------------------------------------------------------------------------------------
+// Backward of the grid_sample lookup (RAFT_SAMPLER_GRID, kernels.cuh) with respect to the pyramid only: the original
+// RAFT detaches the sampling position, so there is no coordinate gradient.  ATen's grid_sampler_2d_backward
+// (align_corners, zeros padding) with the same per-axis set-up as the forward (grid_axis): with go = d loss / d out[q,
+// l, a, b], every IN-FRAME corner of the tap adds fl(fl(wy * wx) * go) to its cell -- zero weights and zero go included,
+// so a non-finite go reaches every cell ATen's backward reaches -- and a corner outside the level adds nothing.
+//
+// Fixed order, no atomics, each operation one rounded fp32 operation (no FMA), as in corr_lookup_bwd_kernel: a touched
+// cell ends as v_in + term_1 + term_2 + ..., added left to right, its terms in ascending tap t = a*(2r+1) + b and, within
+// a tap, in corner order 00, 01, 10, 11 (a tap reaches a cell through one corner at most, since x1 = x0 + 1).  Cells
+// that no in-frame corner reaches are neither read nor written, so a level of height or width 1 receives nothing.
+//
+// Unlike the tf-raft sampler's, consecutive taps' unnormalised ix are not exactly 1 apart (the normalisation rounds),
+// so a column can be reached by taps other than s-1 and s.  One warp per (query, level) owns that query's private
+// slice of grad_pyr[l]: its lanes first compute the 2(2r+1) per-axis set-ups once (shared memory), then stride over
+// the cells of the in-frame corners' bounding box, each cell gathering from the taps whose corners hit it.
+// ------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) corr_lookup_grid_bwd_kernel(const LookupBwdParams p) {
+  extern __shared__ GridAxis grid_bwd_axes[];                    // per warp: [0, S) x set-up of tap column a, [S, 2S) y of b
+  const int lane = threadIdx.x & 31, wpb = blockDim.x >> 5;
+  const int side = 2 * p.radius + 1;
+  GridAxis* ax = grid_bwd_axes + (threadIdx.x >> 5) * 2 * side;
+  const size_t nwork = (size_t)p.nq * p.levels;
+  for (size_t wi = (size_t)blockIdx.x * wpb + (threadIdx.x >> 5); wi < nwork; wi += (size_t)gridDim.x * wpb) {
+    const size_t q = wi / p.levels;
+    const int l = (int)(wi % p.levels);
+    const int H = p.lh[l], W = p.lw[l];
+    float* gimg = p.gpyr[l] + q * H * W;
+    const float* go_row = p.gout + q * p.gout_stride + (size_t)l * side * side;
+    const float inv = 1.0f / (float)(1 << l);                    // exact power of two
+    const float cx = __fmul_rn(__ldg(p.coords + 2 * q), inv), cy = __fmul_rn(__ldg(p.coords + 2 * q + 1), inv);
+    int lox = INT_MAX, hix = -1, loy = INT_MAX, hiy = -1;        // bounding box of the in-frame corners
+    __syncwarp();                                                // the previous item's readers are done with ax
+    for (int i = lane; i < 2 * side; i += 32) {
+      const bool isy = i >= side;
+      const int k = isy ? i - side : i;
+      const GridAxis g = grid_axis(__fadd_rn(isy ? cy : cx, (float)(k - p.radius)), isy ? H : W);
+      ax[i] = g;
+      const int lo = g.i0 >= 0 ? g.i0 : (g.i1 >= 0 ? g.i1 : INT_MAX);
+      const int hi = g.i1 >= 0 ? g.i1 : g.i0;
+      if (isy) { loy = min(loy, lo); hiy = max(hiy, hi); }
+      else { lox = min(lox, lo); hix = max(hix, hi); }
+    }
+    lox = __reduce_min_sync(0xffffffffu, lox);
+    loy = __reduce_min_sync(0xffffffffu, loy);
+    hix = __reduce_max_sync(0xffffffffu, hix);
+    hiy = __reduce_max_sync(0xffffffffu, hiy);
+    __syncwarp();
+    if (lox > hix || loy > hiy) continue;                        // no in-frame corner (warp-uniform)
+    const int nx = hix - lox + 1;
+    const size_t ncell = (size_t)nx * (hiy - loy + 1);
+    for (size_t k = lane; k < ncell; k += 32) {
+      const int y = loy + (int)(k / nx), x = lox + (int)(k % nx);
+      const size_t off = (size_t)y * W + x;
+      float v = 0.0f;
+      bool touched = false;
+      for (int a = 0; a < side; ++a) {
+        const GridAxis X = ax[a];
+        if (X.i0 != x && X.i1 != x) continue;
+        const float wx = X.i0 == x ? X.wf : X.wc;
+        for (int b = 0; b < side; ++b) {
+          const GridAxis Y = ax[side + b];
+          if (Y.i0 != y && Y.i1 != y) continue;
+          const float wy = Y.i0 == y ? Y.wf : Y.wc;
+          if (!touched) {
+            v = gimg[off];
+            touched = true;
+          }
+          v = __fadd_rn(v, __fmul_rn(__fmul_rn(wy, wx), __ldg(go_row + a * side + b)));
+        }
+      }
+      if (touched) gimg[off] = v;
+    }
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
 // tf.linalg.global_norm / tf.clip_by_global_norm (model.py:135) and tfa AdamW (train_chairs.py:87-90) on a flat buffer.
 // sumsq: deterministic two-stage reduction (fixed grid, fixed tree) -> out[0] = sum g^2.
 // ------------------------------------------------------------------------------------------------
@@ -211,6 +287,26 @@ __global__ void adamw_kernel(float* __restrict__ p, const float* __restrict__ g,
     m[i] = mi;
     v[i] = vi;
     p[i] = w - lr_t * mi / (sqrtf(vi) + eps);
+  }
+}
+
+// The original RAFT's optimiser step (RAFT_ADAMW_TORCH): torch.nn.utils.clip_grad_norm_ then torch.optim.AdamW,
+//   g <- g * min(1, clip / (||g|| + 1e-6))   (clip_norm > 0)
+//   var *= 1 - lr * wd;  m = b1 m + (1-b1) g;  v = b2 v + (1-b2) g^2;  var -= (lr / bc1) * m / (sqrt(v) / sqrt(bc2) + eps)
+// with the scheduled lr and the bias corrections bc1 = 1 - b1^t, bc2 = 1 - b2^t from the caller.
+__global__ void adamw_torch_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
+                                   float* __restrict__ v, size_t n, const float* __restrict__ sumsq, float clip_norm,
+                                   float lr, float b1, float b2, float eps, float wd, float bc1, float bc2) {
+  float scale = 1.0f;
+  if (clip_norm > 0.0f) scale = fminf(1.0f, clip_norm / (sqrtf(*sumsq) + 1e-6f));
+  const float decay = 1.0f - lr * wd, step = lr / bc1, bc2_sqrt = sqrtf(bc2);
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const float gi = g[i] * scale;
+    const float mi = b1 * m[i] + (1.0f - b1) * gi;
+    const float vi = b2 * v[i] + (1.0f - b2) * gi * gi;
+    m[i] = mi;
+    v[i] = vi;
+    p[i] = p[i] * decay - step * (mi / (sqrtf(vi) / bc2_sqrt + eps));
   }
 }
 

@@ -54,6 +54,8 @@ class RAFT:
         self._trainer = None
         self._params_stale = False
         self._pending_slots = None                         # optimiser state of load_weights awaiting the Trainer
+        self._frozen_bn = False                            # freeze_bn() (conventions='pytorch')
+        self._num_batches_tracked = 0                      # training-mode BatchNorm steps, for save_pytorch_weights
 
     def _encoder_backend(self):
         # the all-FFMA reference configuration keeps cuDNN IEEE-fp32 encoders; the product path is native
@@ -88,7 +90,11 @@ class RAFT:
         count under `optimizer/iter` (int64), so that `load_weights` resumes the run.
 
         Not written: TensorFlow's `_CHECKPOINTABLE_OBJECT_GRAPH` proto.  `load_weights` and `load_tf_checkpoint` here
-        read these files; TensorFlow's own `load_weights` needs that proto and cannot."""
+        read these files; TensorFlow's own `load_weights` needs that proto and cannot.
+
+        Under conventions='pytorch' this is the resume format too: it stores this project's layout (HWIO kernels, the
+        permuted mask head, fnet's fixed norm gamma / beta, no moments for those), not a `.pth`; `save_pytorch_weights`
+        writes the file the original RAFT reads."""
         from .checkpoint import OPTIMIZER_ITER_KEY, optimizer_slot_key, param_to_tf_key, write_tf_checkpoint
         tensors = {param_to_tf_key(k): v.detach().cpu().numpy() for k, v in self.state_dict().items()}
         slots = self._pending_slots
@@ -114,8 +120,8 @@ class RAFT:
         from .checkpoint import OPTIMIZER_ITER_KEY, load_tf_checkpoint, optimizer_slot_key, read_tf_checkpoint
         self.load_params(load_tf_checkpoint(filepath, expect=self.state_dict()))
         tensors = read_tf_checkpoint(filepath)
-        shapes = {k: tuple(v.shape) for k, v in self.state_dict().items()
-                  if not (k.endswith('.moving_mean') or k.endswith('.moving_variance'))}
+        from .train import is_trainable
+        shapes = {k: tuple(v.shape) for k, v in self.state_dict().items() if is_trainable(k, self.conventions)}
         keys = {(k, name): optimizer_slot_key(k, name) for k in shapes for name in ('m', 'v')}
         found = [key for key in keys.values() if key in tensors]
         if not found and OPTIMIZER_ITER_KEY not in tensors:
@@ -142,15 +148,41 @@ class RAFT:
             raise ValueError("PyTorch RAFT weights need RAFT(conventions='pytorch'); under 'tf-raft' the encoders pad "
                              'and sample differently and every feature would be shifted')
         self.load_params(load_pytorch_checkpoint(path, expect=self.state_dict()))
+        self._num_batches_tracked = 0
+
+    def save_pytorch_weights(self, path):
+        """Writes the parameters (trained ones included) with `torch.save` as a state dict the original PyTorch RAFT
+        loads, the inverse of `load_pytorch_weights`: `module.`-prefixed keys, OIHW weights, BatchNorm weight / bias /
+        running_mean / running_var and `num_batches_tracked` (int64: the training-mode steps this model has taken
+        since it was built or loaded; it does not enter RAFT's arithmetic), each `norm3` written again as its
+        `downsample.1` twin, the mask head in RAFT's channel order, and no fnet norm entries.  Only under
+        conventions='pytorch'; any other raises ValueError."""
+        import torch as _torch
+        from .checkpoint import to_pytorch_state_dict
+        if self.conventions != 'pytorch':
+            raise ValueError("save_pytorch_weights needs RAFT(conventions='pytorch'): a 'tf-raft' model's weights are "
+                             "trained for tf-raft's padding and sampler, which the original RAFT does not compute")
+        params = {k: v.detach().cpu().numpy() for k, v in self.state_dict().items()}
+        _torch.save(to_pytorch_state_dict(params, self._num_batches_tracked), path)
+
+    def freeze_bn(self):
+        """The original RAFT's `freeze_bn()`, which its recipe calls for every stage after FlyingChairs: from now on
+        the training step runs cnet's BatchNorm in eval mode -- it normalises with the running statistics and leaves
+        them unchanged -- while gamma / beta still train.  Only under conventions='pytorch'; any other raises
+        ValueError."""
+        if self.conventions != 'pytorch':
+            raise ValueError("freeze_bn is the original RAFT's and exists under conventions='pytorch' only")
+        self._frozen_bn = True
+        if self._trainer is not None:
+            self._trainer.graph.frozen_bn = True
 
     def _sampler(self):
         return 'grid_sample' if self.conventions == 'pytorch' else 'tf-raft'
 
     def _build_trainer(self):
         """The training state of `train_step`, with the optimiser state `load_weights` left pending applied to it."""
-        from .train import AdamW, Trainer
-        if not isinstance(self.optimizer, AdamW):
-            raise TypeError('optimizer must be tf_raft_b200.train.AdamW (tfa.optimizers.AdamW semantics)')
+        from .train import Trainer
+        self._check_optimizer()
         self._trainer = Trainer(self)
         slots, self._pending_slots = self._pending_slots, None
         if slots is not None:
@@ -447,7 +479,7 @@ class RAFT:
         """train_precision: 'fp32' (IEEE-fp32 library convolutions) or 'f16x2' (the training step's stride-1
         convolutions with cin >= 64 forward and backward on the tensor cores, fp16 hi/lo three-pass; DESIGN.md section 9)."""
         from .train import TRAIN_PRECISIONS
-        self._check_trainable()
+        self._check_trainable(optimizer, loss)
         if train_precision not in TRAIN_PRECISIONS:
             raise ValueError(f'unknown train_precision {train_precision!r}; expected one of {", ".join(TRAIN_PRECISIONS)}')
         self.train_precision = train_precision
@@ -471,10 +503,26 @@ class RAFT:
         self.epe = epe
         self.flow_metrics = OrderedDict((k, [0.0, 0]) for k in ('loss', 'epe', 'u1', 'u3', 'u5'))
 
-    def _check_trainable(self):
-        if self.conventions != 'tf-raft':
-            raise NotImplementedError("training runs in the tf-raft conventions only; conventions='pytorch' is for "
-                                      'inference with the original RAFT checkpoints')
+    def _check_trainable(self, optimizer, loss=None):
+        """conventions='pytorch' trains the original RAFT's step only: TorchAdamW, the supervised loss."""
+        from .losses import UnsupervisedLoss
+        from .train import TorchAdamW
+        if self.conventions != 'pytorch':
+            return
+        if not isinstance(optimizer, TorchAdamW):
+            raise NotImplementedError("conventions='pytorch' trains with the original RAFT's optimiser: "
+                                      f'compile(optimizer=tf_raft_b200.TorchAdamW(...)), got {type(optimizer).__name__}')
+        if isinstance(loss, UnsupervisedLoss):
+            raise NotImplementedError("UnsupervisedLoss is not available under conventions='pytorch'; compile with "
+                                      'TorchAdamW and the supervised sequence_loss')
+
+    def _check_optimizer(self):
+        from .train import AdamW, TorchAdamW
+        if self.conventions == 'pytorch':
+            if not isinstance(self.optimizer, TorchAdamW):
+                raise TypeError("optimizer must be tf_raft_b200.TorchAdamW under conventions='pytorch'")
+        elif not isinstance(self.optimizer, AdamW):
+            raise TypeError('optimizer must be tf_raft_b200.train.AdamW (tfa.optimizers.AdamW semantics)')
 
     def _metric_update(self, key, value):
         m = self.flow_metrics[key]
@@ -492,12 +540,10 @@ class RAFT:
         ground truth is given and not updated otherwise (tf_raft_b200/train.py).  Under an initialised
         torch.distributed process group the gradients are all-reduced (one flat NCCL call) and the context encoder's
         BatchNorm statistics are taken over the global batch (tf_raft_b200/train.py)."""
-        from .train import AdamW
-        self._check_trainable()
+        self._check_trainable(self.optimizer, getattr(self, 'loss', None))
         if self.flow_metrics is None or getattr(self, 'optimizer', None) is None:
             raise RuntimeError('compile(optimizer=..., clip_norm=...) before train_step, as in train_chairs.py:92-98')
-        if not isinstance(self.optimizer, AdamW):
-            raise TypeError('optimizer must be tf_raft_b200.train.AdamW (tfa.optimizers.AdamW semantics)')
+        self._check_optimizer()
         if self._trainer is None:
             self._build_trainer()
         loss, info = self._trainer.step(data, self.optimizer, self.clip_norm, self.loss, self.epe)

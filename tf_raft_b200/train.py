@@ -8,6 +8,9 @@ What runs where (DESIGN.md "Training"):
   scatter of d/d pyramid): hand-written CUDA (raft_b200_corr_lookup / raft_b200_corr_lookup_backward);
 * global-norm clipping + AdamW on ONE flat fp32 parameter / gradient / moment buffer: hand-written CUDA
   (raft_b200_sumsq, raft_b200_adamw_step);
+* under RAFT(conventions='pytorch'), the original PyTorch RAFT's step instead (TrainGraph, TorchAdamW, OneCycleLR): the
+  grid_sample lookup and its pyramid-only backward (raft_b200_corr_lookup_backward_ex), clip_grad_norm_ + torch AdamW
+  (raft_b200_adamw_step_ex), symmetric padding, eps 1e-5, non-affine fnet norms, BatchNorm momentum 0.1 or frozen;
 * data parallelism: one flat all-reduce (NCCL over NVLink) of the 21 MB gradient buffer per step, issued before the
   clipping (global norm of the reduced gradient, as a single-device step on the global batch would compute), and the
   per-channel batch statistics of the context encoder's BatchNorm layers all-reduced in forward and backward (SyncBN:
@@ -251,6 +254,64 @@ class AdamW:
         return float(lr(self.iterations)) if callable(lr) else float(lr)
 
 
+class TorchAdamW:
+    """torch.optim.AdamW as the original PyTorch RAFT configures it (train.py: `AdamW(lr, weight_decay, eps=1e-8)`),
+    for `RAFT(conventions='pytorch')`: beta 0.9 / 0.999, no amsgrad, weight decay `var *= 1 - lr * weight_decay`
+    before the Adam step, preceded by `clip_grad_norm_` (g * min(1, clip / (|g| + 1e-6))).  `learning_rate` is a
+    float or a per-step schedule such as `OneCycleLR`; step k (0-based) uses learning_rate(k).  The update is one CUDA
+    kernel over the flat buffer (FlatState.apply, raft_b200_adamw_step_ex with RAFT_ADAMW_TORCH)."""
+
+    def __init__(self, weight_decay, learning_rate, beta_1=0.9, beta_2=0.999, epsilon=1e-8):
+        self.weight_decay = weight_decay
+        self.learning_rate = learning_rate
+        self.beta_1, self.beta_2, self.epsilon = beta_1, beta_2, epsilon
+        self.iterations = 0
+
+    def lr(self):
+        lr = self.learning_rate
+        return float(lr(self.iterations)) if callable(lr) else float(lr)
+
+
+class OneCycleLR:
+    """torch.optim.lr_scheduler.OneCycleLR(max_lr, total_steps, pct_start, anneal_strategy='linear',
+    cycle_momentum=False, div_factor, final_div_factor) as a function of the step: `schedule(k)` is the learning rate
+    torch's scheduler holds after k calls of `scheduler.step()`, computed with the same floating-point operations, so
+    the values are equal.  Linear from max_lr / div_factor up to max_lr over the first pct_start * total_steps steps,
+    then linear down to max_lr / div_factor / final_div_factor at step total_steps - 1.  A step past total_steps raises
+    ValueError, as torch's does.  RAFT's recipe: OneCycleLR(lr, num_steps + 100)."""
+
+    def __init__(self, max_lr, total_steps, pct_start=0.05, div_factor=25.0, final_div_factor=1e4):
+        if not isinstance(total_steps, int) or total_steps <= 0:
+            raise ValueError(f'Expected positive integer total_steps, but got {total_steps}')
+        if not isinstance(pct_start, float) or not 0 <= pct_start <= 1:
+            raise ValueError(f'Expected float between 0 and 1 pct_start, but got {pct_start}')
+        self.max_lr = max_lr
+        self.total_steps = total_steps
+        self.initial_lr = max_lr / div_factor
+        self.min_lr = self.initial_lr / final_div_factor
+        self._phases = ((float(pct_start * total_steps) - 1, self.initial_lr, max_lr),
+                        (total_steps - 1, max_lr, self.min_lr))
+
+    def __call__(self, step):
+        if step > self.total_steps:
+            raise ValueError(f'Tried to step {step} times. The specified number of total steps is {self.total_steps}')
+        start_step = 0.0
+        for i, (end_step, start_lr, end_lr) in enumerate(self._phases):
+            if step <= end_step or i == len(self._phases) - 1:
+                pct = (step - start_step) / (end_step - start_step)
+                return (end_lr - start_lr) * pct + start_lr
+            start_step = end_step
+
+
+def is_trainable(name, conventions):
+    """Whether parameter `name` of a model's state_dict() is trained: not the BatchNorm moving statistics, and under
+    conventions='pytorch' not fnet's norm gamma / beta (the original's nn.InstanceNorm2d(affine=False): fixed 1 / 0,
+    no gradient, no weight decay)."""
+    if name.endswith('.moving_mean') or name.endswith('.moving_variance'):
+        return False
+    return not (conventions == 'pytorch' and name.startswith('fnet.') and name.endswith(('.gamma', '.beta')))
+
+
 # ------------------------------------------------------------------------------------------------ flat parameter state
 class FlatState:
     """All trainable variables of a model as views into ONE fp32 buffer (plus gradient and Adam moments of the same
@@ -298,6 +359,12 @@ class FlatState:
         opt.iterations += 1
         t = opt.iterations
         lr = opt.lr() if not callable(opt.learning_rate) else float(opt.learning_rate(t - 1))
+        if isinstance(opt, TorchAdamW):                # clip_grad_norm_ + torch.optim.AdamW, same single launch
+            _lib.call('adamw_step_ex', self.g.device, _lib.ptr(self.p), _lib.ptr(self.g), _lib.ptr(self.m),
+                      _lib.ptr(self.v), self.p.numel(), _lib.ptr(sumsq), float(clip_norm if clip_norm else 0.0), lr,
+                      float(opt.beta_1), float(opt.beta_2), float(opt.epsilon), float(opt.weight_decay),
+                      1 - opt.beta_1 ** t, 1 - opt.beta_2 ** t, _lib.ADAMW_RULES['torch'])
+            return
         lr_t = lr * math.sqrt(1 - opt.beta_2 ** t) / (1 - opt.beta_1 ** t)
         _lib.call('adamw_step', self.g.device, _lib.ptr(self.p), _lib.ptr(self.g), _lib.ptr(self.m), _lib.ptr(self.v),
                   self.p.numel(), _lib.ptr(sumsq), float(clip_norm if clip_norm else 0.0), float(lr_t), float(opt.beta_1),
@@ -332,6 +399,40 @@ class _Lookup(torch.autograd.Function):
         _lib.call('corr_lookup_backward', coords.device, _lib.ptr_array(pyramid), _lib.ptr(coords), _lib.ptr(grad_out),
                   b, h, w, levels, ctx.radius, _lib.ptr(g_coords), _lib.ptr_array(g_pyr))
         return (g_coords, None) + tuple(g_pyr)
+
+
+class _GridLookup(torch.autograd.Function):
+    """The original RAFT's CorrBlock.__call__ (conventions='pytorch'): forward = the grid_sample lookup
+    (raft_b200_corr_lookup_ex, RAFT_SAMPLER_GRID); backward = d/d pyramid only (raft_b200_corr_lookup_backward_ex).
+    RAFT detaches the coordinates before the lookup, so coordinates that require grad raise instead of silently
+    receiving none."""
+
+    @staticmethod
+    def forward(ctx, coords, radius, *pyramid):
+        if ctx.needs_input_grad[0]:
+            raise ValueError('the grid_sample lookup has no coordinate gradient: detach the coordinates first, as the '
+                             'original RAFT does at the top of every iteration')
+        coords = coords.contiguous()
+        b, h, w, _ = coords.shape
+        levels = len(pyramid)
+        nch = levels * (2 * radius + 1) ** 2
+        out = torch.empty((b, h, w, nch), dtype=torch.float32, device=coords.device)
+        _lib.call('corr_lookup_ex', coords.device, _lib.ptr_array(pyramid), _lib.ptr(coords), b, h, w, levels, radius,
+                  _lib.ptr(out), nch, _lib.SAMPLERS['grid_sample'])
+        ctx.save_for_backward(coords, *pyramid)
+        ctx.radius = radius
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        coords, *pyramid = ctx.saved_tensors
+        b, h, w, _ = coords.shape
+        grad_out = grad_out.contiguous()
+        g_pyr = [torch.zeros_like(p) for p in pyramid]
+        _lib.call('corr_lookup_backward_ex', coords.device, _lib.ptr_array(pyramid), _lib.ptr(coords),
+                  _lib.ptr(grad_out), b, h, w, len(pyramid), ctx.radius, None, _lib.ptr_array(g_pyr),
+                  _lib.SAMPLERS['grid_sample'])
+        return (None, None) + tuple(g_pyr)
 
 
 class _Upsample8(torch.autograd.Function):
@@ -480,11 +581,20 @@ def _all_reduce_sum(x):
 
 class TrainGraph:
     """The forward of model.py:68-109 / 190-226 with `training=True` in backward-capable form, on leaf parameters `P`
-    (HWIO kernels, reference attribute paths).  NCHW inside, NHWC at the interface."""
+    (HWIO kernels, reference attribute paths).  NCHW inside, NHWC at the interface.
 
-    def __init__(self, P, variant, precision, moving, train_precision='fp32'):
+    conventions='pytorch' is the original PyTorch RAFT's training forward (DESIGN.md section 11): symmetric (k-1)//2
+    padding, eps 1e-5, fnet's instance norms without affine (P holds no fnet gamma / beta), BatchNorm running
+    statistics with momentum 0.1, the grid_sample lookup, and coords1 detached at the top of every iteration.
+    frozen_bn (RAFT's `freeze_bn()`, conventions='pytorch' only): cnet's BatchNorm normalises with the running
+    statistics and leaves them unchanged; gamma / beta still train."""
+
+    def __init__(self, P, variant, precision, moving, train_precision='fp32', conventions='tf-raft', frozen_bn=False):
         self.P, self.variant, self.precision, self.moving = P, variant, precision, moving
         self.train_precision = train_precision
+        self.conventions = conventions
+        self.frozen_bn = frozen_bn
+        self.sampler = 'grid_sample' if conventions == 'pytorch' else 'tf-raft'
         self._conv_ws = {}                              # _ConvTC workspaces by shape
         self.cfg = dict(raft=dict(hidden=128, context=128, levels=4, radius=4, fnorm='instance', cnorm='batch'),
                         small=dict(hidden=96, context=64, levels=4, radius=3, fnorm='instance', cnorm=None))[variant]
@@ -497,6 +607,9 @@ class TrainGraph:
 
     def _conv_lib(self, x, name, stride, padding):
         w = self.P[name + '.kernel'].permute(3, 2, 0, 1)
+        if padding == 'same' and self.conventions == 'pytorch':         # nn.Conv2d(padding=(k-1)//2)
+            return F.conv2d(x, w, self.P[name + '.bias'], stride=stride,
+                            padding=((w.shape[2] - 1) // 2, (w.shape[3] - 1) // 2))
         if padding == 'same':
             pt, pb = _same_pads(x.shape[2], w.shape[2], stride)
             pl, pr = _same_pads(x.shape[3], w.shape[3], stride)
@@ -517,14 +630,18 @@ class TrainGraph:
         return self._conv_lib(x, name, stride, padding).contiguous(memory_format=torch.channels_last)
 
     def norm(self, x, name, norm_type):
-        eps = 1e-3
+        pytorch = self.conventions == 'pytorch'
+        eps = 1e-5 if pytorch else 1e-3
         if norm_type is None:
             return x
-        g = self.P[name + '.gamma'].view(1, -1, 1, 1)
-        b = self.P[name + '.beta'].view(1, -1, 1, 1)
         if norm_type == 'instance':
             mean = x.mean(dim=(2, 3), keepdim=True)
             var = x.var(dim=(2, 3), unbiased=False, keepdim=True)
+            if pytorch:                                 # nn.InstanceNorm2d(affine=False)
+                return (x - mean) * torch.rsqrt(var + eps)
+        elif pytorch and self.frozen_bn:                # BatchNorm in eval mode: running statistics, no update
+            mean = self.moving[name + '.moving_mean'].view(1, -1, 1, 1)
+            var = self.moving[name + '.moving_variance'].view(1, -1, 1, 1)
         else:                                           # batch statistics over the GLOBAL batch (all ranks)
             n_local = x.shape[0] * x.shape[2] * x.shape[3]
             stats = torch.stack([x.sum(dim=(0, 2, 3)), (x * x).sum(dim=(0, 2, 3))])
@@ -532,10 +649,12 @@ class TrainGraph:
             n = n_local * (dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1)
             mean = (stats[0] / n).view(1, -1, 1, 1)
             var = (stats[1] / n).view(1, -1, 1, 1) - mean * mean
-            with torch.no_grad():                       # keras moving statistics, momentum 0.99 (DESIGN.md §9)
-                mom = 0.99
+            with torch.no_grad():                       # keras momentum 0.99 (DESIGN.md §9); torch's 0.1 = keras 0.9
+                mom = 0.9 if pytorch else 0.99
                 self.moving[name + '.moving_mean'].mul_(mom).add_((1 - mom) * mean.flatten())
                 self.moving[name + '.moving_variance'].mul_(mom).add_((1 - mom) * n / max(n - 1, 1) * var.flatten())
+        g = self.P[name + '.gamma'].view(1, -1, 1, 1)
+        b = self.P[name + '.beta'].view(1, -1, 1, 1)
         return (x - mean) * torch.rsqrt(var + eps) * g + b
 
     def res_block(self, x, p, nt, stride):
@@ -635,7 +754,10 @@ class TrainGraph:
         coords1 = coords0.clone()
         preds = []
         for _ in range(iters):
-            corr = _Lookup.apply(coords1, cfg['radius'], *pyramid)
+            if self.conventions == 'pytorch':
+                coords1 = coords1.detach()              # RAFT: no gradient through the sampling position or the flow input
+            lookup = _GridLookup if self.sampler == 'grid_sample' else _Lookup
+            corr = lookup.apply(coords1, cfg['radius'], *pyramid)
             flow = coords1 - coords0
             net, mask, delta = self.update_block(net, inp, corr.permute(0, 3, 1, 2), flow.permute(0, 3, 1, 2))
             coords1 = coords1 + delta.permute(0, 2, 3, 1)
@@ -656,14 +778,18 @@ class Trainer:
         self.model = model
         self.variant = 'raft' if model._variant == _lib.VARIANT_BASIC else 'small'
         sd = model.state_dict()
-        self.flat = FlatState(sd, lambda k: not (k.endswith('.moving_mean') or k.endswith('.moving_variance')))
+        self.conventions = model.conventions
+        self.flat = FlatState(sd, lambda k: is_trainable(k, model.conventions))
         self.moving = {k: v.clone() for k, v in sd.items() if k.endswith('.moving_mean') or k.endswith('.moving_variance')}
-        self.graph = TrainGraph(self.flat.views, self.variant, model.precision, self.moving, model.train_precision)
+        self.fixed = {k: v.clone() for k, v in sd.items() if k not in self.moving and k not in self.flat.views}
+        self.graph = TrainGraph(self.flat.views, self.variant, model.precision, self.moving, model.train_precision,
+                                model.conventions, model._frozen_bn)
         self.world = dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
 
     def params(self):
         out = {k: v.detach() for k, v in self.flat.views.items()}
         out.update(self.moving)
+        out.update(self.fixed)
         return out
 
     def step(self, data, optimizer, clip_norm, loss_fn=sequence_loss, epe_fn=end_point_error):
@@ -691,6 +817,8 @@ class Trainer:
             dist.all_reduce(self.flat.g, op=dist.ReduceOp.SUM)                 # ONE flat NCCL all-reduce per step
             self.flat.g.div_(self.world)
         self.flat.apply(optimizer, clip_norm)                                  # :135-136
+        if self.conventions == 'pytorch' and not self.graph.frozen_bn:
+            self.model._num_batches_tracked += 1                                # BatchNorm's training-mode step count
         with torch.no_grad():
             info = epe_fn([flow_gt, valid], preds[-1].detach())                # :138
         return loss.detach(), info
