@@ -118,9 +118,10 @@ def encoder(ops, x, prefix, norm_type, training):
 
 # ----------------------------------------------------------------------------- corr.py
 
-def coords_grid(batch_size, height, width, dtype=torch.float32):
+def coords_grid(batch_size, height, width, dtype=torch.float32, device=None):
     """corr.py:72-90 -> (B, H, W, 2), (x, y)."""
-    gy, gx = torch.meshgrid(torch.arange(height, dtype=dtype), torch.arange(width, dtype=dtype), indexing='ij')
+    gy, gx = torch.meshgrid(torch.arange(height, dtype=dtype, device=device),
+                            torch.arange(width, dtype=dtype, device=device), indexing='ij')
     return torch.stack([gx, gy], dim=-1)[None].repeat(batch_size, 1, 1, 1)
 
 
@@ -166,7 +167,7 @@ class CorrBlock:
     def retrieve(self, coords):
         r = self.radius
         bs, h, w, _ = coords.shape
-        d = torch.arange(-r, r + 1, dtype=coords.dtype)
+        d = torch.arange(-r, r + 1, dtype=coords.dtype, device=coords.device)
         dy, dx = torch.meshgrid(d, d, indexing='ij')
         delta = torch.stack([dy, dx], dim=-1).reshape(1, 2 * r + 1, 2 * r + 1, 2)
         out = []
@@ -293,7 +294,7 @@ def forward(params, image1, image2, variant='raft', iters=12, training=False,
     cnet = encoder(ops, x1.permute(0, 3, 1, 2), 'cnet', cfg['cnorm'], training)  # :82
     net = torch.tanh(cnet[:, :cfg['hidden']])                               # :84-86
     inp = F.relu(cnet[:, cfg['hidden']:])
-    coords0 = coords_grid(bs, H // 8, W // 8, dtype)                        # :89, :32-37
+    coords0 = coords_grid(bs, H // 8, W // 8, dtype, x1.device)             # :89, :32-37
     coords1 = coords0.clone()
     inter = dict(fmap1=fmap1, fmap2=fmap2, net0=net.permute(0, 2, 3, 1), inp=inp.permute(0, 2, 3, 1),
                  corr=[], net=[], mask=[], delta=[], coords=[]) if return_intermediates else None

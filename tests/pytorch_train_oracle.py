@@ -74,12 +74,15 @@ def _encoder(sd, x, prefix, kind, bn):
     return rp._conv(sd, x, prefix + '.conv2')
 
 
-def train_forward(sd, image1, image2, iters, bn='train', dtype=torch.float64):
+def train_forward(sd, image1, image2, iters, bn='train', dtype=torch.float64, lookup=None):
     """RAFT.forward(iters) with model.train() (and freeze_bn() for bn='frozen') on a state dict `sd` in PyTorch layout
     without the `module.` prefix (tensors of `dtype`; leaves that require grad are differentiated).  The running
-    statistics in `sd` are updated in place under bn='train'.  Returns the `iters` upsampled flows, (B, H, W, 2)."""
-    im1 = torch.as_tensor(np.asarray(image1)).to(dtype).permute(0, 3, 1, 2)
-    im2 = torch.as_tensor(np.asarray(image2)).to(dtype).permute(0, 3, 1, 2)
+    statistics in `sd` are updated in place under bn='train'.  Returns the `iters` upsampled flows, (B, H, W, 2).
+    Runs on the device of `sd` (images: NumPy or tensors).  `lookup(k, pyramid, coords1)` replaces the k-th
+    iteration's CorrBlock.__call__ (teacher forcing, oracle/teacher_forced.py); None is RAFT's own."""
+    dev = sd['fnet.conv1.weight'].device
+    im1 = torch.as_tensor(image1).to(dev, dtype).permute(0, 3, 1, 2)
+    im2 = torch.as_tensor(image2).to(dev, dtype).permute(0, 3, 1, 2)
     im1 = 2 * (im1 / 255.0) - 1.0
     im2 = 2 * (im2 / 255.0) - 1.0
     b = im1.shape[0]
@@ -88,12 +91,12 @@ def train_forward(sd, image1, image2, iters, bn='train', dtype=torch.float64):
     cnet = _encoder(sd, im1, 'cnet', 'batch', bn)
     net, inp = torch.tanh(cnet[:, :128]), torch.relu(cnet[:, 128:])
     _, _, h, w = fmap.shape
-    coords0 = rp.coords_grid(b, h, w, dtype)
+    coords0 = rp.coords_grid(b, h, w, dtype).to(dev)
     coords1 = coords0.clone()
     preds = []
-    for _ in range(iters):
+    for k in range(iters):
         coords1 = coords1.detach()
-        corr = rp.corr_lookup(pyr, coords1)
+        corr = rp.corr_lookup(pyr, coords1) if lookup is None else lookup(k, pyr, coords1)
         net, mask, delta = rp.update_block(sd, net, inp, corr, coords1 - coords0)
         coords1 = coords1 + delta
         preds.append(rp.upsample_flow(coords1 - coords0, mask).permute(0, 2, 3, 1))
@@ -102,8 +105,8 @@ def train_forward(sd, image1, image2, iters, bn='train', dtype=torch.float64):
 
 def sequence_loss(preds, flow_gt, valid, gamma=0.8, max_flow=400):
     """RAFT's sequence_loss on (B, H, W, 2) predictions: valid >= 0.5 and |flow_gt| < max_flow, mean over B*H*W*2."""
-    fg = torch.as_tensor(np.asarray(flow_gt)).to(preds[0].dtype)
-    va = torch.as_tensor(np.asarray(valid)).to(preds[0].dtype)
+    fg = torch.as_tensor(flow_gt).to(preds[0])
+    va = torch.as_tensor(valid).to(preds[0])
     vm = ((va >= 0.5) & (torch.sqrt((fg ** 2).sum(-1)) < max_flow)).to(fg.dtype).unsqueeze(-1)
     n = len(preds)
     return sum(gamma ** (n - i - 1) * (vm * (p - fg).abs()).mean() for i, p in enumerate(preds))
