@@ -54,8 +54,17 @@ typedef enum raft_status {
  *          with fp32 accumulation (DESIGN.md "Precision").                                  */
 typedef enum raft_precision { RAFT_PREC_FP32 = 0, RAFT_PREC_F16X2 = 1 } raft_precision;
 
-/* model.py:10-30 (RAFT, BasicUpdateBlock) / model.py:173-188 (SmallRAFT, SmallUpdateBlock). */
-typedef enum raft_variant { RAFT_VARIANT_BASIC = 0, RAFT_VARIANT_SMALL = 1 } raft_variant;
+/* model.py:10-30 (RAFT, BasicUpdateBlock) / model.py:173-188 (SmallRAFT, SmallUpdateBlock).
+ * SMALL_PYTORCH is the original PyTorch RAFT-small: its encoders are built from bottleneck blocks
+ * (raft_b200_encoder_prepare_bottleneck) and its loop upsamples with raft_b200_upflow8_align_corners.  The encoder
+ * entry points (encoder_prepared_bytes / _workspace_bytes / _forward, encode_pair_workspace_bytes, encode_pair) and
+ * forward_loop / forward_loop_ex accept it; the loop treats it as RAFT_VARIANT_SMALL (same update-block blob, prepared
+ * as SMALL, same workspace, same lookup) except for the upsampling.  Every other entry point returns RAFT_ERR_BAD_ARG. */
+typedef enum raft_variant {
+  RAFT_VARIANT_BASIC = 0,
+  RAFT_VARIANT_SMALL = 1,
+  RAFT_VARIANT_SMALL_PYTORCH = 2
+} raft_variant;
 
 /* Lookup sampler (raft_b200_corr_lookup_ex, raft_b200_forward_loop_ex).
  *   TF    tf-raft's bilinear_sampler (corr.py:28-69): clamp to [0, S-1], floor / ceil corners.
@@ -488,6 +497,34 @@ int raft_b200_encoder_prepare_ex(int variant, int norm_type, int out_dim, const 
                                  int conventions, void* prepared, size_t prepared_bytes, void* stream);
 int raft_b200_encoder_workspace_bytes(int variant, int N, int H, int W, size_t* bytes);
 
+/* The original PyTorch RAFT's BottleneckBlock(in, planes, stride): y = relu(norm1(conv1 1x1, in -> planes/4));
+ * y = relu(norm2(conv2 3x3, padding 1, stride, planes/4 -> planes/4)); y = relu(norm3(conv3 1x1, planes/4 -> planes));
+ * x = norm4(downsample 1x1, stride, in -> planes) when stride != 1, else x = the block input; out = relu(x + y).
+ * downsample.kernel == NULL when stride == 1.                                                                     */
+typedef struct raft_bottleneck {
+  raft_conv conv1, conv2, conv3;
+  raft_norm norm1, norm2, norm3;
+  raft_conv downsample;
+  raft_norm downsample_norm;
+} raft_bottleneck;
+
+/* The original RAFT-small's SmallEncoder: conv1 7x7 s2 3 -> 32, norm1, layer1 = 2 x Bottleneck(32), layer2 =
+ * Bottleneck(32 -> 64, s2), Bottleneck(64), layer3 = Bottleneck(64 -> 96, s2), Bottleneck(96) (block[0..5] in that
+ * order; bottleneck widths 8, 16, 24), conv2 1x1 96 -> out_dim.                                                 */
+typedef struct raft_bottleneck_encoder_weights {
+  raft_conv conv1;
+  raft_norm norm1;
+  raft_bottleneck block[6];
+  raft_conv conv2;
+} raft_bottleneck_encoder_weights;
+
+/* Prepares a RAFT_VARIANT_SMALL_PYTORCH encoder blob (raft_b200_encoder_prepared_bytes(RAFT_VARIANT_SMALL_PYTORCH,
+ * out_dim)).  The blob always records RAFT_CONVENTIONS_PYTORCH (bound to its address as raft_b200_encoder_prepare_ex
+ * describes).  norm_type: RAFT_NORM_INSTANCE (gamma / beta of every norm given) or RAFT_NORM_NONE; RAFT_NORM_BATCH
+ * returns RAFT_ERR_BAD_ARG.                                                                                      */
+int raft_b200_encoder_prepare_bottleneck(int norm_type, int out_dim, const raft_bottleneck_encoder_weights* weights,
+                                         void* prepared, size_t prepared_bytes, void* stream);
+
 /* BasicEncoder.call / SmallEncoder.call (extractor.py:113-130 / 158-175) on N images.
  *   images : (N, H, W, 3); image_norm != 0: values are 0..255 and the 2*(x/255)-1 of model.py:70-71 is
  *            fused into the first load; image_norm == 0: already normalised (the encoder layer on its own)
@@ -565,6 +602,17 @@ int raft_b200_upsample_convex(const float* flow, const float* mask, int B, int h
 /* upflow8(flow): corr.py:93-96 = 8 * bilinear resize with half-pixel centres.                    */
 int raft_b200_upflow8(const float* flow, int B, int h, int w, float* out, void* stream);
 
+/* The original RAFT-small's upflow8: 8 * F.interpolate(flow, size=(8h, 8w), mode='bilinear', align_corners=True), as
+ * ATen's upsample_bilinear2d computes it.  flow (B,h,w,2) -> out (B,8h,8w,2).  Per axis of n input cells, in fp32,
+ * each operation one rounded operation, no FMA:
+ *   scale = fl((n-1) / (8n-1)) (0 when 8n = 1, never the case here);  src = fl(scale * X);  i0 = (int)src;
+ *   i1 = i0 + (i0 < n-1);  l1 = fl(src - i0);  l0 = fl(1 - l1);
+ * and per output pixel and channel, with a = f[y0][x0], b = f[y0][x1], c = f[y1][x0], d = f[y1][x1]:
+ *   val = fl(fl(ly0 * fl(fl(lx0 * a) + fl(lx1 * b))) + fl(ly1 * fl(fl(lx0 * c) + fl(lx1 * d))));  out = fl(8 * val)
+ * (the factor 8 is exact).  All four corners are read even at weight 0, so a NaN or inf reaches the outputs ATen's
+ * kernel gives it.                                                                                               */
+int raft_b200_upflow8_align_corners(const float* flow, int B, int h, int w, float* out, void* stream);
+
 /* Backward of F.interpolate(scale_factor=8, mode='bilinear', align_corners=False), the upsampling of SmallRAFT's
  * training graph (without upflow8's factor 8).  grad_up (B, 8h, 8w, 2) -> grad_flow (B, h, w, 2), WRITTEN (not
  * accumulated); both 8-byte aligned (RAFT_ERR_BAD_ARG otherwise).  PyTorch's upsample_bilinear2d weights: per output
@@ -587,7 +635,8 @@ int raft_b200_upflow8_backward(const float* grad_up, int B, int h, int w, float*
  *                  flow is coords1 - coords_grid
  *   flow_up      : iters pointers to (B,8h,8w,2) outputs; entries may be NULL to skip that
  *                  iteration's upsampling (predict_step keeps only the last, model.py:166);
- *                  for BASIC a skipped iteration also skips the mask head.                        */
+ *                  for BASIC a skipped iteration also skips the mask head.  Upsampling: BASIC convex,
+ *                  SMALL raft_b200_upflow8, SMALL_PYTORCH raft_b200_upflow8_align_corners.        */
 int raft_b200_forward_loop(int variant, const void* prepared, const float* const pyr[], int levels, int radius,
                            float* net, const float* inp, float* coords1, float* const flow_up[], int iters,
                            int B, int h, int w, void* workspace, size_t workspace_bytes, int precision,

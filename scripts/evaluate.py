@@ -19,6 +19,9 @@ A checkpoint of the original PyTorch RAFT (raft-things.pth, ...) is scored with 
 KITTI), 32 iterations on Sintel and 24 on KITTI, each unless --padding, --pad-mode or --iters says otherwise:
 
     python scripts/evaluate.py sintel --root datasets/MPI-Sintel-complete --pytorch-checkpoint models/raft-things.pth
+
+With `--small`, the file is the original RAFT-small (raft-small.pth), scored as SmallRAFT(conventions='pytorch',
+blocks='bottleneck') under the same protocol.
 """
 import argparse
 import json
@@ -52,8 +55,9 @@ def main():
     ap.add_argument('--root', required=True)
     src = ap.add_mutually_exclusive_group(required=True)
     src.add_argument('--checkpoint', help='TF checkpoint prefix (the path before .index)')
-    src.add_argument('--pytorch-checkpoint', help="the original PyTorch RAFT's .pth (basic model)")
-    ap.add_argument('--small', action='store_true', help='SmallRAFT instead of RAFT')
+    src.add_argument('--pytorch-checkpoint', help="the original PyTorch RAFT's .pth (raft-small.pth with --small)")
+    ap.add_argument('--small', action='store_true', help='SmallRAFT instead of RAFT (the original RAFT-small with '
+                                                         '--pytorch-checkpoint)')
     ap.add_argument('--dstype', default=None, help="Sintel 'clean' / 'final'; Things 'frames_cleanpass' / ...")
     ap.add_argument('--split-txt', default='FlyingChairs_train_val.txt')
     ap.add_argument('--iters', type=int, default=None, help='default 24; with --pytorch-checkpoint 32 on Sintel')
@@ -76,13 +80,14 @@ def main():
     if args.max_flow >= 0:
         max_flow = args.max_flow or None
     if args.pytorch_checkpoint:
-        if args.small:
-            ap.error('--pytorch-checkpoint loads the basic RAFT model only')
         args.padding = args.padding or 'replicate'                      # RAFT's InputPadder
         args.pad_mode = args.pad_mode or ('kitti' if args.dataset == 'kitti' else 'sintel')
         if args.iters is None:
             args.iters = 32 if args.dataset == 'sintel' else 24
-        model = T.RAFT(iters_pred=args.iters, conventions='pytorch')
+        if args.small:
+            model = T.SmallRAFT(iters_pred=args.iters, conventions='pytorch', blocks='bottleneck')
+        else:
+            model = T.RAFT(iters_pred=args.iters, conventions='pytorch')
         model.load_pytorch_weights(args.pytorch_checkpoint)
     else:
         args.iters = 24 if args.iters is None else args.iters

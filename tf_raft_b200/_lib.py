@@ -17,6 +17,7 @@ PREC_FP32 = 0
 PREC_F16X2 = 1
 VARIANT_BASIC = 0
 VARIANT_SMALL = 1
+VARIANT_SMALL_PYTORCH = 2          # the original PyTorch RAFT-small: bottleneck encoders, align-corners upflow8
 MAX_LEVELS = 8
 
 _PRECISIONS = {'fp32': PREC_FP32, 'f16x2': PREC_F16X2, PREC_FP32: PREC_FP32, PREC_F16X2: PREC_F16X2}
@@ -53,6 +54,17 @@ class RaftResBlock(ctypes.Structure):
 class RaftEncoderWeights(ctypes.Structure):
     """struct raft_encoder_weights"""
     _fields_ = [('conv1', RaftConv), ('norm1', RaftNorm), ('block', RaftResBlock * 6), ('conv2', RaftConv)]
+
+
+class RaftBottleneck(ctypes.Structure):
+    """struct raft_bottleneck"""
+    _fields_ = [('conv1', RaftConv), ('conv2', RaftConv), ('conv3', RaftConv), ('norm1', RaftNorm), ('norm2', RaftNorm),
+                ('norm3', RaftNorm), ('downsample', RaftConv), ('downsample_norm', RaftNorm)]
+
+
+class RaftBottleneckEncoderWeights(ctypes.Structure):
+    """struct raft_bottleneck_encoder_weights"""
+    _fields_ = [('conv1', RaftConv), ('norm1', RaftNorm), ('block', RaftBottleneck * 6), ('conv2', RaftConv)]
 
 
 NORM_TYPES = {None: 0, 'instance': 1, 'batch': 2}
@@ -109,9 +121,11 @@ _SIGNATURES = {
     'raft_b200_upsample_convex': (_i, [_vp, _vp, _i, _i, _i, _vp, _vp]),
     'raft_b200_upflow8': (_i, [_vp, _i, _i, _i, _vp, _vp]),
     'raft_b200_upflow8_backward': (_i, [_vp, _i, _i, _i, _vp, _vp]),
+    'raft_b200_upflow8_align_corners': (_i, [_vp, _i, _i, _i, _vp, _vp]),
     'raft_b200_encoder_prepared_bytes': (_i, [_i, _i, ctypes.POINTER(_sz)]),
     'raft_b200_encoder_prepare': (_i, [_i, _i, _i, _vp, _vp, _sz, _vp]),
     'raft_b200_encoder_prepare_ex': (_i, [_i, _i, _i, _vp, _i, _vp, _sz, _vp]),
+    'raft_b200_encoder_prepare_bottleneck': (_i, [_i, _i, _vp, _vp, _sz, _vp]),
     'raft_b200_encoder_workspace_bytes': (_i, [_i, _i, _i, _i, ctypes.POINTER(_sz)]),
     'raft_b200_encoder_forward': (_i, [_i, _i, _i, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _sz, _vp]),
     'raft_b200_context_split': (_i, [_vp, _i, _i, _i, _vp, _vp, _vp]),

@@ -383,17 +383,35 @@ def mask_head_permutation():
     return (c % 9) * 64 + c // 9
 
 
+def _pt_instance_norms(small):
+    """fnet's nn.InstanceNorm2d(affine=False) layers, (name, width), of the basic model or of RAFT-small."""
+    c0, stages = (32, ((32, 1), (64, 2), (96, 2))) if small else (64, ((64, 1), (96, 2), (128, 2)))
+    out = [('fnet.norm1', c0)]
+    for li, (c, stride) in enumerate(stages, start=1):
+        for bi in (0, 1):
+            p = f'fnet.layer{li}.{bi}'
+            out += [(f'{p}.norm1', c // 4), (f'{p}.norm2', c // 4), (f'{p}.norm3', c)] if small else \
+                [(f'{p}.norm1', c), (f'{p}.norm2', c)]
+            if bi == 0 and stride != 1:
+                out.append((f'{p}.downsample.1', c))
+    return out
+
+
 def load_pytorch_checkpoint(path_or_state_dict, expect=None):
-    """A checkpoint of the original PyTorch RAFT (basic model) -> `{param name: ndarray}` for `RAFT.load_params` of a
-    model built with `conventions='pytorch'`.
+    """A checkpoint of the original PyTorch RAFT -> `{param name: ndarray}` for `load_params` of a model built with
+    `conventions='pytorch'`: the basic model (`RAFT`), or RAFT-small (`raft-small.pth`, recognised by its bottleneck
+    blocks' `conv3` keys) for `SmallRAFT(conventions='pytorch', blocks='bottleneck')`.
 
     Read with `torch.load(map_location='cpu', weights_only=True)` (or given as a state dict).  The mapping: the
     `module.` prefix of nn.DataParallel is stripped; OIHW weights become HWIO kernels; BatchNorm's weight / bias /
     running_mean / running_var become gamma / beta / moving_mean / moving_variance and `num_batches_tracked` is dropped;
     each ResidualBlock's `norm3`, which PyTorch also stores as `downsample.1`, must equal that twin and is dropped;
     fnet's instance norms (affine=False, no parameters) get gamma = 1 and beta = 0; the mask head's output channels are
-    permuted (`mask_head_permutation`).  Missing, unexpected and mis-shaped keys are reported in ONE ValueError (with
-    `expect` = the model's `state_dict()`, against its names and shapes)."""
+    permuted (`mask_head_permutation`).  A RAFT-small file holds convolutions only (its norms are parameter-free instance
+    norms in fnet and none in cnet): fnet's norms get the identity affine, widths 32, 8 / 16 / 24 and 32 / 64 / 96, and
+    there is no mask head.  A file of the other model than `expect`'s raises one ValueError naming RAFT-small.  Missing,
+    unexpected and mis-shaped keys are reported in ONE ValueError (with `expect` = the model's `state_dict()`, against
+    its names and shapes)."""
     import torch
     label = 'state dict'
     sd = path_or_state_dict
@@ -408,16 +426,24 @@ def load_pytorch_checkpoint(path_or_state_dict, expect=None):
     for k, v in sd.items():
         k = k[len('module.'):] if k.startswith('module.') else k
         src[k] = v.detach().cpu().numpy() if isinstance(v, torch.Tensor) else np.asarray(v)
-    small = sorted(k for k in src if re.search(r'\.(conv3|norm4)\.', k))
-    if small:
-        raise ValueError(f'{label}: bottleneck-block keys {small[:4]} -- a RAFT-small checkpoint; only the basic RAFT '
-                         'model loads (this SmallRAFT is built from residual blocks)')
+    small_keys = sorted(k for k in src if re.search(r'\.(conv3|norm4)\.', k))
+    small = bool(small_keys)
+    if expect is not None:
+        want_small = any(re.search(r'\.conv3\.', k) for k in dict(expect))
+        if small and not want_small:
+            raise ValueError(f'{label}: bottleneck-block keys {small_keys[:4]} -- a RAFT-small checkpoint; load it into '
+                             "SmallRAFT(conventions='pytorch', blocks='bottleneck'), not the basic RAFT model")
+        if want_small and not small:
+            raise ValueError(f'{label}: no bottleneck-block (conv3) keys -- not a RAFT-small checkpoint, which the model '
+                             "(RAFT-small) needs; a basic RAFT checkpoint loads into RAFT(conventions='pytorch')")
+    # the downsample norm's twin: ResidualBlock registers it as norm3 too, BottleneckBlock as norm4
+    twin_norm = 'norm4' if small else 'norm3'
     params, extra, twins = {}, [], []
     for k, v in src.items():
         if k.endswith('.num_batches_tracked'):
             continue
-        m = re.fullmatch(r'(.*\.layer\d\.\d)\.norm3\.(weight|bias|running_mean|running_var)', k)
-        if m:                                  # ResidualBlock.norm3 is also downsample.1: keep one copy
+        m = re.fullmatch(r'(.*\.layer\d\.\d)\.' + twin_norm + r'\.(weight|bias|running_mean|running_var)', k)
+        if m:                                  # the block's norm3 / norm4 is also downsample.1: keep one copy
             twin = f'{m.group(1)}.downsample.1.{m.group(2)}'
             if twin not in src or np.shape(src[twin]) != np.shape(v) or not np.array_equal(src[twin], v):
                 twins.append(k)
@@ -437,14 +463,8 @@ def load_pytorch_checkpoint(path_or_state_dict, expect=None):
         if 'update_block.mask.2.bias' in params and params['update_block.mask.2.bias'].shape == (576,):
             params['update_block.mask.2.bias'] = params['update_block.mask.2.bias'][perm]
     # fnet's nn.InstanceNorm2d(affine=False): the identity affine of tfa InstanceNormalization
-    fnorms = [('fnet.norm1', 64)]
-    for li, (c, stride) in enumerate(((64, 1), (96, 2), (128, 2)), start=1):
-        for bi in (0, 1):
-            fnorms += [(f'fnet.layer{li}.{bi}.norm1', c), (f'fnet.layer{li}.{bi}.norm2', c)]
-            if bi == 0 and stride != 1:
-                fnorms.append((f'fnet.layer{li}.{bi}.downsample.1', c))
     if any(k.startswith('fnet.') for k in params):
-        for name, c in fnorms:
+        for name, c in _pt_instance_norms(small):
             if f'{name}.gamma' not in params:
                 params[f'{name}.gamma'] = np.ones(c, np.float32)
                 params[f'{name}.beta'] = np.zeros(c, np.float32)
@@ -452,7 +472,7 @@ def load_pytorch_checkpoint(path_or_state_dict, expect=None):
         raise ValueError(f'{label}: no fnet / cnet / update_block parameters found')
     problems = []
     if twins:
-        problems.append(f'norm3 differing from its downsample.1 twin {twins[:4]}')
+        problems.append(f'{twin_norm} differing from its downsample.1 twin {twins[:4]}')
     if expect is not None:
         want = {k: tuple(np.shape(v)) for k, v in dict(expect).items()}
         missing = sorted(set(want) - set(params))
@@ -476,7 +496,8 @@ def to_pytorch_state_dict(params, num_batches_tracked=0):
     state dict the original PyTorch RAFT loads (float32 CPU tensors): `module.` prefix, HWIO kernels as OIHW weights,
     gamma / beta / moving_mean / moving_variance as weight / bias / running_mean / running_var plus an int64
     `num_batches_tracked`, each ResidualBlock's `norm3` written again as its `downsample.1` twin, the mask head back in
-    RAFT's channel order, and no entries for fnet's norms (nn.InstanceNorm2d(affine=False) has none)."""
+    RAFT's channel order, and no entries for fnet's norms (nn.InstanceNorm2d(affine=False) has none).  A RAFT-small
+    model's parameters give convolution weights and biases only, the layout of `raft-small.pth`."""
     import torch
     inv_norm = {v: k for k, v in _PT_NORM.items()}
     out = OrderedDict()

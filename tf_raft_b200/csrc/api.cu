@@ -23,6 +23,12 @@ thread_local long long g_launches = 0;
 
 static int check_dims(int B, int h, int w) { return (B > 0 && h > 0 && w > 0) ? 0 : RAFT_ERR_BAD_SHAPE; }
 static int check_variant(int v) { return (v == RAFT_VARIANT_BASIC || v == RAFT_VARIANT_SMALL) ? 0 : RAFT_ERR_BAD_ARG; }
+// The encoder entry points also take the original RAFT-small's bottleneck encoders, which have no BatchNorm; norm = -1
+// checks the variant alone.
+static int check_enc_variant(int v, int norm = -1) {
+  if (v == RAFT_VARIANT_SMALL_PYTORCH) return norm == RAFT_NORM_BATCH ? RAFT_ERR_BAD_ARG : RAFT_OK;
+  return check_variant(v);
+}
 static int check_precision(int p) { return (p == RAFT_PREC_FP32 || p == RAFT_PREC_F16X2) ? 0 : RAFT_ERR_BAD_ARG; }
 static int check_sampler(int s) { return (s == RAFT_SAMPLER_TF || s == RAFT_SAMPLER_GRID) ? 0 : RAFT_ERR_BAD_ARG; }
 static int check_conventions(int c) {
@@ -814,6 +820,15 @@ int raft_b200_upflow8(const float* flow, int B, int h, int w, float* out, void* 
                 w, out);
 }
 
+int raft_b200_upflow8_align_corners(const float* flow, int B, int h, int w, float* out, void* stream) {
+  if (!flow || !out || (reinterpret_cast<uintptr_t>(flow) & 7) || (reinterpret_cast<uintptr_t>(out) & 7)) return RAFT_ERR_BAD_ARG;
+  RAFT_TRY(check_dims(B, h, w));
+  // ATen's area_pixel_compute_scale (align_corners): (in - 1) / (out - 1), one IEEE fp32 division on the host
+  const float sy = (float)(h - 1) / (float)(8 * h - 1), sx = (float)(w - 1) / (float)(8 * w - 1);
+  return launch(upflow8_align_kernel, grid_for((size_t)B * h * w * 64), 256, 0, reinterpret_cast<cudaStream_t>(stream), flow,
+                B, h, w, sy, sx, out);
+}
+
 int raft_b200_upflow8_backward(const float* grad_up, int B, int h, int w, float* grad_flow, void* stream) {
   if (!grad_up || !grad_flow || (reinterpret_cast<uintptr_t>(grad_up) & 7) || (reinterpret_cast<uintptr_t>(grad_flow) & 7))
     return RAFT_ERR_BAD_ARG;
@@ -824,7 +839,7 @@ int raft_b200_upflow8_backward(const float* grad_up, int B, int h, int w, float*
 
 int raft_b200_encoder_prepared_bytes(int variant, int out_dim, size_t* bytes) {
   if (!bytes) return RAFT_ERR_BAD_ARG;
-  RAFT_TRY(check_variant(variant));
+  RAFT_TRY(check_enc_variant(variant));
   if (out_dim < 32 || out_dim > 256 || out_dim % 32) return RAFT_ERR_BAD_SHAPE;
   *bytes = enc_layout(variant, out_dim).total;
   return RAFT_OK;
@@ -841,6 +856,14 @@ int raft_b200_encoder_prepare_ex(int variant, int norm_type, int out_dim, const 
                          reinterpret_cast<cudaStream_t>(stream));
 }
 
+int raft_b200_encoder_prepare_bottleneck(int norm_type, int out_dim, const raft_bottleneck_encoder_weights* weights,
+                                         void* prepared, size_t prepared_bytes, void* stream) {
+  if (!weights || !prepared) return RAFT_ERR_BAD_ARG;
+  if (norm_type != RAFT_NORM_INSTANCE && norm_type != RAFT_NORM_NONE) return RAFT_ERR_BAD_ARG;
+  if (out_dim < 32 || out_dim > 256 || out_dim % 32) return RAFT_ERR_BAD_SHAPE;
+  return encoder_prepare_bottleneck(norm_type, out_dim, weights, prepared, prepared_bytes, reinterpret_cast<cudaStream_t>(stream));
+}
+
 int raft_b200_encoder_prepare(int variant, int norm_type, int out_dim, const raft_encoder_weights* weights,
                               void* prepared, size_t prepared_bytes, void* stream) {
   return raft_b200_encoder_prepare_ex(variant, norm_type, out_dim, weights, RAFT_CONVENTIONS_TF, prepared, prepared_bytes,
@@ -849,7 +872,7 @@ int raft_b200_encoder_prepare(int variant, int norm_type, int out_dim, const raf
 
 int raft_b200_encoder_workspace_bytes(int variant, int N, int H, int W, size_t* bytes) {
   if (!bytes) return RAFT_ERR_BAD_ARG;
-  RAFT_TRY(check_variant(variant));
+  RAFT_TRY(check_enc_variant(variant));
   RAFT_TRY(check_dims(N, H, W));
   *bytes = enc_ws_layout(nullptr, variant, N, H, W).total;
   return RAFT_OK;
@@ -859,8 +882,8 @@ int raft_b200_encoder_forward(int variant, int norm_type, int out_dim, const voi
                               int N, int H, int W, int training, int image_norm, float* out, void* workspace,
                               size_t workspace_bytes, void* stream) {
   if (!prepared || !images || !out || !workspace) return RAFT_ERR_BAD_ARG;
-  RAFT_TRY(check_variant(variant));
   if (norm_type < 0 || norm_type > 2) return RAFT_ERR_BAD_ARG;
+  RAFT_TRY(check_enc_variant(variant, norm_type));
   RAFT_TRY(check_dims(N, H, W));
   if (out_dim < 32 || out_dim > 256 || out_dim % 32 || H < 8 || W < 8) return RAFT_ERR_BAD_SHAPE;
   return encoder_forward(variant, norm_type, out_dim, prepared, images, N, H, W, training, image_norm, out, workspace, workspace_bytes,
@@ -877,7 +900,7 @@ int raft_b200_context_split(const float* cnet, int npix, int hidden, int context
 
 int raft_b200_encode_pair_workspace_bytes(int variant, int N, int H, int W, int cnet_dim, size_t* bytes) {
   if (!bytes) return RAFT_ERR_BAD_ARG;
-  RAFT_TRY(check_variant(variant));
+  RAFT_TRY(check_enc_variant(variant));
   RAFT_TRY(check_dims(N, H, W));
   if (cnet_dim < 1) return RAFT_ERR_BAD_SHAPE;
   *bytes = pair_ws_layout(nullptr, variant, N, H, W, cnet_dim).total;
@@ -890,8 +913,9 @@ int raft_b200_encode_pair(int variant, const void* fnet_prepared, int fnet_norm,
                           void* stream) {
   if (!fnet_prepared || !cnet_prepared || !image1 || !image2 || !fmap1 || !fmap2 || !net || !inp || !workspace)
     return RAFT_ERR_BAD_ARG;
-  RAFT_TRY(check_variant(variant));
   if (fnet_norm < 0 || fnet_norm > 2 || cnet_norm < 0 || cnet_norm > 2) return RAFT_ERR_BAD_ARG;
+  RAFT_TRY(check_enc_variant(variant, fnet_norm));
+  RAFT_TRY(check_enc_variant(variant, cnet_norm));
   RAFT_TRY(check_dims(N, H, W));
   const int cnet_dim = hidden + context;
   for (int d : {fnet_dim, cnet_dim})
@@ -959,6 +983,9 @@ int raft_b200_forward_loop_ex(int variant, const void* prepared, const float* co
   if (!pyr || !net || !inp || !coords1 || !flow_up || iters < 0) return RAFT_ERR_BAD_ARG;
   if (levels < 1 || levels > RAFT_MAX_LEVELS || radius < 0) return RAFT_ERR_BAD_ARG;
   RAFT_TRY(check_sampler(sampler));
+  // the original RAFT-small: SmallRAFT's update block and loop, with the align-corners upflow8
+  const bool upflow_align = variant == RAFT_VARIANT_SMALL_PYTORCH;
+  if (upflow_align) variant = RAFT_VARIANT_SMALL;
   UpdateCtx c;
   RAFT_TRY(make_ctx(c, variant, prepared, B, h, w, workspace, workspace_bytes, precision, stream));
   const VariantDims d = variant_dims(variant);
@@ -995,6 +1022,8 @@ int raft_b200_forward_loop_ex(int variant, const void* prepared, const float* co
     if (flow_up[i]) {                                                                               // :105 / :223
       if (variant == RAFT_VARIANT_BASIC)
         RAFT_TRY(raft_b200_upsample_convex(W.flow, W.mask, B, h, w, flow_up[i], stream));
+      else if (upflow_align)
+        RAFT_TRY(raft_b200_upflow8_align_corners(W.flow, B, h, w, flow_up[i], stream));
       else
         RAFT_TRY(raft_b200_upflow8(W.flow, B, h, w, flow_up[i], stream));
     }

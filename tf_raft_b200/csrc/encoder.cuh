@@ -5,6 +5,9 @@
 // Conventions (recorded in the prepared blob): RAFT_CONVENTIONS_TF as above with norm epsilon 1e-3, or
 // RAFT_CONVENTIONS_PYTORCH -- the original RAFT's symmetric padding ((k-1)/2 at every stride) and epsilon 1e-5.
 //   conv2 1x1.
+// RAFT_VARIANT_SMALL_PYTORCH: the original RAFT-small's SmallEncoder, the same stem and conv2 around six bottleneck
+// blocks (include/raft_b200.h, raft_bottleneck): 1x1 -> 3x3 (stride here) -> 1x1 over 8, 16 and 24 channels, each
+// narrow plane padded to one 64-channel K chunk; always under RAFT_CONVENTIONS_PYTORCH.
 // Norms: 'batch' in inference is a per-channel affine folded into the conv epilogue (everything fuses);
 // 'instance' (and 'batch' in training) need statistics of the raw conv output: two deterministic reduction
 // passes + one apply kernel that also does ReLU, the residual add and the fp16 hi/lo re-split.
@@ -34,6 +37,10 @@ struct EncLayout {
   TcWeightSlot bc1[6], bc2[6], bds[6];
   EncNormSlot bn1[6], bn2[6], bnd[6];
   int has_ds[6], bc[6], bstride[6];
+  int bottleneck;                             // RAFT_VARIANT_SMALL_PYTORCH: blocks are bottlenecks of width bw[k]
+  TcWeightSlot bc3[6];                        // bottleneck conv3 (1x1, bw -> bc) and its norm3
+  EncNormSlot bn3[6];
+  int bw[6];
   TcWeightSlot conv2;
   size_t conventions;                         // one byte: RAFT_CONVENTIONS_*
   size_t total;
@@ -55,14 +62,26 @@ inline EncLayout enc_layout(int variant, int out_dim) {
   };
   L.conv1 = conv_slot(1, 1, 147, S.c0);
   L.norm1 = norm_slot(S.c0);
+  L.bottleneck = variant == RAFT_VARIANT_SMALL_PYTORCH;
   int cin = S.c0;
   for (int k = 0; k < 6; ++k) {
     const int c = S.c[k / 2], st = (k % 2 == 0) ? S.s[k / 2] : 1;
     L.bc[k] = c; L.bstride[k] = st;
-    L.bc1[k] = conv_slot(3, 3, cin, c);
-    L.bc2[k] = conv_slot(3, 3, c, c);
-    L.bn1[k] = norm_slot(c);
-    L.bn2[k] = norm_slot(c);
+    if (L.bottleneck) {                       // conv1 1x1 cin -> c/4, conv2 3x3 (stride) c/4 -> c/4, conv3 1x1 c/4 -> c
+      const int q = c / 4;
+      L.bw[k] = q;
+      L.bc1[k] = conv_slot(1, 1, cin, q);
+      L.bc2[k] = conv_slot(3, 3, q, q);
+      L.bc3[k] = conv_slot(1, 1, q, c);
+      L.bn1[k] = norm_slot(q);
+      L.bn2[k] = norm_slot(q);
+      L.bn3[k] = norm_slot(c);
+    } else {
+      L.bc1[k] = conv_slot(3, 3, cin, c);
+      L.bc2[k] = conv_slot(3, 3, c, c);
+      L.bn1[k] = norm_slot(c);
+      L.bn2[k] = norm_slot(c);
+    }
     L.has_ds[k] = st != 1;
     if (L.has_ds[k]) { L.bds[k] = conv_slot(1, 1, cin, c); L.bnd[k] = norm_slot(c); }
     cin = c;
@@ -77,6 +96,7 @@ struct EncWs {
   float *X32, *O32, *Y32, *D32;
   __half *Xh, *Xl, *Oh, *Ol, *Fh, *Fl, *Ih, *Il;
   float *part, *mean, *mult;
+  __half *Gh, *Gl;                           // RAFT_VARIANT_SMALL_PYTORCH only: a bottleneck's 3x3 output
   size_t total;
 };
 constexpr int kNormSplit = 64;
@@ -107,6 +127,7 @@ inline EncWs enc_ws_layout(void* base, int variant, int N, int H, int W) {
   E.part = (float*)take((size_t)N * kNormSplit * 3 * 256 * 4);
   E.mean = (float*)take((size_t)N * 256 * 4);
   E.mult = (float*)take((size_t)N * 256 * 4);
+  if (variant == RAFT_VARIANT_SMALL_PYTORCH) { E.Gh = (__half*)take(max16 * 2); E.Gl = (__half*)take(max16 * 2); }
   E.total = off;
   return E;
 }
@@ -197,6 +218,39 @@ inline int encoder_prepare(int variant, int norm_type, int out_dim, const raft_e
   return raft_launch_status();
 }
 
+// The original RAFT-small's encoder (RAFT_VARIANT_SMALL_PYTORCH), always under the PyTorch conventions.
+inline int encoder_prepare_bottleneck(int norm_type, int out_dim, const raft_bottleneck_encoder_weights* w, void* prepared,
+                                      size_t bytes, cudaStream_t st) {
+  const EncLayout L = enc_layout(RAFT_VARIANT_SMALL_PYTORCH, out_dim);
+  if (L.total > bytes) return RAFT_ERR_WORKSPACE;
+  const EncSpec S = enc_spec(RAFT_VARIANT_SMALL_PYTORCH);
+  const float eps = enc_norm_eps(RAFT_CONVENTIONS_PYTORCH);
+  uint8_t* base = reinterpret_cast<uint8_t*>(prepared);
+  RAFT_CUDA_TRY(cudaMemsetAsync(base, 0, L.total, st));
+  RAFT_CUDA_TRY(cudaMemsetAsync(base + L.conventions, RAFT_CONVENTIONS_PYTORCH, 1, st));
+  enc_conventions_record(prepared, RAFT_CONVENTIONS_PYTORCH);
+  RAFT_TRY(enc_pack_conv(w->conv1, 7, 7, 3, S.c0, L.conv1, true, base, st));
+  RAFT_TRY(enc_pack_norm(w->norm1, L.norm1, norm_type, eps, base, st));
+  int cin = S.c0;
+  for (int k = 0; k < 6; ++k) {
+    const int c = L.bc[k], q = L.bw[k];
+    const raft_bottleneck& b = w->block[k];
+    RAFT_TRY(enc_pack_conv(b.conv1, 1, 1, cin, q, L.bc1[k], false, base, st));
+    RAFT_TRY(enc_pack_conv(b.conv2, 3, 3, q, q, L.bc2[k], false, base, st));
+    RAFT_TRY(enc_pack_conv(b.conv3, 1, 1, q, c, L.bc3[k], false, base, st));
+    RAFT_TRY(enc_pack_norm(b.norm1, L.bn1[k], norm_type, eps, base, st));
+    RAFT_TRY(enc_pack_norm(b.norm2, L.bn2[k], norm_type, eps, base, st));
+    RAFT_TRY(enc_pack_norm(b.norm3, L.bn3[k], norm_type, eps, base, st));
+    if (L.has_ds[k]) {
+      RAFT_TRY(enc_pack_conv(b.downsample, 1, 1, cin, c, L.bds[k], false, base, st));
+      RAFT_TRY(enc_pack_norm(b.downsample_norm, L.bnd[k], norm_type, eps, base, st));
+    }
+    cin = c;
+  }
+  RAFT_TRY(enc_pack_conv(w->conv2, 1, 1, cin, out_dim, L.conv2, false, base, st));
+  return raft_launch_status();
+}
+
 // ---- forward ----------------------------------------------------------------------------------
 struct EncCtx {
   const uint8_t* prep; EncLayout L; EncWs W; cudaStream_t st;
@@ -269,6 +323,51 @@ inline int enc_conv_tc(const EncCtx& c, const TcWeightSlot& cs, int cout, const 
   return tc_launch(p, nsplit, c.st);
 }
 
+// Bottleneck block k (RAFT_VARIANT_SMALL_PYTORCH) from the block input X (h x w, fp32 X32 when the norms fuse, fp16 hi/lo
+// planes always) to O (ho x wo): 1x1 -> F (h x w, width q), 3x3 at the block's stride -> G, optional 1x1 downsample -> D32,
+// 1x1 -> O with relu(skip + relu(norm3(.))).  Every narrow plane (q < 64, or cc = 32 / 96) has its channels past the
+// width cleared before the next layer reads its 64-channel K chunk: norm_apply_kernel writes them as zeros, a fused
+// epilogue writes only whole 32-column chunks, so the plane is cleared first.
+inline int enc_bottleneck(const EncCtx& c, int k, int h, int w, int ho, int wo, const float* X32, const __half* Xh,
+                          const __half* Xl, float* O32, __half* Oh, __half* Ol) {
+  const EncLayout& L = c.L;
+  const EncWs& E = c.W;
+  const cudaStream_t st = c.st;
+  const int st2 = L.bstride[k], cc = L.bc[k], q = L.bw[k];
+  const size_t npi = (size_t)c.N * h * w, npo = (size_t)c.N * ho * wo;
+  auto clear = [&](__half* hi, __half* lo, size_t np, int ch) -> int {
+    if (c.stats || pad64(ch) == ch) return RAFT_OK;
+    RAFT_CUDA_TRY(cudaMemsetAsync(hi, 0, np * pad64(ch) * 2, st));
+    RAFT_CUDA_TRY(cudaMemsetAsync(lo, 0, np * pad64(ch) * 2, st));
+    return RAFT_OK;
+  };
+  // conv1 1x1 + norm1 + relu -> F (input resolution)
+  RAFT_TRY(clear(E.Fh, E.Fl, npi, q));
+  RAFT_TRY(enc_conv_tc(c, L.bc1[k], q, &L.bn1[k], Xh, Xl, h, w, h, w, 1, 1, nullptr, c.stats ? E.Y32 : nullptr, E.Fh, E.Fl));
+  if (c.stats) RAFT_TRY(enc_norm_apply(c, L.bn1[k], E.Y32, npi, h * w, 1, nullptr, nullptr, nullptr, nullptr, E.Fh, E.Fl));
+  // conv2 3x3 at the block's stride + norm2 + relu -> G
+  RAFT_TRY(clear(E.Gh, E.Gl, npo, q));
+  RAFT_TRY(enc_conv_tc(c, L.bc2[k], q, &L.bn2[k], E.Fh, E.Fl, h, w, ho, wo, st2, 1, nullptr, c.stats ? E.Y32 : nullptr, E.Gh,
+                       E.Gl));
+  if (c.stats) RAFT_TRY(enc_norm_apply(c, L.bn2[k], E.Y32, npo, ho * wo, 1, nullptr, nullptr, nullptr, nullptr, E.Gh, E.Gl));
+  // skip branch: downsample 1x1 at the stride + norm4 -> D32, or the block input
+  const float* skip = X32;
+  if (L.has_ds[k]) {
+    RAFT_TRY(enc_conv_tc(c, L.bds[k], cc, &L.bnd[k], Xh, Xl, h, w, ho, wo, st2, 0, nullptr, c.stats ? E.Y32 : E.D32, nullptr,
+                         nullptr));
+    if (c.stats) RAFT_TRY(enc_norm_apply(c, L.bnd[k], E.Y32, npo, ho * wo, 0, nullptr, nullptr, nullptr, E.D32, nullptr, nullptr));
+    skip = E.D32;
+  }
+  // conv3 1x1 + norm3 + relu, then relu(skip + y) -> O
+  RAFT_TRY(clear(Oh, Ol, npo, cc));
+  RAFT_TRY(enc_conv_tc(c, L.bc3[k], cc, &L.bn3[k], E.Gh, E.Gl, ho, wo, ho, wo, 1, 1, skip, c.stats ? E.Y32 : O32, Oh, Ol));
+  if (c.stats) {   // skip = block input: from D32 after a downsample, else from the block's own fp16 operand planes
+    if (L.has_ds[k]) return enc_norm_apply(c, L.bn3[k], E.Y32, npo, ho * wo, 1, E.D32, nullptr, nullptr, nullptr, Oh, Ol);
+    return enc_norm_apply(c, L.bn3[k], E.Y32, npo, ho * wo, 1, nullptr, Xh, Xl, nullptr, Oh, Ol);
+  }
+  return raft_launch_status();
+}
+
 // The stem's operand: the 7x7 s2 input window of every output pixel as 192-channel fp16 planes (E.Ih / E.Il of `ws`).
 // It depends on the images alone, so encoders of the same images can share it (raft_b200_encode_pair).
 inline int encoder_stem_im2col(int variant, const float* images, int N, int H, int W, int image_norm, int conventions,
@@ -332,6 +431,14 @@ inline int encoder_forward(int variant, int norm_type, int out_dim, const void* 
     const int ho = (h + st2 - 1) / st2, wo = (w + st2 - 1) / st2;
     const size_t npo = (size_t)N * ho * wo;
     const bool zero_pad_out = pad64(cc) != cc;     // fused epilogues write 32-column chunks: clear the 64-pad tail
+    if (L.bottleneck) {
+      RAFT_TRY(enc_bottleneck(c, k, h, w, ho, wo, X32, Xh, Xl, O32, Oh, Ol));
+      float* t32 = X32; X32 = O32; O32 = t32;
+      __half* th_ = Xh; Xh = Oh; Oh = th_;
+      __half* tl_ = Xl; Xl = Ol; Ol = tl_;
+      h = ho; w = wo;
+      continue;
+    }
     // conv1 + norm1 + relu -> F
     if (!c.stats && zero_pad_out) {
       RAFT_CUDA_TRY(cudaMemsetAsync(E.Fh, 0, npo * pad64(cc) * 2, st));

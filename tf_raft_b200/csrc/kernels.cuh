@@ -541,6 +541,36 @@ __global__ void upflow8_kernel(const float* __restrict__ flow, int B, int h, int
   }
 }
 
+// upflow8 of the original RAFT-small: 8 * F.interpolate(flow, size=(8h, 8w), mode='bilinear', align_corners=True), with
+// ATen upsample_bilinear2d's source index and weights.  Per axis of n cells, scale = fl((n-1) / (8n-1)) from the host:
+// src = fl(scale * X), i0 = (int)src, i1 = i0 + (i0 < n-1), l1 = fl(src - i0), l0 = fl(1 - l1).  The value is
+// l0y * (l0x * a + l1x * b) + l1y * (l0x * c + l1x * d), every operation one rounded fp32 operation in that order (no
+// FMA), then times 8 (exact).  One thread per output pixel, both channels.
+__global__ void __launch_bounds__(256) upflow8_align_kernel(const float* __restrict__ flow, int B, int h, int w,
+                                                            float scale_y, float scale_x, float* __restrict__ out) {
+  const int H = 8 * h, W = 8 * w;
+  const size_t total = (size_t)B * H * W;
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const int X = (int)(i % W), Y = (int)((i / W) % H);
+    const size_t b = i / ((size_t)W * H);
+    const float sx = __fmul_rn(scale_x, (float)X), sy = __fmul_rn(scale_y, (float)Y);
+    const int x0 = (int)sx, y0 = (int)sy;
+    const int x1 = x0 + (x0 < w - 1 ? 1 : 0), y1 = y0 + (y0 < h - 1 ? 1 : 0);
+    const float lx1 = __fsub_rn(sx, (float)x0), ly1 = __fsub_rn(sy, (float)y0);
+    const float lx0 = __fsub_rn(1.0f, lx1), ly0 = __fsub_rn(1.0f, ly1);
+    const float2* f = reinterpret_cast<const float2*>(flow) + b * h * w;
+    const float2 a = __ldg(f + (size_t)y0 * w + x0), bb = __ldg(f + (size_t)y0 * w + x1);
+    const float2 c = __ldg(f + (size_t)y1 * w + x0), d = __ldg(f + (size_t)y1 * w + x1);
+    const float top0 = __fadd_rn(__fmul_rn(lx0, a.x), __fmul_rn(lx1, bb.x));
+    const float top1 = __fadd_rn(__fmul_rn(lx0, a.y), __fmul_rn(lx1, bb.y));
+    const float bot0 = __fadd_rn(__fmul_rn(lx0, c.x), __fmul_rn(lx1, d.x));
+    const float bot1 = __fadd_rn(__fmul_rn(lx0, c.y), __fmul_rn(lx1, d.y));
+    const float v0 = __fadd_rn(__fmul_rn(ly0, top0), __fmul_rn(ly1, bot0));
+    const float v1 = __fadd_rn(__fmul_rn(ly0, top1), __fmul_rn(ly1, bot1));
+    reinterpret_cast<float2*>(out)[i] = make_float2(__fmul_rn(8.0f, v0), __fmul_rn(8.0f, v1));
+  }
+}
+
 // Backward of the training graph's F.interpolate(scale_factor=8, mode='bilinear', align_corners=False) (SmallRAFT's
 // upsampling), with PyTorch upsample_bilinear2d's source indices and weights.  Per output coordinate X of an input axis
 // of n cells: src = max(0.125 * (X + 0.5) - 0.5, 0), i0 = (int)src, i1 = i0 + (i0 < n - 1), l1 = src - i0, l0 = 1 - l1

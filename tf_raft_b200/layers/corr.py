@@ -111,14 +111,17 @@ def coords_init(flow_init):
     return out
 
 
-def upflow8(flow, mode='bilinear'):
-    """Reference corr.py:93-96: 8 * tf.image.resize(flow, (8h, 8w), 'bilinear') (half-pixel centres)."""
+def upflow8(flow, mode='bilinear', align_corners=False):
+    """Reference corr.py:93-96: 8 * tf.image.resize(flow, (8h, 8w), 'bilinear') (half-pixel centres).
+
+    `align_corners=True` (an addition): the original PyTorch RAFT-small's upflow8, 8 * F.interpolate(flow, size=(8h, 8w),
+    mode='bilinear', align_corners=True) in ATen's arithmetic (raft_b200_upflow8_align_corners)."""
     if mode != 'bilinear':
         raise NotImplementedError("only mode='bilinear' is implemented")
-    flow = _lib.f32c(flow)
+    flow = _flow_field(flow, 'upflow8') if align_corners else _lib.f32c(flow)
     b, h, w, _ = flow.shape
     out = torch.empty((b, 8 * h, 8 * w, 2), dtype=torch.float32, device=flow.device)
-    _lib.call('upflow8', flow.device, _lib.ptr(flow), b, h, w, _lib.ptr(out))
+    _lib.call('upflow8_align_corners' if align_corners else 'upflow8', flow.device, _lib.ptr(flow), b, h, w, _lib.ptr(out))
     return out
 
 

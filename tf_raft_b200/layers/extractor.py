@@ -9,6 +9,9 @@ independent GPU cross-check of the native path, never selected implicitly.
 Parameter names are the reference's Keras attribute paths, kernels HWIO, NHWC tensors at the interface.
 `conventions='pytorch'` (keyword-only) computes what the original PyTorch RAFT's encoders compute on both backends:
 symmetric padding at stride 2 and eps = 1e-5 (include/raft_b200.h, raft_conventions).
+`SmallEncoder(..., conventions='pytorch', blocks='bottleneck')` is the original RAFT-small's encoder: the same stem and
+conv2 around six bottleneck blocks (1x1 -> 3x3 at the block's stride -> 1x1, widths 8, 16, 24), parameters named by the
+original module paths (`layer2.0.conv3`, `layer2.0.downsample.0`, norms `norm1..3`, `downsample.1`).
 """
 import ctypes
 import os
@@ -49,14 +52,26 @@ class _Encoder:
     _c0 = 0
     _stages = ()
     _variant = None
+    _blocks = ('residual',)
 
     def __init__(self, output_dim=128, norm_type='batch', drop_rate=0.0, *, device='cuda', seed=None, backend=None,
-                 conventions='tf-raft'):
+                 conventions='tf-raft', blocks='residual'):
         self.backend = backend or os.environ.get('RAFT_B200_ENCODER', 'native')
         if self.backend not in ('native', 'torch'):
             raise ValueError(f'unknown encoder backend {self.backend!r}')
         if conventions not in _lib.CONVENTIONS:
             raise ValueError(f'unknown conventions {conventions!r}; expected one of {", ".join(_lib.CONVENTIONS)}')
+        if blocks not in self._blocks:
+            raise ValueError(f'{type(self).__name__}: unknown blocks {blocks!r}; expected one of {", ".join(self._blocks)}')
+        if blocks == 'bottleneck':
+            if conventions != 'pytorch':
+                raise ValueError("blocks='bottleneck' is the original PyTorch RAFT-small's encoder and needs "
+                                 "conventions='pytorch'; tf-raft's SmallEncoder is built from residual blocks")
+            if norm_type not in ('instance', None):
+                raise ValueError(f"blocks='bottleneck' takes norm_type 'instance' or None (the original RAFT-small's); "
+                                 f'got {norm_type!r}')
+            self._variant = _lib.VARIANT_SMALL_PYTORCH
+        self.blocks = blocks
         self.conventions = conventions
         self._prepared = None
         self.workspaces = _lib.WorkspaceCache()
@@ -71,6 +86,17 @@ class _Encoder:
         for li, (c, stride) in enumerate(self._stages, start=1):
             for bi, st in enumerate((stride, 1)):
                 p = f'layer{li}.{bi}'
+                if blocks == 'bottleneck':
+                    s.add_conv(p + '.conv1', 1, 1, cin, c // 4)
+                    s.add_conv(p + '.conv2', 3, 3, c // 4, c // 4)
+                    s.add_conv(p + '.conv3', 1, 1, c // 4, c)
+                    for n, width in (('norm1', c // 4), ('norm2', c // 4), ('norm3', c)):
+                        s.add_norm(f'{p}.{n}', norm_type, width)
+                    if st != 1:
+                        s.add_conv(p + '.downsample.0', 1, 1, cin, c)
+                        s.add_norm(p + '.downsample.1', norm_type, c)
+                    cin = c
+                    continue
                 s.add_conv(p + '.conv1', 3, 3, cin, c)
                 s.add_conv(p + '.conv2', 3, 3, c, c)
                 s.add_norm(p + '.norm1', norm_type, c)
@@ -106,7 +132,31 @@ class _Encoder:
         return _lib.RaftNorm(p[name + '.gamma'].data_ptr(), p[name + '.beta'].data_ptr(),
                              None if mm is None else mm.data_ptr(), None if mv is None else mv.data_ptr())
 
+    def _prepared_bottleneck(self, blob):
+        w = _lib.RaftBottleneckEncoderWeights()
+        w.conv1 = self._conv_struct('conv1')
+        w.norm1 = self._norm_struct('norm1')
+        k = 0
+        for li, (_, stride) in enumerate(self._stages, start=1):
+            for bi, st in enumerate((stride, 1)):
+                p = f'layer{li}.{bi}'
+                blk = w.block[k]
+                blk.conv1, blk.conv2, blk.conv3 = (self._conv_struct(f'{p}.conv{i}') for i in (1, 2, 3))
+                blk.norm1, blk.norm2, blk.norm3 = (self._norm_struct(f'{p}.norm{i}') for i in (1, 2, 3))
+                if st != 1:
+                    blk.downsample = self._conv_struct(p + '.downsample.0')
+                    blk.downsample_norm = self._norm_struct(p + '.downsample.1')
+                k += 1
+        w.conv2 = self._conv_struct('conv2')
+        _lib.call('encoder_prepare_bottleneck', blob.device, _lib.NORM_TYPES[self.norm_type], self.output_dim,
+                  ctypes.cast(ctypes.pointer(w), ctypes.c_void_p), _lib.ptr(blob), blob.numel())
+
     def prepared(self):
+        if self._prepared is None and self.blocks == 'bottleneck':
+            blob = _lib.workspace(_lib.query_bytes('encoder_prepared_bytes', self._variant, self.output_dim),
+                                  self.store.device)
+            self._prepared_bottleneck(blob)
+            self._prepared = blob
         if self._prepared is None:
             w = _lib.RaftEncoderWeights()
             w.conv1 = self._conv_struct('conv1')
@@ -153,6 +203,16 @@ class _Encoder:
             x = s.norm(s.conv(x, p + '.downsample.0', stride, padding='valid'), p + '.downsample.1', nt, training)
         return F.relu(x + fx)
 
+    def _bottleneck_block(self, x, p, stride, training):
+        """The original RAFT's BottleneckBlock.forward (symmetric padding through the store's 'pytorch' conventions)."""
+        s, nt = self.store, self.norm_type
+        y = F.relu(s.norm(s.conv(x, p + '.conv1', 1), p + '.norm1', nt, training))
+        y = F.relu(s.norm(s.conv(y, p + '.conv2', stride), p + '.norm2', nt, training))
+        y = F.relu(s.norm(s.conv(y, p + '.conv3', 1), p + '.norm3', nt, training))
+        if stride != 1:
+            x = s.norm(s.conv(x, p + '.downsample.0', stride, padding='valid'), p + '.downsample.1', nt, training)
+        return F.relu(x + y)
+
     def __call__(self, inputs, training=False, *, raw_image=False):
         """NHWC tensor, or a list/tuple of two (concatenated along the batch, split on return).
 
@@ -171,9 +231,10 @@ class _Encoder:
         x = x.permute(0, 3, 1, 2)
         s, nt = self.store, self.norm_type
         x = F.relu(s.norm(s.conv(x, 'conv1', 2), 'norm1', nt, training))
+        block = self._bottleneck_block if self.blocks == 'bottleneck' else self._res_block
         for li, (_, stride) in enumerate(self._stages, start=1):
-            x = self._res_block(x, f'layer{li}.0', stride, training)
-            x = self._res_block(x, f'layer{li}.1', 1, training)
+            x = block(x, f'layer{li}.0', stride, training)
+            x = block(x, f'layer{li}.1', 1, training)
         x = s.conv(x, 'conv2', 1, padding='valid')
         if self.drop_rate > 0 and training:
             x = F.dropout(x, self.drop_rate, training=True)
@@ -192,7 +253,9 @@ class BasicEncoder(_Encoder):
 
 
 class SmallEncoder(_Encoder):
-    """Reference extractor.py:133-175 (built from ResBlocks, not bottlenecks)."""
+    """Reference extractor.py:133-175 (built from ResBlocks); with conventions='pytorch', blocks='bottleneck' the
+    original PyTorch RAFT-small's encoder (bottleneck blocks, norm 'instance' or None)."""
     _c0 = 32
     _stages = ((32, 1), (64, 2), (96, 2))
     _variant = _lib.VARIANT_SMALL
+    _blocks = ('residual', 'bottleneck')

@@ -28,11 +28,12 @@ class RAFT:
 
     def __init__(self, drop_rate=0, iters=12, iters_pred=24, *, precision=None, device='cuda', seed=None,
                  use_graph=False, encoder_backend=None, conventions='tf-raft', **kwargs):
+        if 'blocks' in kwargs:
+            raise TypeError("RAFT takes no 'blocks' argument: the basic model is built from residual blocks "
+                            "(SmallRAFT(conventions='pytorch', blocks='bottleneck') is the original RAFT-small)")
         if conventions not in _lib.CONVENTIONS:
             raise ValueError(f'unknown conventions {conventions!r}; expected one of {", ".join(_lib.CONVENTIONS)}')
-        if conventions == 'pytorch' and self._variant != _lib.VARIANT_BASIC:
-            raise ValueError("conventions='pytorch' is RAFT's only: the original RAFT-small's encoder is built from "
-                             'bottleneck blocks, this SmallRAFT from residual blocks')
+        self._check_conventions(conventions)
         self.conventions = conventions
         self.hidden_dim = 128
         self.context_dim = 128
@@ -56,6 +57,9 @@ class RAFT:
         self._pending_slots = None                         # optimiser state of load_weights awaiting the Trainer
         self._frozen_bn = False                            # freeze_bn() (conventions='pytorch')
         self._num_batches_tracked = 0                      # training-mode BatchNorm steps, for save_pytorch_weights
+
+    def _check_conventions(self, conventions):
+        """Raises ValueError for a convention this model cannot compute (SmallRAFT restricts it)."""
 
     def _encoder_backend(self):
         # the all-FFMA reference configuration keeps cuDNN IEEE-fp32 encoders; the product path is native
@@ -140,7 +144,8 @@ class RAFT:
             self._build_trainer()
 
     def load_pytorch_weights(self, path):
-        """Loads a checkpoint of the original PyTorch RAFT (`raft-things.pth`, ...; a path or a state dict) through
+        """Loads a checkpoint of the original PyTorch RAFT (`raft-things.pth`, ...; `raft-small.pth` into
+        SmallRAFT(conventions='pytorch', blocks='bottleneck'); a path or a state dict) through
         `load_pytorch_checkpoint`.  Only a model built with `conventions='pytorch'` computes what those weights were
         trained for; any other raises ValueError."""
         from .checkpoint import load_pytorch_checkpoint
@@ -504,9 +509,13 @@ class RAFT:
         self.flow_metrics = OrderedDict((k, [0.0, 0]) for k in ('loss', 'epe', 'u1', 'u3', 'u5'))
 
     def _check_trainable(self, optimizer, loss=None):
-        """conventions='pytorch' trains the original RAFT's step only: TorchAdamW, the supervised loss."""
+        """conventions='pytorch' trains the original RAFT's step only: TorchAdamW, the supervised loss; the original
+        RAFT-small (SmallRAFT(blocks='bottleneck')) runs inference only."""
         from .losses import UnsupervisedLoss
         from .train import TorchAdamW
+        if getattr(self, 'blocks', 'residual') == 'bottleneck':
+            raise NotImplementedError("SmallRAFT(blocks='bottleneck') (the original RAFT-small) runs inference only: "
+                                      'its training step is not implemented')
         if self.conventions != 'pytorch':
             return
         if not isinstance(optimizer, TorchAdamW):
@@ -587,7 +596,27 @@ class RAFT:
 
 
 class SmallRAFT(RAFT):
+    """tf-raft's SmallRAFT (model.py:173-226).  `SmallRAFT(conventions='pytorch', blocks='bottleneck')` is the original
+    PyTorch RAFT-small, the model of `raft-small.pth` (`load_pytorch_weights`): bottleneck-block encoders under PyTorch
+    padding and eps, the grid_sample lookup, and 8 * F.interpolate(align_corners=True) upsampling (DESIGN.md section
+    11.2).  It runs inference only."""
     _variant = _lib.VARIANT_SMALL
+
+    def __init__(self, drop_rate=0, iters=12, iters_pred=24, *, blocks='residual', **kwargs):
+        if blocks not in ('residual', 'bottleneck'):
+            raise ValueError(f"unknown blocks {blocks!r}; expected 'residual' or 'bottleneck'")
+        self.blocks = blocks
+        if blocks == 'bottleneck':
+            self._variant = _lib.VARIANT_SMALL_PYTORCH
+        super().__init__(drop_rate, iters, iters_pred, **kwargs)
+
+    def _check_conventions(self, conventions):
+        if conventions == 'pytorch' and self.blocks != 'bottleneck':
+            raise ValueError("SmallRAFT(conventions='pytorch') is the original RAFT-small, whose encoders are built from "
+                             "bottleneck blocks: pass blocks='bottleneck' (tf-raft's SmallRAFT uses residual blocks)")
+        if self.blocks == 'bottleneck' and conventions != 'pytorch':
+            raise ValueError("blocks='bottleneck' is the original PyTorch RAFT-small and needs conventions='pytorch'; "
+                             'tf-raft never uses the bottleneck block')
 
     def _build_layers(self, seed):
         self.hidden_dim = 96
@@ -595,13 +624,14 @@ class SmallRAFT(RAFT):
         self.corr_levels = 4
         self.corr_radius = 3
         s = 0 if seed is None else seed
-        self.fnet = SmallEncoder(output_dim=128, norm_type='instance', drop_rate=self.drop_rate, device=self.device,
-                                 seed=s, backend=self._encoder_backend())
-        self.cnet = SmallEncoder(output_dim=self.hidden_dim + self.context_dim, norm_type=None,
-                                 drop_rate=self.drop_rate, device=self.device, seed=s + 1, backend=self._encoder_backend())
+        enc = dict(drop_rate=self.drop_rate, device=self.device, backend=self._encoder_backend())
+        if self.blocks == 'bottleneck':
+            enc.update(conventions=self.conventions, blocks='bottleneck')
+        self.fnet = SmallEncoder(output_dim=128, norm_type='instance', seed=s, **enc)
+        self.cnet = SmallEncoder(output_dim=self.hidden_dim + self.context_dim, norm_type=None, seed=s + 1, **enc)
         self.update_block = SmallUpdateBlock(filters=self.hidden_dim, precision=self.precision, device=self.device,
                                              seed=s + 2)
 
     def upsample_flow(self, flow, mask=None):
-        """SmallRAFT upsamples with upflow8 (model.py:223)."""
-        return upflow8(flow)
+        """SmallRAFT upsamples with upflow8 (model.py:223); the original RAFT-small with its align-corners form."""
+        return upflow8(flow, align_corners=self.blocks == 'bottleneck')
