@@ -294,6 +294,45 @@ int raft_b200_augment_sparse(const raft_augment_sample* samples_host, const raft
                              void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Colour jitter  (the original RAFT's core/utils/augmentor.py colour step: torchvision ColorJitter on RGB PIL images,
+ * Pillow's arithmetic, given ColorJitter.get_params' draws)
+ * ------------------------------------------------------------------------------------------- */
+
+/* Ops of raft_colour_jitter_sample.order, torchvision's fn_idx values.                                               */
+enum { RAFT_JITTER_NONE = -1, RAFT_JITTER_BRIGHTNESS = 0, RAFT_JITTER_CONTRAST = 1, RAFT_JITTER_SATURATION = 2,
+       RAFT_JITTER_HUE = 3 };
+
+/* One sample: two (H, W, 3) uint8 images, device memory, HWC and contiguous, jittered into out_img1 / out_img2 (which
+ * may be the sources).  stacked != 0: parameter set 0 jitters img1 stacked above img2 as one (2H, W) image;
+ * otherwise set k jitters image k.  A set applies order[0..3] to every pixel, each op at most once; RAFT_JITTER_NONE
+ * stands for an op that ColorJitter skips (a strength of 0 makes get_params return None for its factor):
+ *   brightness  c = blend(0, c, factor[0])
+ *   contrast    c = blend(m, c, factor[1]), m = int(S / n + 0.5) in float64, S the integer sum of L over the set's
+ *               n pixels after the ops before contrast
+ *   saturation  c = blend(L, c, factor[2]), L the pixel's own L
+ *   hue         Pillow RGB->HSV, H = (H + hue) mod 256, Pillow HSV->RGB (the round trip also runs for hue = 0)
+ * with blend(a, b, f) = clip(trunc(fl32(a + fl32(f * (b - a)))), 0, 255) and L = (19595 R + 38470 G + 7471 B + 0x8000)
+ * >> 16.  Pillow's RGB<->HSV mixes float32 and float64 as its C source promotes them (DESIGN.md section 3.8).       */
+typedef struct raft_colour_jitter_sample {
+  const uint8_t* img1;
+  const uint8_t* img2;
+  uint8_t* out_img1;
+  uint8_t* out_img2;
+  int H, W;
+  int stacked;
+  int order[2][4];              /* per set: the ops in application order, or RAFT_JITTER_NONE                      */
+  float factor[2][3];           /* per set: brightness, contrast and saturation factors, finite                    */
+  int hue[2];                   /* per set: the byte added to H, 0..255: uint8(int32(hue_factor * 255))            */
+} raft_colour_jitter_sample;
+
+/* ColorJitter on B samples of any sizes in one launch pair (2 kernels after a memset of sums).  samples_host and
+ * samples_dev hold the same array (host copy for checks and grid sizes, device copy read by the kernels).
+ * sums: device, 2 * B unsigned 64-bit words, overwritten (the L sums of each sample's two sets).  Set 1 of a stacked
+ * sample is neither checked nor read.  Asynchronous on `stream`, no allocation: graph-capturable.                    */
+int raft_b200_colour_jitter(const raft_colour_jitter_sample* samples_host, const raft_colour_jitter_sample* samples_dev,
+                            int B, unsigned long long* sums, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Flow visualisation  (tf_raft/datasets/flow_viz.py: make_colorwheel :20-67, flow_uv_to_colors :70-106,
  * flow_to_image :109-132)
  * ------------------------------------------------------------------------------------------- */

@@ -26,6 +26,10 @@ the sequence loss's weight decay over the iterations (RAFT's later stages use 0.
 written as a `.pth` the original code reads, `<logdir>/<timestamp>/checkpoints/model.pth`, at the end.  Refused with
 `--small` and `--self-supervised`.
 
+`--colour-jitter torchvision` replaces tf-raft's albumentations colour augmentation with the original RAFT's torchvision
+ColorJitter on PIL images (DESIGN.md section 3.8), and `--add-noise` adds RAFT's `--add_noise` Gaussian noise to both
+training images.  Both are opt-in in every mode, and both draw from torch's CPU generator, which `--seed` then seeds too.
+
 `--self-supervised` compiles with `UnsupervisedLoss()` (DESIGN.md section 9.1): the training batches' ground truth is not
 used by the loss (the epe metrics of the forward prediction are still logged); the config, datasets, validation (val_epe
 against ground truth) and callbacks are the same.
@@ -38,6 +42,7 @@ import sys
 from datetime import datetime
 
 import numpy as np
+import torch
 
 try:
     import yaml
@@ -72,9 +77,11 @@ def need(config, path):
 
 
 def train(name, config, logdir, small=False, workers=4, self_supervised=False, train_precision='fp32',
-          pytorch_checkpoint=None, freeze_bn=False, gamma=None):
+          pytorch_checkpoint=None, freeze_bn=False, gamma=None, colour_jitter='albumentations', add_noise=False):
     root = need(config, 'data.root')
     aug_params = need(config, 'augment')
+    if colour_jitter != 'albumentations':
+        aug_params = dict(aug_params, colour=colour_jitter)
     iters, iters_pred, resume = (need(config, 'model.' + k) for k in ('iters', 'iters_pred', 'resume'))
     epochs, batch_size, learning_rate, weight_decay, clip_norm = (
         need(config, 'train.' + k) for k in ('epochs', 'batch_size', 'learning_rate', 'weight_decay', 'clip_norm'))
@@ -130,7 +137,10 @@ def train(name, config, logdir, small=False, workers=4, self_supervised=False, t
         T.ModelCheckpoint(filepath=os.path.join(logdir, 'checkpoints', 'model'), save_weights_only=True,
                           monitor='val_epe', mode='min', save_best_only=True),
     ]
-    history = raft.fit(ds_train.batches(batch_size, workers=workers, repeat=True), epochs=epochs, callbacks=callbacks,
+    batches = ds_train.batches(batch_size, workers=workers, repeat=True)
+    if add_noise:
+        batches = (D.add_noise(b[0], b[1]) + tuple(b[2:]) for b in batches)
+    history = raft.fit(batches, epochs=epochs, callbacks=callbacks,
                        steps_per_epoch=steps_per_epoch,
                        validation_data=Batches(ds_val, 1, target_size=VAL_SIZE[name], workers=workers),
                        validation_steps=val_size)
@@ -160,6 +170,12 @@ def main():
                         help="with --pytorch-checkpoint: RAFT's freeze_bn(), cnet's BatchNorm in eval mode")
     parser.add_argument('--gamma', type=float, default=None,
                         help='weight decay of the sequence loss over the iterations (default 0.8)')
+    parser.add_argument('--colour-jitter', choices=('albumentations', 'torchvision'), default='albumentations',
+                        help="colour augmentation: tf-raft's albumentations jitter, or the original RAFT's torchvision "
+                             "ColorJitter on PIL images (random order, contrast towards the mean grey)")
+    parser.add_argument('--add-noise', action='store_true',
+                        help="the original RAFT's --add_noise: Gaussian noise of a std drawn from U(0, 5) on both "
+                             "training images")
     args = parser.parse_args()
     if args.pytorch_checkpoint and (args.small or args.self_supervised):
         parser.error('--pytorch-checkpoint trains the basic RAFT with ground truth: not with --small or --self-supervised')
@@ -181,9 +197,11 @@ def main():
     if args.seed is not None:
         np.random.seed(args.seed)
         random.seed(args.seed)
+        if args.colour_jitter == 'torchvision' or args.add_noise:       # these draw from torch's CPU generator
+            torch.manual_seed(args.seed)
     train(args.dataset, config, logdir, small=args.small, workers=args.workers, self_supervised=args.self_supervised,
           train_precision=args.train_precision, pytorch_checkpoint=args.pytorch_checkpoint, freeze_bn=args.freeze_bn,
-          gamma=args.gamma)
+          gamma=args.gamma, colour_jitter=args.colour_jitter, add_noise=args.add_noise)
 
 
 if __name__ == '__main__':

@@ -8,6 +8,7 @@
 #include <algorithm>
 
 #include "augment.cuh"
+#include "colour.cuh"
 #include "conv_train.cuh"
 #include "corr_tc.cuh"
 #include "dataset.cuh"
@@ -645,6 +646,35 @@ int raft_b200_augment_dense(const raft_augment_sample* samples_host, const raft_
 int raft_b200_augment_sparse(const raft_augment_sample* samples_host, const raft_augment_sample* samples_dev, int B,
                              void* workspace, size_t workspace_bytes, void* stream) {
   return augment_run(samples_host, samples_dev, B, 1, workspace, workspace_bytes, stream);
+}
+
+int raft_b200_colour_jitter(const raft_colour_jitter_sample* samples_host, const raft_colour_jitter_sample* samples_dev,
+                            int B, unsigned long long* sums, void* stream) {
+  if (!samples_host || !samples_dev || !sums || reinterpret_cast<uintptr_t>(sums) % 8) return RAFT_ERR_BAD_ARG;
+  if (B < 1 || B > 65535) return RAFT_ERR_BAD_SHAPE;
+  int max_src = 1;
+  for (int b = 0; b < B; ++b) {
+    const raft_colour_jitter_sample& s = samples_host[b];
+    if (!s.img1 || !s.img2 || !s.out_img1 || !s.out_img2) return RAFT_ERR_BAD_ARG;
+    if (s.H < 1 || s.W < 1 || (size_t)s.H * s.W * 6 > (size_t)INT_MAX) return RAFT_ERR_BAD_SHAPE;
+    for (int k = 0; k < (s.stacked ? 1 : 2); ++k) {
+      unsigned seen = 0;
+      for (int q = 0; q < 4; ++q) {
+        const int op = s.order[k][q];
+        if (op < RAFT_JITTER_NONE || op > RAFT_JITTER_HUE || (op >= 0 && (seen >> op & 1u))) return RAFT_ERR_BAD_ARG;
+        if (op >= 0) seen |= 1u << op;
+      }
+      if (s.hue[k] < 0 || s.hue[k] > 255) return RAFT_ERR_BAD_ARG;
+      for (int q = 0; q < 3; ++q)
+        if (!(fabsf(s.factor[k][q]) <= FLT_MAX)) return RAFT_ERR_BAD_ARG;
+    }
+    max_src = std::max(max_src, 2 * s.H * s.W);
+  }
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const dim3 grid((unsigned)std::min(ceil_div(max_src, kJitterThreads), 4096), B);
+  RAFT_CUDA_TRY(cudaMemsetAsync(sums, 0, 2 * (size_t)B * sizeof(unsigned long long), st));
+  RAFT_TRY(launch(colour_jitter_sum_kernel, grid, kJitterThreads, 0, st, samples_dev, sums));
+  return launch(colour_jitter_apply_kernel, grid, kJitterThreads, 0, st, samples_dev, sums);
 }
 
 int raft_b200_flow_to_image(const float* u, const float* v, int stride, int B, int H, int W, int clip, float clip_flow,
