@@ -203,6 +203,41 @@ int raft_b200_coords_init(const float* flow_init, int B, int h, int w, float* co
 int raft_b200_fb_occlusion(const float* flow_fw, const float* flow_bw, int B, int H, int W, float alpha1, float alpha2,
                            uint8_t* occ_fw, uint8_t* occ_bw, void* stream);
 
+/* Flow warping and composition (additions beyond the reference; DESIGN.md section 3.9).  Both use
+ * raft_b200_fb_occlusion's conventions: flows (B, H, W, 2) float32, 8-byte aligned; pixel (x, y) lands at
+ * p = (x + fx, y + fy); p is inside a (Hs, Ws) grid iff 0 <= px <= Ws-1 and 0 <= py <= Hs-1 (NaN never is);
+ *   bilinear(T, p): x0 = floor(px), x1 = min(x0+1, Ws-1), ax = px - x0, bx = 1 - ax (y likewise),
+ *                   by*(bx*T[y0,x0] + ax*T[y0,x1]) + ay*(bx*T[y1,x0] + ax*T[y1,x1]);
+ *   nearest(p):     xi = min(floor(px + 0.5), Ws-1), yi = min(floor(py + 0.5), Hs-1).
+ * Every operation is one rounded fp32 operation in the order written, no FMA; a non-finite texel makes a bilinear
+ * sample non-finite even at weight 0.  Each call is one asynchronous launch with no allocation and no host
+ * synchronisation.                                                                                                   */
+typedef enum raft_warp_mode { RAFT_WARP_BILINEAR = 0, RAFT_WARP_NEAREST = 1 } raft_warp_mode;
+typedef enum raft_warp_dtype { RAFT_WARP_F32 = 0, RAFT_WARP_U8 = 1 } raft_warp_dtype;
+
+/* Backward warping: out[b,y,x,:] = sample of src[b] at the landing of flow[b,y,x] (bilinear or nearest, raft_warp_mode).
+ * src (B, Hs, Ws, C) of raft_warp_dtype (float32 4-byte aligned, or uint8 with RAFT_WARP_NEAREST only, which copies
+ * labels unchanged); flow (B, H, W, 2) sets the output grid: out is (B, H, W, C) of src's dtype.  The flow is in pixels
+ * of src and is not rescaled when (Hs, Ws) differs from (H, W).  Where the landing is outside src's frame or not
+ * finite, out is `fill` (for uint8 an integer 0..255) and occ[b,y,x] = 1; elsewhere occ is 0.  occ (B, H, W) uint8 may
+ * be NULL.  out and occ must not overlap each other, src or flow.  RAFT_ERR_BAD_ARG: NULL src / flow / out, unknown
+ * mode or dtype, uint8 with BILINEAR, a bad uint8 fill, misalignment or overlap; RAFT_ERR_BAD_SHAPE: a non-positive
+ * dimension, C outside 1..1024, or H*W*C or Hs*Ws*C above 2^31 - 1.                                                 */
+int raft_b200_warp(const void* src, int dtype, int Hs, int Ws, int C, const float* flow, int B, int H, int W, int mode,
+                   float fill, void* out, uint8_t* occ, void* stream);
+
+/* Flow composition, the chaining step of tracking.  With p the landing of f1 at pixel x of image b, on one (H, W) grid:
+ *   out(x)     = f1(x) + bilinear(f2[b], p)   (the sum one fp32 addition per component),
+ *   occ_out(x) = occ1(x) || !inside(p) || occ2[b](nearest(p)) || !finite(out(x)),
+ * and out(x) = f1(x) unchanged wherever occ_out(x) is set, so a lost track keeps its last position.  occ1, occ2,
+ * occ_out: (B, H, W) uint8, nonzero = no correspondence; occ1 and occ2 may be NULL (no mask).  out may be f1 itself and
+ * occ_out may be occ1 itself; any other overlap of an output with another buffer is RAFT_ERR_BAD_ARG, as are NULL
+ * f1 / f2 / out / occ_out and misaligned flows.  RAFT_ERR_BAD_SHAPE: a non-positive dimension or H*W above 2^31 - 1.
+ *   forward chaining  (frame 0 -> t): acc, lost = compose(acc, F_{t-1->t}, lost, occ_fw);
+ *   backward chaining (frame t -> 0): acc, lost = compose(B_{t->t-1}, acc, occ_bw, lost).                             */
+int raft_b200_compose_flow(const float* f1, const float* f2, const uint8_t* occ1, const uint8_t* occ2, int B, int H,
+                           int W, float* out, uint8_t* occ_out, void* stream);
+
 /* Self-supervised training (an addition beyond the reference; DESIGN.md section 9.1).
  *
  * raft_b200_census: images (B, H, W, 3) float32 in 0..255 -> out (B, H, W, 48) float32, 16-byte aligned.  With

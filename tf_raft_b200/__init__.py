@@ -11,6 +11,7 @@ from .layers.extractor import BasicEncoder, SmallEncoder
 from .layers.update import BasicUpdateBlock, SmallUpdateBlock
 from .losses import EndPointError, UnsupervisedLoss, end_point_error, sequence_loss
 from .model import RAFT, SmallRAFT
+from .warp import compose_flow, warp
 from .checkpoint import (load_pytorch_checkpoint, load_tf_checkpoint, param_to_tf_key, read_tf_checkpoint, tf_key_to_param,
                          to_pytorch_state_dict, write_tf_checkpoint)
 from .preprocess import CropOrPadder, InputPadder, pad_to_multiple, resize_with_crop_or_pad
@@ -22,7 +23,7 @@ from . import datasets
 from .submission import create_kitti_submission, create_sintel_submission
 
 __all__ = ['CorrBlock', 'bilinear_sampler', 'coords_grid', 'fb_occlusion', 'forward_interpolate', 'tfa_sampler', 'upflow8',
-           'BasicEncoder', 'SmallEncoder',
+           'warp', 'compose_flow', 'BasicEncoder', 'SmallEncoder',
            'BasicUpdateBlock', 'SmallUpdateBlock', 'RAFT', 'SmallRAFT', 'sequence_loss', 'end_point_error', 'UnsupervisedLoss',
            'resize_with_crop_or_pad', 'CropOrPadder', 'InputPadder', 'pad_to_multiple',
            'load_pytorch_checkpoint', 'load_tf_checkpoint', 'to_pytorch_state_dict', 'TorchAdamW', 'OneCycleLR',

@@ -73,6 +73,9 @@ CONVENTIONS = {'tf-raft': 0, 'pytorch': 1}
 SAMPLERS = {'tf-raft': 0, 'grid_sample': 1}
 # raft_adamw_rule: tfa AdamW after tf.clip_by_global_norm, or torch.optim.AdamW after clip_grad_norm_
 ADAMW_RULES = {'tfa': 0, 'torch': 1}
+# raft_warp_mode / raft_warp_dtype
+WARP_MODES = {'bilinear': 0, 'nearest': 1}
+WARP_F32, WARP_U8 = 0, 1
 
 _vp, _i, _sz = ctypes.c_void_p, ctypes.c_int, ctypes.c_size_t
 _SIGNATURES = {
@@ -100,6 +103,8 @@ _SIGNATURES = {
     'raft_b200_forward_interpolate': (_i, [_vp, _i, _i, _i, _vp, _vp]),
     'raft_b200_coords_init': (_i, [_vp, _i, _i, _i, _vp, _vp]),
     'raft_b200_fb_occlusion': (_i, [_vp, _vp, _i, _i, _i, ctypes.c_float, ctypes.c_float, _vp, _vp, _vp]),
+    'raft_b200_warp': (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _i, _i, ctypes.c_float, _vp, _vp, _vp]),
+    'raft_b200_compose_flow': (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp]),
     'raft_b200_census': (_i, [_vp, _i, _i, _i, _vp, _vp]),
     'raft_b200_unsup_loss': (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, ctypes.c_float, ctypes.c_float, ctypes.c_float,
                                   ctypes.c_float, _vp, _sz, _vp, _vp, _vp]),

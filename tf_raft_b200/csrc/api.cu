@@ -18,6 +18,7 @@
 #include "train.cuh"
 #include "unsup.cuh"
 #include "video.cuh"
+#include "warp.cuh"
 
 namespace raft {
 thread_local long long g_launches = 0;
@@ -529,6 +530,67 @@ int raft_b200_fb_occlusion(const float* flow_fw, const float* flow_bw, int B, in
   return launch(fb_occlusion_kernel, grid_for(2 * (size_t)B * H * W), 256, 0, reinterpret_cast<cudaStream_t>(stream),
                 reinterpret_cast<const float2*>(flow_fw), reinterpret_cast<const float2*>(flow_bw), B, H, W, alpha1, alpha2,
                 occ_fw, occ_bw);
+}
+
+// True when the byte ranges [a, a + na) and [b, b + nb) share a byte (a NULL range shares none).
+static bool overlap(const void* a, size_t na, const void* b, size_t nb) {
+  if (!a || !b) return false;
+  const uintptr_t x = reinterpret_cast<uintptr_t>(a), y = reinterpret_cast<uintptr_t>(b);
+  return x < y + nb && y < x + na;
+}
+
+int raft_b200_warp(const void* src, int dtype, int Hs, int Ws, int C, const float* flow, int B, int H, int W, int mode,
+                   float fill, void* out, uint8_t* occ, void* stream) {
+  if (!src || !flow || !out) return RAFT_ERR_BAD_ARG;
+  if (mode != RAFT_WARP_BILINEAR && mode != RAFT_WARP_NEAREST) return RAFT_ERR_BAD_ARG;
+  if (dtype != RAFT_WARP_F32 && dtype != RAFT_WARP_U8) return RAFT_ERR_BAD_ARG;
+  const bool u8 = dtype == RAFT_WARP_U8;
+  if (u8 && (mode != RAFT_WARP_NEAREST || !(fill >= 0.0f && fill <= 255.0f && fill == floorf(fill))))
+    return RAFT_ERR_BAD_ARG;
+  if (reinterpret_cast<uintptr_t>(flow) % sizeof(float2) ||
+      (!u8 && (reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(out)) % sizeof(float)))
+    return RAFT_ERR_BAD_ARG;
+  RAFT_TRY(check_dims(B, H, W));
+  RAFT_TRY(check_dims(1, Hs, Ws));
+  if (C < 1 || C > 1024) return RAFT_ERR_BAD_SHAPE;
+  if ((size_t)H * W * C > (size_t)INT_MAX || (size_t)Hs * Ws * C > (size_t)INT_MAX) return RAFT_ERR_BAD_SHAPE;
+  const size_t esz = u8 ? 1 : sizeof(float), npix = (size_t)B * H * W;
+  const size_t src_bytes = (size_t)B * Hs * Ws * C * esz, out_bytes = npix * C * esz, flow_bytes = npix * sizeof(float2);
+  if (overlap(out, out_bytes, src, src_bytes) || overlap(out, out_bytes, flow, flow_bytes) ||
+      overlap(occ, npix, src, src_bytes) || overlap(occ, npix, flow, flow_bytes) || overlap(occ, npix, out, out_bytes))
+    return RAFT_ERR_BAD_ARG;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const int grid = grid_for(npix * C);
+  const float2* f = reinterpret_cast<const float2*>(flow);
+  if (u8) {
+    const WarpParams<uint8_t> p{static_cast<const uint8_t*>(src), f, static_cast<uint8_t*>(out), occ, B, Hs, Ws, C, H, W,
+                                (uint8_t)fill};
+    return launch(warp_kernel<uint8_t, false>, grid, 256, 0, st, p);
+  }
+  const WarpParams<float> p{static_cast<const float*>(src), f, static_cast<float*>(out), occ, B, Hs, Ws, C, H, W, fill};
+  return mode == RAFT_WARP_BILINEAR ? launch(warp_kernel<float, true>, grid, 256, 0, st, p)
+                                    : launch(warp_kernel<float, false>, grid, 256, 0, st, p);
+}
+
+int raft_b200_compose_flow(const float* f1, const float* f2, const uint8_t* occ1, const uint8_t* occ2, int B, int H,
+                           int W, float* out, uint8_t* occ_out, void* stream) {
+  if (!f1 || !f2 || !out || !occ_out) return RAFT_ERR_BAD_ARG;
+  if ((reinterpret_cast<uintptr_t>(f1) | reinterpret_cast<uintptr_t>(f2) | reinterpret_cast<uintptr_t>(out)) %
+      sizeof(float2))
+    return RAFT_ERR_BAD_ARG;
+  RAFT_TRY(check_dims(B, H, W));
+  if ((size_t)H * W > (size_t)INT_MAX) return RAFT_ERR_BAD_SHAPE;
+  const size_t npix = (size_t)B * H * W, fb = npix * sizeof(float2);
+  // out may be f1 itself and occ_out occ1 itself (each thread reads them at its own pixel only); any other overlap
+  // between an output and a buffer the kernel reads or writes is refused.
+  if (overlap(out, fb, f2, fb) || (out != f1 && overlap(out, fb, f1, fb)) || overlap(out, fb, occ1, npix) ||
+      overlap(out, fb, occ2, npix) || overlap(out, fb, occ_out, npix) || overlap(occ_out, npix, f1, fb) ||
+      overlap(occ_out, npix, f2, fb) || overlap(occ_out, npix, occ2, npix) ||
+      (occ_out != occ1 && overlap(occ_out, npix, occ1, npix)))
+    return RAFT_ERR_BAD_ARG;
+  return launch(compose_flow_kernel, grid_for(npix), 256, 0, reinterpret_cast<cudaStream_t>(stream),
+                reinterpret_cast<const float2*>(f1), reinterpret_cast<const float2*>(f2), occ1, occ2, B, H, W,
+                reinterpret_cast<float2*>(out), occ_out);
 }
 
 int raft_b200_census(const float* images, int B, int H, int W, float* out, void* stream) {

@@ -21,6 +21,7 @@ from .layers.corr import CorrBlock, coords_grid, coords_init, fb_occlusion, forw
 from .layers.extractor import BasicEncoder, SmallEncoder
 from .layers.update import BasicUpdateBlock, SmallUpdateBlock
 from .losses import end_point_error, sequence_loss
+from .warp import compose_flow
 
 
 class RAFT:
@@ -475,6 +476,32 @@ class RAFT:
             frame_prev, fmap_prev = frame, fmap
             if bidirectional:
                 ctx_prev = ctx
+
+    def track_video(self, frames, *, direction='forward', warm_start=True):
+        """Long-range tracking along B video clips (an addition: tf-raft evaluates pairs only): the per-pair flows of
+        `predict_video(frames, warm_start=warm_start, bidirectional=True)` chained with `compose_flow`.
+
+        A generator: for t = 1 .. T-1 it yields (flow, occ), a (B, H, W, 2) flow and a torch.bool (B, H, W) mask.
+          direction='forward':  flow(x) is the displacement of pixel x of frame 0 to frame t.  The first yield is
+                                (F_{0->1}, occ_fw) of the pair (0, 1); then acc, lost = compose_flow(acc, F_{t-1->t},
+                                lost, occ_fw).
+          direction='backward': flow(x) is the displacement of pixel x of frame t back to frame 0, so
+                                `warp(labels_0, flow, mode='nearest')` carries frame 0's labels to frame t.  The first
+                                yield is (B_{1->0}, occ_bw); then acc, lost = compose_flow(B_{t->t-1}, acc, occ_bw, lost).
+        occ is True where the track is lost: a pixel that was occluded or left the frame once stays lost, and its
+        flow keeps its last value.  Batches, shape checks, `iters_pred >= 1` and eager-only behaviour are
+        `predict_video`'s; every yielded tensor is a new one."""
+        if direction not in ('forward', 'backward'):
+            raise ValueError(f"direction must be 'forward' or 'backward', got {direction!r}")
+        acc = lost = None
+        for flow_fw, flow_bw, occ_fw, occ_bw in self.predict_video(frames, warm_start=warm_start, bidirectional=True):
+            if acc is None:
+                acc, lost = (flow_fw, occ_fw) if direction == 'forward' else (flow_bw, occ_bw)
+            elif direction == 'forward':
+                acc, lost = compose_flow(acc, flow_fw, lost, occ_fw)
+            else:
+                acc, lost = compose_flow(flow_bw, acc, occ_bw, lost)
+            yield acc, lost
 
     call = __call__
 
